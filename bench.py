@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py - KITTI-shape frames/s of the Point-GNN message-passing hot path on B200.
+"""bench.py - KITTI-shape frames/s of the Point-GNN message-passing hot path on H100.
 
     python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload NAME] [--precision P]
+                    [--dump-outputs DIR]
 
 A *step* is one pass of the hot path (GPU graph construction + car_auto_T3 forward, real
 trained weights) over one batch of synthetic 20k-point KITTI-crop frames per GPU.  One JSON line is
@@ -14,6 +15,9 @@ roofline   dominant kernel = the fused edge-MLP/segment-max kernel of the GNN it
            with CUDA events; achieved = algorithmic FLOPs (E1 * 361 800 per launch, SURVEY 8d) / time
 cpu_baseline  the CPU oracle (a port: TF-1.15 cannot be installed) on one frame of the same workload
 --impl reference   times that CPU port alone, all host threads, one frame per step
+--dump-outputs DIR  after the timed steps, rank 0 writes what the last timed step computed (class probabilities,
+                    box encodings, keypoint indices, both edge lists) as DIR/<name>.npy; the inputs depend only on
+                    the arguments, so two builds can be compared output for output
 """
 import argparse
 import json
@@ -39,29 +43,22 @@ WORKLOADS = {
 METRIC = 'KITTI-shape frames/sec (car_auto_T3, graph build + GNN forward)'
 UNIT = 'frames/s'
 FRAME_POOL = 6     # distinct step inputs the timed loop cycles through (L2 is flushed between steps)
-# `ncu --set full` summaries of the dominant kernel, newest first (tools/ncu_summary.py output, committed under
-# profiles/): roofline.traffic = dram__bytes_read.sum + dram__bytes_write.sum of one launch is parsed from the first
-# one that exists - a measurement taken under the profiler at the default workload, named in the JSON line
-NCU_SUMMARIES = ('profiles/r2_seg_tc_ncu_summary.txt', 'profiles/r1_seg_tc_ncu_summary.txt')
+DUMP_BYTES = 64 << 20   # cap of --dump-outputs; larger arrays are written as a fixed, seeded row sample
 
 
-def edge_kernel_dram_traffic():
-    """-> (bytes per launch or None, file it came from)."""
-    for rel in NCU_SUMMARIES:
-        path = os.path.join(ROOT, rel)
-        if not os.path.isfile(path):
-            continue
-        total, seen = 0.0, 0
-        scale = {'byte': 1.0, 'Kbyte': 1e3, 'Mbyte': 1e6, 'Gbyte': 1e9}
-        with open(path) as f:
-            for line in f:
-                parts = line.split()
-                if len(parts) >= 3 and parts[0] in ('dram__bytes_read.sum', 'dram__bytes_write.sum') and parts[1] in scale:
-                    total += float(parts[2]) * scale[parts[1]]
-                    seen += 1
-        if seen == 2:
-            return total, rel
-    return None, None
+def dump_outputs(out_dir, arrays):
+    """Write {name: array} as out_dir/<name>.npy (float32 / float64).  An array whose share of DUMP_BYTES is
+    exceeded is replaced by the rows at a fixed seeded sample of indices (written beside it as <name>_rows.npy)."""
+    os.makedirs(out_dir, exist_ok=True)
+    share = DUMP_BYTES // (2 * len(arrays))
+    rng = np.random.default_rng(0)
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(a)
+        if a.nbytes > share:
+            rows = np.sort(rng.choice(a.shape[0], max(1, share // max(1, a.nbytes // a.shape[0])), replace=False))
+            np.save(os.path.join(out_dir, name + '_rows.npy'), rows.astype(np.float64))
+            a = a[rows]
+        np.save(os.path.join(out_dir, name + '.npy'), a)
 
 
 def load_config(name):
@@ -280,7 +277,7 @@ def run_gpu(args, rank, world):
         host_steps.append((torch.from_numpy(np.vstack(pts)).pin_memory(), torch.from_numpy(np.vstack(inten)).pin_memory(),
                            torch.from_numpy(fp).pin_memory()))
     dev_steps = [(a.to(dev), b.to(dev), c.to(dev)) for a, b, c in host_steps]
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > 50 MB L2
 
     stage_ms = {'gen graph': 0.0, 'gnn inference': 0.0, 'edge kernel': 0.0}
     counters = {'edges1': 0, 'edges0': 0, 'keypoints': 0, 'edge_launches': 0}
@@ -299,7 +296,7 @@ def run_gpu(args, rank, world):
             torch.cuda.synchronize()
             stage_ms['gen graph'] += ev[0].elapsed_time(ev[1])
             stage_ms['gnn inference'] += ev[1].elapsed_time(ev[2])
-        return probs, boxes, kp[0].shape[0], edges[0].shape[0], edges[1].shape[0]
+        return probs, boxes, kp[0].shape[0], edges[0].shape[0], edges[1].shape[0], (kp, edges)
 
     # end-to-end arm: pinned host buffers on both sides (inputs above; outputs here, sized for the worst case of
     # one keypoint per point), asynchronous copies on the compute stream, ONE synchronisation per step
@@ -311,7 +308,7 @@ def run_gpu(args, rank, world):
         xyz = hx.to(dev, non_blocking=True)
         inten = hi.to(dev, non_blocking=True)
         fp = hfp.to(dev, non_blocking=True)
-        probs, boxes, k, e0, e1 = step_device(xyz, inten, fp)
+        probs, boxes, k, e0, e1, _ = step_device(xyz, inten, fp)
         hp, hb = out_probs[:k], out_boxes[:k]
         hp.copy_(probs, non_blocking=True)
         hb.copy_(boxes, non_blocking=True)
@@ -370,7 +367,7 @@ def run_gpu(args, rank, world):
         a = torch.cuda.Event(enable_timing=True)
         b = torch.cuda.Event(enable_timing=True)
         a.record()
-        probs, boxes, k, e0, e1 = step_device(*dev_steps[(args.warmup + s) % pool])
+        probs, boxes, k, e0, e1, graph = step_device(*dev_steps[(args.warmup + s) % pool])
         b.record()
         b.synchronize()
         elapsed_ms += a.elapsed_time(b)
@@ -381,6 +378,13 @@ def run_gpu(args, rank, world):
     barrier()
     t_wall1 = time.perf_counter()
     launches = _lib.launch_count() - launches0
+    if args.dump_outputs and rank == 0 and args.steps > 0:
+        kp_last, edges_last = graph
+        dump_outputs(args.dump_outputs, {
+            'probs': probs.float().cpu().numpy(), 'boxes': boxes.float().cpu().numpy(),
+            'keypoint_indices': kp_last[0].cpu().numpy().astype(np.float64).reshape(-1),
+            'edges0': edges_last[0].cpu().numpy().astype(np.float64),
+            'edges1': edges_last[1].cpu().numpy().astype(np.float64)})
 
     # ---- timed: end to end through the public API with host buffers ---------------------------
     barrier()
@@ -431,11 +435,11 @@ def run_gpu(args, rank, world):
         except OSError:
             pass
         # the kernel is timed in isolation (a handful of back-to-back launches): the BURST peak is the denominator
-        peak_tf = peaks.get('bf16_tflops', 1590.0)
-        peak_src = 'measured (MEASURED_PEAKS.json bf16_tflops, burst)' if peaks else 'fallback 1.59 PFLOP/s burst'
-        traffic, traffic_src = edge_kernel_dram_traffic()
-        hbm = peaks.get('hbm_gbs', 6650.0)
-        hbm_src = 'measured (MEASURED_PEAKS.json hbm_gbs)' if peaks else 'fallback 6.65 TB/s'
+        peak_tf = peaks.get('bf16_tflops', 989.0)
+        peak_src = ('measured (MEASURED_PEAKS.json bf16_tflops, burst)' if peaks else
+                    'H100 SXM data sheet, 989 TFLOP/s dense BF16 at 700 W (not reached under a lower power limit)')
+        hbm = peaks.get('hbm_gbs', 3350.0)
+        hbm_src = 'measured (MEASURED_PEAKS.json hbm_gbs)' if peaks else 'H100 SXM data sheet, 3.35 TB/s HBM3'
         achieved = edge_flops / (edge_ms * 1e-3) / 1e12 if edge_ms > 0 else 0.0
         k_avg = counters['keypoints'] / args.steps / frames_per_step
         e0_avg = counters['edges0'] / args.steps / frames_per_step
@@ -471,11 +475,11 @@ def run_gpu(args, rank, world):
             'gpu_launches': launches,
             'clocks': clocks,
             'stages_ms_per_step': {k: v / n_instr for k, v in stage_ms.items() if k != 'edge kernel'},
-            'roofline': {'bound': 'tensor', 'kernel': 'seg_gemm_tc_kernel (fused GNN edge layer: gather + edge MLP + '
-                                                      'segment max; timed as the prepared pg_layer_edge_mlp_max call = '
-                                                      'hoisted per-vertex GEMM + output fill + the fused kernel)',
+            'roofline': {'bound': 'tensor', 'kernel': 'wg_gemm_kernel<PROD_GNN, EPI_SEGMAX> (fused GNN edge layer: gather + '
+                                                      'edge MLP + segment max; timed as the prepared pg_layer_edge_mlp_max '
+                                                      'call = hoisted per-vertex GEMM + output fill + the fused kernel)',
                          'achieved': achieved, 'peak': peak_tf, 'unit': 'TFLOP/s', 'frac': achieved / peak_tf,
-                         'traffic': traffic, 'traffic_source': traffic_src, 'peak_source': peak_src,
+                         'traffic': None, 'peak_source': peak_src,
                          'launch_ms': edge_ms / max(edge_launches, 1),
                          'algorithmic_flops_per_launch': edge_flops / max(edge_launches, 1),
                          # the kernel executes 3 BF16 MMAs per product (BF16x3 split) on the padded 304x304 second
@@ -585,6 +589,7 @@ def main():
     ap.add_argument('--precision', default=None, choices=['fp32', 'bf16x3'])
     ap.add_argument('--frames-per-step', type=int, default=0)
     ap.add_argument('--no-cpu-baseline', action='store_true')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR')
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == 'ours' else args.warmup
     rank = int(os.environ.get('RANK', 0))

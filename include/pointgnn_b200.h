@@ -1,7 +1,7 @@
 /*
  * pointgnn_b200.h - C ABI of libpointgnn_b200.so
  *
- * B200 (sm_100a) implementation of Point-GNN's per-frame message-passing hot
+ * H100 (sm_90a) implementation of Point-GNN's per-frame message-passing hot
  * path.  Every entry point replaces one piece of the reference's Python/TF path;
  * the reference interface each one stands in for is cited as
  * /root/reference/<file>:<line>.
@@ -46,9 +46,9 @@ extern "C" {
 PG_API int pg_version(void);
 /* Message of the last error on this thread ("" if none). */
 PG_API const char* pg_last_error(void);
-/* 1 if the visible device is sm_100 (B200); the tcgen05 kernels require it. */
-PG_API int pg_device_is_sm100(void);
-/* 1 if the tcgen05 (precision = 1) kernels are built in AND the device can run them. */
+/* 1 if the visible device is sm_90 (H100); the wgmma kernels require it. */
+PG_API int pg_device_is_sm90(void);
+/* 1 if the wgmma (precision = 1) kernels are built in AND the device can run them. */
 PG_API int pg_tc_available(void);
 
 /* ------------------------------------------------------------------------ *
@@ -277,7 +277,7 @@ PG_API int pg_gather_rows(const float* params, int64_t num_rows, int32_t num_cha
  * One slim.fully_connected layer (gnn.py:63-80,93-103), normalizer NONE:
  *   out[M,N] = act(x[M,K] @ w[K,N] + bias[N]) (+ residual[M,N] if not NULL)
  * act: 0 = linear (the is_logits last layer), 1 = ReLU.
- * precision: 0 = fp32 FFMA, 1 = tcgen05 BF16x3 split (fp32-class accuracy).
+ * precision: 0 = fp32 FFMA, 1 = wgmma BF16x3 split (fp32-class accuracy).
  */
 PG_API int pg_fully_connected(const float* x, int64_t m, int32_t k, const float* w, const float* bias,
                        int32_t n, int32_t act, const float* residual, float* out,
@@ -304,7 +304,7 @@ PG_API int pg_fully_connected(const float* x, int64_t m, int32_t k, const float*
  *                W_l is [dims[l], dims[l+1]] row-major, dims[0] = C_in + 3.
  *   dims_host    (host) [num_layers+1]
  *   out          [num_dst, dims[num_layers]]; empty segments get -FLT_MAX.
- *   precision    0 = fp32 FFMA, 1 = tcgen05 BF16x3 for the wide layers; may be OR-ed with
+ *   precision    0 = fp32 FFMA, 1 = wgmma BF16x3 for the wide layers; may be OR-ed with
  *                PG_FLAG_TRUSTED_INDICES: the caller guarantees src / dst are in range (they come from
  *                pg_radius_graph, or passed pg_check_edges), so the call skips the device->host
  *                read-back of the range-error flag and does not synchronise the stream.  Out-of-range
@@ -349,7 +349,7 @@ PG_API int pg_check_edges(const int32_t* src, const int32_t* dst, int64_t num_ed
  *                            reference creates them: cls fc (D->H), cls fc_1 (H->C), then
  *                            for every class c: loc fc (D->H), fc_1 (H->H), fc_2 (H->box_len);
  *                            num_layers = 2 + 3 C.
- *   precision 0 = fp32 FFMA, 1 = tcgen05 BF16x3 wherever the shapes allow.
+ *   precision 0 = fp32 FFMA, 1 = wgmma BF16x3 wherever the shapes allow.
  * ------------------------------------------------------------------------ */
 typedef struct pg_layer pg_layer;
 #define PG_LAYER_MLP 0
@@ -436,7 +436,8 @@ PG_API int pg_nms_boxes_3d(const int32_t* class_labels, const float* boxes, cons
                     float* out_box, float* out_score, int32_t* out_index, int64_t capacity,
                     int32_t* out_det_frame_ptr, int64_t* out_sizes_host, void* stream);
 
-/* tcgen05 kernel launches so far (which: 0 = fused edge MLP + segment max, 1 = dense layer);
+/* wgmma kernel launches so far (which: 0 = segment-max launches of the edge layers, 1 = store launches:
+ * dense layers and the stored per-edge layers of point-set pooling);
  * lets callers and tests verify that the tensor-core path, not the FFMA path, actually ran. */
 PG_API int64_t pg_tc_launch_count(int32_t which);
 

@@ -24,7 +24,7 @@ c_i32 = ctypes.c_int32
 SIGNATURES = {
     'pg_version': (ctypes.c_int, []),
     'pg_last_error': (ctypes.c_char_p, []),
-    'pg_device_is_sm100': (ctypes.c_int, []),
+    'pg_device_is_sm90': (ctypes.c_int, []),
     'pg_launch_count': (c_i64, []),
     'pg_tc_available': (ctypes.c_int, []),
     'pg_tc_launch_count': (c_i64, [c_i32]),
@@ -147,17 +147,17 @@ def launch_count():
     return int(load().pg_launch_count())
 
 
-def device_is_sm100():
-    return bool(load().pg_device_is_sm100())
+def device_is_sm90():
+    return bool(load().pg_device_is_sm90())
 
 
 def tc_launch_count(which=0):
-    """tcgen05 launches so far: which=0 fused edge kernel, 1 dense-layer kernel."""
+    """tensor-core launches so far: which=0 segment-max (edge layer) launches, 1 dense-layer launches."""
     return int(load().pg_tc_launch_count(int(which)))
 
 
 def tc_available():
-    """True when the tcgen05 (precision=1) kernels are compiled in and the device is sm_100."""
+    """True when the wgmma (precision=1) kernels are compiled in and the device is sm_90."""
     return bool(load().pg_tc_available())
 
 

@@ -27,11 +27,11 @@ int pg_version(void) { return 1; }
 
 const char* pg_last_error(void) { return pg::g_error; }
 
-int pg_device_is_sm100(void) {
+int pg_device_is_sm90(void) {
   int dev = 0, major = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return 0;
   if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
-  return major == 10 ? 1 : 0;
+  return major == 9 ? 1 : 0;
 }
 
 int64_t pg_launch_count(void) { return pg::g_launches.load(std::memory_order_relaxed); }

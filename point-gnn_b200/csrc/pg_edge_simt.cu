@@ -11,7 +11,7 @@
 // tile per destination before touching HBM: because edges are grouped by destination, each
 // column thread walks the 64 rows keeping a running max and issues one atomic per (segment,
 // tile, column).  This is the bit-faithful baseline (same fp32 association order as a CPU loop);
-// the tcgen05 version in pg_tc.cu is the fast path.
+// the wgmma version in pg_tc.cu is the fast path.
 #include "pg_common.cuh"
 
 namespace pg {

@@ -1,5 +1,5 @@
 """GNN layers and ops - same classes / functions / argument lists as the reference's
-``models/gnn.py`` (/root/reference/models/gnn.py), executing on hand-written sm_100a kernels.
+``models/gnn.py`` (/root/reference/models/gnn.py), executing on hand-written sm_90a kernels.
 
 The reference builds a TF-1 graph whose variables are created by ``slim.fully_connected``
 inside nested ``tf.variable_scope``s; here the same scoping is reproduced eagerly so that the

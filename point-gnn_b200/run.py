@@ -113,7 +113,7 @@ def write_kitti_file(filename, pred_labels):
 
 
 def main(argv=None):
-    parser = argparse.ArgumentParser(description='Point-GNN inference on KITTI (B200-native twin of run.py)')
+    parser = argparse.ArgumentParser(description='Point-GNN inference on KITTI (H100 twin of run.py)')
     parser.add_argument('checkpoint_path', type=str, help='Path to checkpoint')
     parser.add_argument('-l', '--level', type=int, default=0, help='Visualization level: only 0 (disabled) is built')
     parser.add_argument('--test', dest='test', action='store_true', default=False, help='Enable test model')
@@ -128,7 +128,7 @@ def main(argv=None):
     parser.add_argument('--output_dir', type=str, default='',
                         help='Path to save the detection results. Default="CHECKPOINT_PATH/eval/"')
     parser.add_argument('--precision', type=str, default=None, choices=['fp32', 'bf16x3'],
-                        help='Arithmetic of the dense layers (default: bf16x3 on sm_100, fp32-class accuracy)')
+                        help='Arithmetic of the dense layers (default: bf16x3 on sm_90, fp32-class accuracy)')
     args = parser.parse_args(argv)
     if args.level != 0:
         raise NotImplementedError('visualisation levels 1 / 2 (Open3D windows) are not built')

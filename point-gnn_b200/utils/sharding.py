@@ -7,7 +7,7 @@ same single-GPU path on its own frames, and the ONLY collective is an all-gather
 per-rank counters at the end (``gather_counters``): frames, device milliseconds, edges,
 keypoints.  No feature / gradient / graph data ever crosses NVLink.
 
-Backend-agnostic on purpose: ``nccl`` on the B200 box, ``gloo`` in the CPU tests
+Backend-agnostic on purpose: ``nccl`` on the GPU machines, ``gloo`` in the CPU tests
 (tests/test_sharding_cpu.py runs it with world_size 2).
 """
 import torch

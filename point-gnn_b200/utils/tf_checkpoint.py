@@ -114,7 +114,8 @@ def read_index(index_path):
                 shape=_parse_shape(p[2][0]) if 2 in p else (),
                 shard=p.get(3, [0])[0],
                 offset=p.get(4, [0])[0],
-                size=p.get(5, [0])[0])
+                size=p.get(5, [0])[0],
+                crc32c=p.get(6, [None])[0])         # masked CRC32C of the tensor's bytes
     return entries
 
 

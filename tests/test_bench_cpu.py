@@ -46,7 +46,8 @@ def test_reference_arm_rank_nonzero_is_silent():
 
 
 def test_committed_bench_line_has_the_contract_keys():
-    path = os.path.join(ROOT, 'profiles', 'r1_bench_line.json')
+    """A line bench.py printed on one H100 80GB HBM3 (700 W power limit), default workload."""
+    path = os.path.join(ROOT, 'tests', 'golden', 'bench_line.json')
     line = [l for l in open(path).read().splitlines() if l.startswith('{')][-1]
     d = json.loads(line)
     for key in ('metric', 'value', 'unit', 'n_gpus', 'steps', 'warmup', 'ms_per_step', 'higher_is_better', 'scaling',

@@ -2,7 +2,7 @@
 Python layer API) vs the fp32 CPU oracle, with the reference's trained weights.
 
 Tolerance (BASELINE.json north_star): vertex features / logits / box encodings within 1e-3
-absolute of the fp32 CPU path.  The fp32 FFMA kernels are expected ~1e-5; the tcgen05 BF16x3
+absolute of the fp32 CPU path.  The fp32 FFMA kernels are expected ~1e-5; the wgmma BF16x3
 kernels ~1e-4 (three-term split, see DESIGN.md)."""
 import numpy as np
 import pytest
@@ -21,7 +21,7 @@ PRECISIONS = ['fp32', 'bf16x3']
 def _need(precision):
     from pointgnn_b200 import _lib
     if precision == 'bf16x3' and not _lib.tc_available():
-        pytest.skip('tcgen05 path needs an sm_100 device')
+        pytest.skip('tensor-core path needs an sm_90 device')
 
 
 def _cuda(a, dtype=None):
@@ -53,7 +53,7 @@ def test_scatter_max_vs_oracle():
 def test_fully_connected_vs_oracle(precision):
     """pg_fully_connected alone (NumPy fp32 as the checker): odd shapes, row tails (m % 256 != 0), K not a
     multiple of 16, N < 8 heads, bias / ReLU / residual combinations - for the FFMA kernel and for the
-    tcgen05 BF16x3 dense kernel (which must really run for the wide shapes)."""
+    wgmma BF16x3 dense kernel (which must really run for the wide shapes)."""
     _need(precision)
     import pointgnn_b200
     from pointgnn_b200 import _lib
@@ -79,8 +79,8 @@ def test_fully_connected_vs_oracle(precision):
                 assert got.shape == want.shape and np.abs(got - want).max() < tol, (m, k, n, relu)
     if precision == 'bf16x3':
         # (257,300,300), (255,256,256), (256,300,64), (33,128,300) x 4 bias/residual combinations; the others are
-        # K % 4 != 0, K < 64 or N < 8 and take the FFMA kernel; (130,512,256) and (700,512,300) exceed one resident
-        # weight image and run as two column blocks (2 launches per call)
+        # K % 4 != 0, K < 64 or N < 8 and take the FFMA kernel; (130,512,256), (700,512,300) add one launch per
+        # call and (4099,300,320) is wider than one launch covers and runs as two column blocks
         assert _lib.tc_launch_count(1) - dense0 >= 4 * 4 + 2 * 4 * 2
     pointgnn_b200.set_precision('fp32')
 
@@ -193,9 +193,9 @@ def test_predict_matches_golden(name, precision, request):
     logits, boxes, probs = _predict(g, g.layer_configs, precision, (g.graph['intensity'], coords, keypoints, edges))
     if precision == 'bf16x3':
         # the tensor-core kernels must really have run: 3 GNN iterations (+ the car pooling layer) are
-        # fused tcgen05 edge launches, and the wide per-vertex layers go through the dense tcgen05
-        # kernel (no silent FFMA fallback).  The ped pooling MLP (4 -> 32 -> 64 -> 128 -> 256 -> 512) is two
-        # launches: the chain kernel up to 256 (store mode) + pool_last_tc_kernel (256 -> 512 + segment max).
+        # segment-max tensor-core launches, and the wide per-vertex layers go through the dense tensor-core
+        # kernel (no silent FFMA fallback).  The ped pooling MLP (4 -> 32 -> 64 -> 128 -> 256 -> 512) ends in two
+        # segment-max launches: its last layer (256 -> 512) runs as two column blocks of 256.
         assert _lib.tc_launch_count(0) - tc0[0] == (4 if name == 'car' else 5)
         assert _lib.tc_launch_count(1) - tc0[1] >= 10
     assert isinstance(logits, np.ndarray) and logits.shape == g.gnn['logits'].shape
@@ -413,7 +413,7 @@ def test_index_contract_of_predict(car):
 
 @pytest.mark.parametrize('d,c_in', [(300, 300), (256, 256), (64, 32), (128, 300)])
 def test_tc_edge_kernel_shapes_and_tails(d, c_in):
-    """The tcgen05 edge kernel on its own: odd widths, tails, tiny / huge / empty segments."""
+    """The tensor-core edge kernel on its own: odd widths, tails, tiny / huge / empty segments."""
     _need('bf16x3')
     from pointgnn_b200 import _lib
     rng = np.random.default_rng(d)
@@ -454,14 +454,14 @@ def test_tc_edge_kernel_shapes_and_tails(d, c_in):
 @pytest.mark.parametrize('dims', [(4, 32, 64, 128, 300), (4, 32, 64, 128, 256, 512), (4, 32, 64, 128, 256, 300),
                                   (4, 16, 64, 200), (4, 32, 128, 64)])
 def test_tc_pool_chain_shapes_and_tails(dims):
-    """The point-set pooling MLP on tensor cores: the full chain kernel (car shape), the chain in store mode +
-    pool_last_tc_kernel (ped shape 256 -> 512, and a last layer that only half fills its second 256-feature
-    block), tails, one-edge / tile-spanning / empty segments, keypoint indirection."""
+    """The point-set pooling MLP on tensor cores: per-edge layers in store mode, then the segment-max layer (car
+    shape; ped shape 256 -> 512 as two column blocks; a last layer of 300 in one block), tails, one-edge /
+    tile-spanning / empty segments, keypoint indirection."""
     _need('bf16x3')
     from pointgnn_b200 import _lib
     rng = np.random.default_rng(sum(dims))
     nv, nk = 900, 400
-    launches = 2 if (len(dims) == 6) else 1
+    launches = -(-dims[-1] // 304)           # one segment-max launch per column block of at most 304 features
     ws = [(rng.standard_normal((dims[i], dims[i + 1])) / np.sqrt(dims[i])).astype(np.float32) for i in range(len(dims) - 1)]
     bs = [(rng.standard_normal(dims[i + 1]) * 0.1).astype(np.float32) for i in range(len(dims) - 1)]
     for case, (e, pattern) in enumerate(((1, 'one'), (255, 'long'), (256, 'long'), (257, 'short'), (5000, 'mixed'),

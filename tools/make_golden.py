@@ -13,11 +13,15 @@
   frame with the real weights -> pins oracle/gnn.py and the CUDA kernels to the graph the
   reference built (op order, concat order, gather indices, segment ids), for all seven shipped
   checkpoints.  The script asserts that oracle/gnn.py reproduces those vectors to <= 1e-5.
+* graph_live_reference.npz : the reference's radius graphs on a second seeded frame (two voxel / radius settings).
+* checkpoints/<cfg>/ : index and state file of each shipped checkpoint (+ two gzipped saved graphs), from which
+  oracle/checkpoint_fixture.py rebuilds the checkpoints with the weights above.
 """
 import glob
 import json
 import os
 import sys
+import tempfile
 
 import numpy as np
 
@@ -331,6 +335,47 @@ def graph_rnd3d_goldens():
     np.savez_compressed(os.path.join(GOLDEN, 'graph_rnd3d.npz'), **out)
 
 
+def graph_live_reference_goldens():
+    """graph_live_reference.npz: the REFERENCE's gen_disjointed_rnn_local_graph_v3 (canonical edge order) on a seeded
+    2 500-point frame, for the oracle's keypoints at two voxel / radius settings (both graph levels each)."""
+    ref = reference_graph.load()
+    xyz, _ = synth.lidar_frame(11, 2500)
+    out = {}
+    for i, (voxel, r0, r1) in enumerate(((0.4, 1.0, 4.0), (0.2, 0.4, 1.6))):
+        kxyz = xyz[graph.nearest_point(xyz, graph.voxel_down_sample(xyz, voxel))]
+        for lvl, (pts, ctr, r) in enumerate(((xyz, kxyz, r0), (kxyz, kxyz, r1))):
+            e = graph.canonical_edges(ref.gen_disjointed_rnn_local_graph_v3(pts, ctr, r, -1))
+            out['edges_%d_%d' % (i, lvl)] = e.astype(np.int32)
+    np.savez_compressed(os.path.join(GOLDEN, 'graph_live_reference.npz'), **out)
+    print('graph_live_reference:', {k: v.shape for k, v in out.items()})
+
+
+def checkpoint_fixtures():
+    """checkpoints/<cfg>/: the reference's `checkpoint` state file and model-N.index of every shipped checkpoint, and
+    the gzipped model-N.meta of the two the saved-graph test re-interprets.  The tensor bytes are not stored: the
+    data file is rebuilt from weights_<cfg>.npz (oracle/checkpoint_fixture.py), checked against the index's CRC32C."""
+    import gzip
+    import shutil
+    from oracle import checkpoint_fixture
+    root = os.path.join(reference_graph.REFERENCE_ROOT, 'checkpoints')
+    for name in sorted(os.listdir(root)):
+        dst = os.path.join(checkpoint_fixture.FIXTURES, name)
+        os.makedirs(dst, exist_ok=True)
+        for f in os.listdir(os.path.join(root, name)):
+            path = os.path.join(root, name, f)
+            if f == 'checkpoint' or f.endswith('.index'):
+                shutil.copy(path, dst)
+            elif f.endswith('.meta') and name in ('car_auto_T1_train', 'car_fixed_T3_train'):
+                with open(path, 'rb') as i, gzip.GzipFile(os.path.join(dst, f + '.gz'), 'wb', mtime=0) as o:
+                    o.write(i.read())
+        tmp = tempfile.mkdtemp()
+        try:
+            checkpoint_fixture.rebuild(name, tmp)        # raises unless every tensor matches the index's CRC32C
+        finally:
+            shutil.rmtree(tmp)
+        print('checkpoint fixture', name)
+
+
 if __name__ == '__main__':
     which = sys.argv[1] if len(sys.argv) > 1 else 'all'
     if which in ('all', 'graph_random'):
@@ -347,3 +392,7 @@ if __name__ == '__main__':
         post_goldens()
     if which in ('all', 'kitti'):
         kitti_goldens()
+    if which in ('all', 'graph_live_reference'):
+        graph_live_reference_goldens()
+    if which in ('all', 'checkpoints'):
+        checkpoint_fixtures()

@@ -17,7 +17,7 @@ from pointgnn_b200.models import graph_gen  # noqa: E402
 frames = int(sys.argv[1]) if len(sys.argv) > 1 else 8
 reps = int(sys.argv[2]) if len(sys.argv) > 2 else 3
 prec = int(sys.argv[3]) if len(sys.argv) > 3 else 1
-name = sys.argv[4] if len(sys.argv) > 4 else 'car_auto_T3_train'       # or ped_cyl_auto_T3_trainval (chain store mode + pool_last)
+name = sys.argv[4] if len(sys.argv) > 4 else 'car_auto_T3_train'       # or ped_cyl_auto_T3_trainval (last layer 256 -> 512 in two column blocks)
 cfg = json.load(open(os.path.join(ROOT, 'tests/golden/config_%s.json' % name)))
 w = dict(np.load(os.path.join(ROOT, 'tests/golden/weights_%s.npz' % name)))
 fr = [synth.lidar_frame(i, 20000) for i in range(frames)]
