@@ -83,18 +83,30 @@ __global__ void frame_min_kernel(const float* __restrict__ xyz, const int32_t* _
   }
 }
 
+// How a point's cell index follows from its coordinates and the bounding-box minimum of its frame.
+enum class CellRule : int {
+  // open3d.voxel_down_sample (graph_gen.py:41-45): origin = frame_min - cell / 2, floor((p - origin) / cell) in fp64
+  kVoxel,
+  // radius and nearest-vertex search grids: origin = frame_min, floor((p - origin) / cell) in fp64 on the coordinates
+  // divided by `scale` if `scaled`
+  kRadius,
+  // multi_layer_downsampling_random without add_rnd3d (graph_gen.py:124-126): floor_divide(p - frame_min, cell) in
+  // float32
+  kNumpyF32,
+  // add_rnd3d (graph_gen.py:24-31, 127-130): floor_divide((p - frame_min)[float32] + cell * shift[frame], cell) in
+  // float64, shift = the np.random.random((1, 3)) draw of the frame
+  kNumpyF64Shift,
+};
+
 // Grid description shared by key generation and queries.
 struct GridSpec {
   double cell[3];     // cell edge per axis
-  double origin_off;  // origin = frame_min - cell * origin_off   (0.5 for Open3D voxels, 0 for radius grids)
+  CellRule rule;
   // gen_disjointed_rnn_local_graph_v3's `scale` (graph_gen.py:203-206): every coordinate is DIVIDED by scale[axis] in
   // float64 before anything else (points_xyz / np.array(scale) -> float64).  scaled == 0: coordinates as they are.
   int scaled;
   double scale[3];
-  // multi_layer_downsampling with add_rnd3d (graph_gen.py:24-31): cell = floor_divide((p - frame_min)[float32] +
-  // cell * shift[frame], cell) in float64, shift = the np.random.random((1, 3)) draw of the frame.  shift == nullptr:
-  // the rule of cell_of below.
-  const double* shift;
+  const double* shift;   // kNumpyF64Shift: [num_frames][3] on the device
 };
 
 // coordinate of axis a as the reference sees it: float32 value -> float64, divided by the scale if there is one
@@ -102,19 +114,41 @@ __device__ __forceinline__ double coord(const GridSpec& g, float v, int a) {
   return g.scaled ? __ddiv_rn(double(v), g.scale[a]) : double(v);
 }
 
-__device__ inline void cell_of(const GridSpec& g, const uint32_t* __restrict__ bounds, int f, float x,
-                               float y, float z, long long* ix, long long* iy, long long* iz) {
-  const double ox = __dsub_rn(coord(g, ordered_to_float(bounds[3 * f + 0]), 0), __dmul_rn(g.cell[0], g.origin_off));
-  const double oy = __dsub_rn(coord(g, ordered_to_float(bounds[3 * f + 1]), 1), __dmul_rn(g.cell[1], g.origin_off));
-  const double oz = __dsub_rn(coord(g, ordered_to_float(bounds[3 * f + 2]), 2), __dmul_rn(g.cell[2], g.origin_off));
-  *ix = (long long)floor(__ddiv_rn(__dsub_rn(coord(g, x, 0), ox), g.cell[0]));
-  *iy = (long long)floor(__ddiv_rn(__dsub_rn(coord(g, y, 1), oy), g.cell[1]));
-  *iz = (long long)floor(__ddiv_rn(__dsub_rn(coord(g, z, 2), oz), g.cell[2]));
+// grid origin of frame f on axis a (kVoxel, kRadius)
+__device__ inline double frame_origin(const GridSpec& g, const uint32_t* __restrict__ bounds, int f, int a) {
+  const double m = coord(g, ordered_to_float(bounds[3 * f + a]), a);
+  return g.rule == CellRule::kVoxel ? __dsub_rn(m, __dmul_rn(g.cell[a], 0.5)) : m;
 }
 
-// graph_gen.py:24-31 (defined next to the random keypoint path further down)
-__device__ void shifted_cell_of(const GridSpec& g, const uint32_t* __restrict__ bounds, int f, float x, float y, float z,
-                                long long* ix, long long* iy, long long* iz);
+__device__ inline void cell_of(const GridSpec& g, const uint32_t* __restrict__ bounds, int f, float x,
+                               float y, float z, long long* ix, long long* iy, long long* iz) {
+  *ix = (long long)floor(__ddiv_rn(__dsub_rn(coord(g, x, 0), frame_origin(g, bounds, f, 0)), g.cell[0]));
+  *iy = (long long)floor(__ddiv_rn(__dsub_rn(coord(g, y, 1), frame_origin(g, bounds, f, 1)), g.cell[1]));
+  *iz = (long long)floor(__ddiv_rn(__dsub_rn(coord(g, z, 2), frame_origin(g, bounds, f, 2)), g.cell[2]));
+}
+
+// NumPy's floor_divide for floats (npy_floor_divide / npy_divmod): Python semantics
+template <typename T>
+__device__ inline T np_floor_divide(T a, T b) {
+  T mod = fmod(a, b);
+  T div = (a - mod) / b;
+  if (mod != T(0) && ((b < T(0)) != (mod < T(0)))) div -= T(1);
+  if (div != T(0)) {
+    T fl = floor(div);
+    if (div - fl > T(0.5)) fl += T(1);
+    return fl;
+  }
+  return copysign(T(0), a / b);
+}
+
+// cell index of coordinate p on axis a under kNumpyF32 / kNumpyF64Shift; p - frame_min is a float32 difference, as
+// points_xyz - xyz_offset is upstream
+__device__ inline long long numpy_cell(const GridSpec& g, const uint32_t* __restrict__ bounds, int f, float p, int a) {
+  const float d = __fsub_rn(p, ordered_to_float(bounds[3 * f + a]));
+  if (g.rule == CellRule::kNumpyF32) return (long long)np_floor_divide<float>(d, float(g.cell[a]));
+  const double t = __dadd_rn(double(d), __dmul_rn(g.cell[a], g.shift[3 * f + a]));
+  return (long long)np_floor_divide<double>(t, g.cell[a]);
+}
 
 // `n_valid` (optional, device): only rows [0, *n_valid) of the n-row buffer hold points (a point set whose size is
 // still on the device, e.g. the keypoints of the same call); the others get the key of frame `num_frames`, which
@@ -134,9 +168,18 @@ __global__ void point_keys_kernel(const float* __restrict__ xyz, const int32_t* 
     return;
   }
   const int f = find_frame(frame_ptr, num_frames, i);
+  const float x = xyz[3 * i], y = xyz[3 * i + 1], z = xyz[3 * i + 2];
   long long ix, iy, iz;
-  if (g.shift != nullptr) shifted_cell_of(g, bounds, f, xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], &ix, &iy, &iz);
-  else cell_of(g, bounds, f, xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], &ix, &iy, &iz);
+  switch (g.rule) {
+    case CellRule::kVoxel:
+    case CellRule::kRadius:
+      cell_of(g, bounds, f, x, y, z, &ix, &iy, &iz);
+      break;
+    default:
+      ix = numpy_cell(g, bounds, f, x, 0);
+      iy = numpy_cell(g, bounds, f, y, 1);
+      iz = numpy_cell(g, bounds, f, z, 2);
+  }
   if (ix < 0 || iy < 0 || iz < 0 || ix > kAxisMax || iy > kAxisMax || iz > kAxisMax) {
     atomicOr(range_error, kErrRange);
     ix = iy = iz = 0;
@@ -197,11 +240,68 @@ __device__ inline void row_range(const SortedGrid& g, uint32_t f, uint32_t iz, u
   *end = g.cell_start[b];
 }
 
-__device__ inline double dist2_rn(double ax, double ay, double az, float bx, float by, float bz) {
-  const double dx = __dsub_rn(ax, double(bx));
-  const double dy = __dsub_rn(ay, double(by));
-  const double dz = __dsub_rn(az, double(bz));
+__device__ inline double dist2_rn(double ax, double ay, double az, double bx, double by, double bz) {
+  const double dx = __dsub_rn(ax, bx);
+  const double dy = __dsub_rn(ay, by);
+  const double dz = __dsub_rn(az, bz);
   return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
+}
+
+// fp64 centroid of the sorted points [s, e) of one voxel, summed in ascending point order (the sort is stable)
+__device__ inline void voxel_centroid(const SortedGrid& g, int s, int e, double c[3]) {
+  double sx = 0.0, sy = 0.0, sz = 0.0;
+  for (int i = s; i < e; ++i) {
+    const float4 p = g.pts[i];
+    sx = __dadd_rn(sx, double(p.x));
+    sy = __dadd_rn(sy, double(p.y));
+    sz = __dadd_rn(sz, double(p.z));
+  }
+  const double cnt = double(e - s);
+  c[0] = __ddiv_rn(sx, cnt);
+  c[1] = __ddiv_rn(sy, cnt);
+  c[2] = __ddiv_rn(sz, cnt);
+}
+
+// ---- exact nearest point: fp64 squared distance, ties -> lowest original index ----------------------------------
+struct Nearest {
+  double d = DBL_MAX;
+  int idx = 0x7fffffff;
+};
+
+__device__ inline void nearest_in_range(const SortedGrid& g, int b, int e, const double c[3], Nearest& best) {
+  for (int i = b; i < e; ++i) {
+    const float4 p = g.pts[i];
+    const double d = dist2_rn(c[0], c[1], c[2], p.x, p.y, p.z);
+    const int idx = __float_as_int(p.w);
+    if (d < best.d || (d == best.d && idx < best.idx)) { best.d = d; best.idx = idx; }
+  }
+}
+
+// every cell of frame f in the box lo..hi (clamped to the key space)
+__device__ inline void nearest_in_box(const SortedGrid& g, uint32_t f, const long long lo[3], const long long hi[3],
+                                      const double c[3], Nearest& best) {
+  const long long x0 = max(lo[0], 0ll), x1 = min(hi[0], (long long)kAxisMax);
+  if (x0 > x1) return;
+  for (long long iz = max(lo[2], 0ll); iz <= min(hi[2], (long long)kAxisMax); ++iz)
+    for (long long iy = max(lo[1], 0ll); iy <= min(hi[1], (long long)kAxisMax); ++iy) {
+      int b, e;
+      row_range(g, f, uint32_t(iz), uint32_t(iy), uint32_t(x0), uint32_t(x1), &b, &e);
+      nearest_in_range(g, b, e, c, best);
+    }
+}
+
+// Every point closer than sqrt(best.d) lies in a cell overlapping the box c +- reach: one pass over those cells.
+// reach is inflated by 1e-9 relative, far above the fp64 rounding of the box bounds, so they need no explicit rounding.
+__device__ inline void nearest_in_ball(const SortedGrid& g, const GridSpec& spec, const uint32_t* __restrict__ bounds,
+                                       uint32_t f, const double c[3], Nearest& best) {
+  const double reach = sqrt(best.d) * (1.0 + 1e-9) + 1e-12;
+  long long lo[3], hi[3];
+  for (int a = 0; a < 3; ++a) {
+    const double o = frame_origin(spec, bounds, f, a);
+    lo[a] = (long long)floor((c[a] - reach - o) / spec.cell[a]);
+    hi[a] = (long long)floor((c[a] + reach - o) / spec.cell[a]);
+  }
+  nearest_in_box(g, f, lo, hi, c, best);
 }
 
 // ---- voxel keypoints: centroid (fp64, ascending point order) + exact nearest original point ----
@@ -210,50 +310,12 @@ __global__ void voxel_keypoint_kernel(SortedGrid g, GridSpec spec, const uint32_
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= __ldg(g.num_cells)) return;
   const int s = g.cell_start[v], e = g.cell_start[v + 1];
-  double sx = 0.0, sy = 0.0, sz = 0.0;
-  for (int i = s; i < e; ++i) {  // sorted by (key, original index): ascending point order
-    const float4 p = g.pts[i];
-    sx = __dadd_rn(sx, double(p.x));
-    sy = __dadd_rn(sy, double(p.y));
-    sz = __dadd_rn(sz, double(p.z));
-  }
-  const double cnt = double(e - s);
-  const double cx = __ddiv_rn(sx, cnt), cy = __ddiv_rn(sy, cnt), cz = __ddiv_rn(sz, cnt);
-  // best candidate inside the own voxel
-  double best = DBL_MAX;
-  int best_idx = 0x7fffffff;
-  for (int i = s; i < e; ++i) {
-    const float4 p = g.pts[i];
-    const double d = dist2_rn(cx, cy, cz, p.x, p.y, p.z);
-    const int idx = __float_as_int(p.w);
-    if (d < best || (d == best && idx < best_idx)) { best = d; best_idx = idx; }
-  }
-  // every point closer than sqrt(best) lies in a cell overlapping the box centroid +- reach
-  const uint64_t key = g.cell_key[v];
-  const uint32_t f = uint32_t(key >> 48);
-  const double reach = sqrt(best) * (1.0 + 1e-9) + 1e-12;
-  const double ox = double(ordered_to_float(bounds[3 * f + 0])) - spec.cell[0] * spec.origin_off;
-  const double oy = double(ordered_to_float(bounds[3 * f + 1])) - spec.cell[1] * spec.origin_off;
-  const double oz = double(ordered_to_float(bounds[3 * f + 2])) - spec.cell[2] * spec.origin_off;
-  // reach is inflated by 1e-9 relative, far above the fp64 rounding of the corner cells
-  long long x0 = (long long)floor((cx - reach - ox) / spec.cell[0]), x1 = (long long)floor((cx + reach - ox) / spec.cell[0]);
-  long long y0 = (long long)floor((cy - reach - oy) / spec.cell[1]), y1 = (long long)floor((cy + reach - oy) / spec.cell[1]);
-  long long z0 = (long long)floor((cz - reach - oz) / spec.cell[2]), z1 = (long long)floor((cz + reach - oz) / spec.cell[2]);
-  x0 = max(x0, 0ll); y0 = max(y0, 0ll); z0 = max(z0, 0ll);
-  x1 = min(x1, (long long)kAxisMax); y1 = min(y1, (long long)kAxisMax); z1 = min(z1, (long long)kAxisMax);
-  for (long long iz = z0; iz <= z1; ++iz) {
-    for (long long iy = y0; iy <= y1; ++iy) {
-      int b, en;
-      row_range(g, f, uint32_t(iz), uint32_t(iy), uint32_t(x0), uint32_t(x1), &b, &en);
-      for (int i = b; i < en; ++i) {
-        const float4 p = g.pts[i];
-        const double d = dist2_rn(cx, cy, cz, p.x, p.y, p.z);
-        const int idx = __float_as_int(p.w);
-        if (d < best || (d == best && idx < best_idx)) { best = d; best_idx = idx; }
-      }
-    }
-  }
-  if (v < capacity) out_idx[v] = best_idx;
+  double c[3];
+  voxel_centroid(g, s, e, c);
+  Nearest best;
+  nearest_in_range(g, s, e, c, best);   // best candidate inside the own voxel
+  nearest_in_ball(g, spec, bounds, uint32_t(g.cell_key[v] >> 48), c, best);
+  if (v < capacity) out_idx[v] = best.idx;
 }
 
 // ---- general multi-scale keypoints (graph_gen.py:11-47 + :49-90 with more than one distinct scale) -------------
@@ -265,18 +327,7 @@ __global__ void voxel_centroid_kernel(SortedGrid g, double* __restrict__ out_cen
                                       int64_t capacity) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= __ldg(g.num_cells) || v >= capacity) return;
-  const int s = g.cell_start[v], e = g.cell_start[v + 1];
-  double sx = 0.0, sy = 0.0, sz = 0.0;
-  for (int i = s; i < e; ++i) {  // ascending point order (stable sort)
-    const float4 p = g.pts[i];
-    sx = __dadd_rn(sx, double(p.x));
-    sy = __dadd_rn(sy, double(p.y));
-    sz = __dadd_rn(sz, double(p.z));
-  }
-  const double cnt = double(e - s);
-  out_centroid[3 * int64_t(v) + 0] = __ddiv_rn(sx, cnt);
-  out_centroid[3 * int64_t(v) + 1] = __ddiv_rn(sy, cnt);
-  out_centroid[3 * int64_t(v) + 2] = __ddiv_rn(sz, cnt);
+  voxel_centroid(g, g.cell_start[v], g.cell_start[v + 1], out_centroid + 3 * int64_t(v));
   if (out_frame) out_frame[v] = int32_t(g.cell_key[v] >> 48);
 }
 
@@ -294,124 +345,37 @@ __global__ void nearest_point_kernel(SortedGrid g, GridSpec spec, const uint32_t
     out_idx[q] = 0;
     return;
   }
-  const double cx = q_xyz[3 * q], cy = q_xyz[3 * q + 1], cz = q_xyz[3 * q + 2];
-  const double ox = double(ordered_to_float(bounds[3 * f + 0])) - spec.cell[0] * spec.origin_off;
-  const double oy = double(ordered_to_float(bounds[3 * f + 1])) - spec.cell[1] * spec.origin_off;
-  const double oz = double(ordered_to_float(bounds[3 * f + 2])) - spec.cell[2] * spec.origin_off;
-  double best = DBL_MAX;
-  int best_idx = 0x7fffffff;
-  auto scan = [&](long long x0, long long x1, long long y0, long long y1, long long z0, long long z1) {
-    x0 = max(x0, 0ll); y0 = max(y0, 0ll); z0 = max(z0, 0ll);
-    x1 = min(x1, (long long)kAxisMax); y1 = min(y1, (long long)kAxisMax); z1 = min(z1, (long long)kAxisMax);
-    if (x0 > x1) return;
-    for (long long iz = z0; iz <= z1; ++iz)
-      for (long long iy = y0; iy <= y1; ++iy) {
-        int b, en;
-        row_range(g, f, uint32_t(iz), uint32_t(iy), uint32_t(x0), uint32_t(x1), &b, &en);
-        for (int i = b; i < en; ++i) {
-          const float4 p = g.pts[i];
-          const double d = dist2_rn(cx, cy, cz, p.x, p.y, p.z);
-          const int idx = __float_as_int(p.w);
-          if (d < best || (d == best && idx < best_idx)) { best = d; best_idx = idx; }
-        }
-      }
-  };
-  const long long ix = (long long)floor((cx - ox) / spec.cell[0]);
-  const long long iy = (long long)floor((cy - oy) / spec.cell[1]);
-  const long long iz = (long long)floor((cz - oz) / spec.cell[2]);
+  const double c[3] = {q_xyz[3 * q], q_xyz[3 * q + 1], q_xyz[3 * q + 2]};
+  long long ic[3];
+  for (int a = 0; a < 3; ++a) ic[a] = (long long)floor((c[a] - frame_origin(spec, bounds, f, a)) / spec.cell[a]);
+  Nearest best;
   // the frame is not empty, so a box that covers the whole key space terminates the loop
-  for (long long r = 1; best == DBL_MAX; r *= 2) {
-    scan(ix - r, ix + r, iy - r, iy + r, iz - r, iz + r);
-    if (r > 4ll * (kAxisMax + 1) + llabs(ix) + llabs(iy) + llabs(iz)) break;
+  for (long long r = 1; best.d == DBL_MAX; r *= 2) {
+    const long long lo[3] = {ic[0] - r, ic[1] - r, ic[2] - r}, hi[3] = {ic[0] + r, ic[1] + r, ic[2] + r};
+    nearest_in_box(g, f, lo, hi, c, best);
+    if (r > 4ll * (kAxisMax + 1) + llabs(ic[0]) + llabs(ic[1]) + llabs(ic[2])) break;
   }
-  if (best == DBL_MAX) {
+  if (best.d == DBL_MAX) {
     atomicOr(err, kErrRange);
     out_idx[q] = 0;
     return;
   }
-  // every point closer than sqrt(best) lies in a cell overlapping the box centroid +- reach
-  const double reach = sqrt(best) * (1.0 + 1e-9) + 1e-12;
-  scan((long long)floor((cx - reach - ox) / spec.cell[0]), (long long)floor((cx + reach - ox) / spec.cell[0]),
-       (long long)floor((cy - reach - oy) / spec.cell[1]), (long long)floor((cy + reach - oy) / spec.cell[1]),
-       (long long)floor((cz - reach - oz) / spec.cell[2]), (long long)floor((cz + reach - oz) / spec.cell[2]));
-  out_idx[q] = best_idx;
+  nearest_in_ball(g, spec, bounds, f, c, best);
+  out_idx[q] = best.idx;
 }
 
-__global__ void frame_ranges_kernel(const uint64_t* __restrict__ cell_key, const int32_t* __restrict__ num_cells,
-                                    int num_frames, int32_t* __restrict__ out_frame_ptr) {
+// frame_ptr of a key array sorted by frame: out_frame_ptr[f] = first key whose frame field (bits from
+// `frame_shift` up) is >= f
+__global__ void frame_ranges_kernel(const uint64_t* __restrict__ keys, const int32_t* __restrict__ num_keys,
+                                    int num_frames, int frame_shift, int32_t* __restrict__ out_frame_ptr) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f > num_frames) return;
-  out_frame_ptr[f] = lower_bound_u64(cell_key, __ldg(num_cells), uint64_t(f) << 48);
+  out_frame_ptr[f] = lower_bound_u64(keys, __ldg(num_keys), uint64_t(f) << frame_shift);
 }
 
-// ---- radius graph ----------------------------------------------------------------------------
-struct CenterCell {
-  uint32_t f;
-  long long ix, iy, iz;
-};
-
-// One warp per centre.  kFill=false: count neighbours.  kFill=true: write source indices at
-// row_ptr[c] + rank (rank from a warp ballot prefix, traversal order; rows are sorted afterwards).
-template <bool kFill>
-__global__ void __launch_bounds__(256) radius_query_kernel(
-    SortedGrid g, GridSpec spec, const uint32_t* __restrict__ bounds, const float* __restrict__ centers,
-    const int32_t* __restrict__ center_frame_ptr, int num_frames, int64_t num_centers_cap,
-    const int32_t* __restrict__ num_centers_dev, double r2, int32_t* __restrict__ counts,
-    const int32_t* __restrict__ row_ptr, int32_t* __restrict__ out_src, int64_t capacity, int* __restrict__ err,
-    unsigned long long* __restrict__ total64) {
-  const int lane = threadIdx.x & 31;
-  const int64_t c = (int64_t(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
-  // the number of centres may still be on the device (keypoints of the same call): launch for the capacity
-  const int64_t num_centers = num_centers_dev ? int64_t(*num_centers_dev) : num_centers_cap;
-  if (c >= num_centers || c >= num_centers_cap) return;
-  if (kFill && int64_t(row_ptr[min(num_centers, num_centers_cap)]) > capacity) return;   // edge buffer too small: reported by the host
-  if (!kFill && c == 0 && lane == 0 &&
-      (center_frame_ptr[0] != 0 || int64_t(center_frame_ptr[num_frames]) != num_centers))
-    atomicOr(err, kErrCenterPtr);
-  const int f = find_frame(center_frame_ptr, num_frames, c);
-  const float cxf = centers[3 * c], cyf = centers[3 * c + 1], czf = centers[3 * c + 2];
-  const double cx = coord(spec, cxf, 0), cy = coord(spec, cyf, 1), cz = coord(spec, czf, 2);
-  long long ix, iy, iz;
-  cell_of(spec, bounds, f, cxf, cyf, czf, &ix, &iy, &iz);
-  const long long x0 = max(ix - 1, 0ll), x1 = min(ix + 1, (long long)kAxisMax);
-  int total = 0;
-  int base = kFill ? row_ptr[c] : 0;
-  if (x0 <= x1) {
-    for (long long zz = iz - 1; zz <= iz + 1; ++zz) {
-      if (zz < 0 || zz > kAxisMax) continue;
-      for (long long yy = iy - 1; yy <= iy + 1; ++yy) {
-        if (yy < 0 || yy > kAxisMax) continue;
-        int b, e;
-        row_range(g, uint32_t(f), uint32_t(zz), uint32_t(yy), uint32_t(x0), uint32_t(x1), &b, &e);
-        for (int i0 = b; i0 < e; i0 += 32) {
-          const int i = i0 + lane;
-          bool hit = false;
-          int idx = 0;
-          if (i < e) {
-            const float4 p = g.pts[i];
-            if (spec.scaled) {
-              const double dx = __dsub_rn(cx, coord(spec, p.x, 0)), dy = __dsub_rn(cy, coord(spec, p.y, 1));
-              const double dz = __dsub_rn(cz, coord(spec, p.z, 2));
-              hit = __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)) <= r2;
-            } else {
-              hit = dist2_rn(cx, cy, cz, p.x, p.y, p.z) <= r2;
-            }
-            idx = __float_as_int(p.w);
-          }
-          const uint32_t m = __ballot_sync(0xffffffffu, hit);
-          if (kFill && hit) out_src[base + total + __popc(m & ((1u << lane) - 1u))] = idx;
-          total += __popc(m);
-        }
-      }
-    }
-  }
-  if (!kFill && lane == 0) {
-    counts[c] = total;
-    atomicAdd(total64, (unsigned long long)total);   // 64-bit edge total: the int32 row_ptr scan may wrap
-  }
-}
-
-// ---- single-traversal variant (pg_multi_level_graph) -------------------------------------------------------------
+// ---- radius graph: one traversal of the points per centre ---------------------------------------------------------
+// The number of centres is `num_centers_dev` (device, e.g. the keypoints of the same call) or, when that is null,
+// `num_centers_cap`; the kernels are launched for the capacity.
 // Pass A, one THREAD per centre: the nine sorted-point ranges of its 3 x 3 x 3 cell neighbourhood (18 ints) and
 // their total length = an upper bound of the row length.  No point is touched.
 __global__ void radius_candidates_kernel(SortedGrid g, GridSpec spec, const uint32_t* __restrict__ bounds,
@@ -420,12 +384,12 @@ __global__ void radius_candidates_kernel(SortedGrid g, GridSpec spec, const uint
                                          int32_t* __restrict__ ranges, int32_t* __restrict__ cand, int* __restrict__ err) {
   const int64_t c = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
   if (c > num_centers_cap) return;
-  const int64_t num_centers = min(int64_t(*num_centers_dev), num_centers_cap);
-  if (c >= num_centers) {
+  const int64_t num_centers = num_centers_dev ? int64_t(*num_centers_dev) : num_centers_cap;
+  if (c >= min(num_centers, num_centers_cap)) {
     cand[c] = 0;
     return;
   }
-  if (c == 0 && (center_frame_ptr[0] != 0 || int64_t(center_frame_ptr[num_frames]) != int64_t(*num_centers_dev)))
+  if (c == 0 && (center_frame_ptr[0] != 0 || int64_t(center_frame_ptr[num_frames]) != num_centers))
     atomicOr(err, kErrCenterPtr);
   const int f = find_frame(center_frame_ptr, num_frames, c);
   long long ix, iy, iz;
@@ -445,49 +409,52 @@ __global__ void radius_candidates_kernel(SortedGrid g, GridSpec spec, const uint
   cand[c] = total;
 }
 
-// Pass B, one WARP per centre: the only traversal of the points.  Hits are parked, compacted in traversal order, at
-// tmp[cand_off[c] ...] (cand_off = exclusive scan of the candidate counts, so the slots never overlap); counts[c]
-// = row length.  The row sort then reads the parked hits and writes the final CSR row.
-__global__ void __launch_bounds__(256) radius_collect_kernel(SortedGrid g, const float* __restrict__ centers,
+// Pass B, one WARP per centre: the only traversal of the points.  The hits of centre c are written, compacted in
+// traversal order, at out[out_off[c] ...]: either parked at the exclusive scan of the candidate counts (the slots never
+// overlap; the row sort then reads them and writes the final CSR row) or written at row_ptr (the row is then sorted in
+// place).  out == nullptr: count only.  counts (optional): counts[c] = row length, added to the 64-bit total.
+// kScaled = spec.scaled as a template parameter: the fp64 division takes the unscaled kernel from 32 to 52 registers.
+template <bool kScaled>
+__global__ void __launch_bounds__(256) radius_collect_kernel(SortedGrid g, GridSpec spec, const float* __restrict__ centers,
                                                              int64_t num_centers_cap,
                                                              const int32_t* __restrict__ num_centers_dev, double r2,
                                                              const int32_t* __restrict__ ranges,
-                                                             const int32_t* __restrict__ cand_off, int64_t tmp_capacity,
-                                                             int32_t* __restrict__ tmp, int32_t* __restrict__ counts,
+                                                             const int32_t* __restrict__ out_off, int64_t out_capacity,
+                                                             int32_t* __restrict__ out, int32_t* __restrict__ counts,
                                                              unsigned long long* __restrict__ total64, int* __restrict__ err) {
   const int lane = threadIdx.x & 31;
   const int64_t c = (int64_t(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
-  const int64_t num_centers = min(int64_t(*num_centers_dev), num_centers_cap);
+  const int64_t num_centers = num_centers_dev ? min(int64_t(*num_centers_dev), num_centers_cap) : num_centers_cap;
   if (c >= num_centers) return;
-  if (int64_t(cand_off[num_centers_cap]) > tmp_capacity) {     // the parking buffer is too small: reported by the host
+  if (out && int64_t(out_off[num_centers_cap]) > out_capacity) {     // the output buffer is too small: reported by the host
     if (c == 0 && lane == 0) atomicOr(err, kErrParking);
     return;
   }
-  const double cx = double(centers[3 * c]), cy = double(centers[3 * c + 1]), cz = double(centers[3 * c + 2]);
-  const int base = cand_off[c];
+  auto co = [&](float v, int a) { return kScaled ? coord(spec, v, a) : double(v); };
+  const double cx = co(centers[3 * c], 0), cy = co(centers[3 * c + 1], 1), cz = co(centers[3 * c + 2], 2);
+  const int base = out ? out_off[c] : 0;
   int total = 0;
-  int rb = 0, re = 0;
+  int rb = 0;
   if (lane < 18) rb = ranges[c * 18 + lane];
   for (int k = 0; k < 9; ++k) {
     const int b = __shfl_sync(0xffffffffu, rb, 2 * k), e = __shfl_sync(0xffffffffu, rb, 2 * k + 1);
-    (void)re;
     for (int i0 = b; i0 < e; i0 += 32) {
       const int i = i0 + lane;
       bool hit = false;
       int idx = 0;
       if (i < e) {
         const float4 p = g.pts[i];
-        hit = dist2_rn(cx, cy, cz, p.x, p.y, p.z) <= r2;
+        hit = dist2_rn(cx, cy, cz, co(p.x, 0), co(p.y, 1), co(p.z, 2)) <= r2;
         idx = __float_as_int(p.w);
       }
       const uint32_t m = __ballot_sync(0xffffffffu, hit);
-      if (hit) tmp[base + total + __popc(m & ((1u << lane) - 1u))] = idx;
+      if (out && hit) out[base + total + __popc(m & ((1u << lane) - 1u))] = idx;
       total += __popc(m);
     }
   }
-  if (lane == 0) {
+  if (counts && lane == 0) {
     counts[c] = total;
-    atomicAdd(total64, (unsigned long long)total);
+    atomicAdd(total64, (unsigned long long)total);   // 64-bit edge total: the int32 row_ptr scan may wrap
   }
 }
 
@@ -604,6 +571,13 @@ struct BuiltGrid {
   SortedGrid view{};
 };
 
+// key bits the frame field needs, including frame `num_frames` (the key of rows beyond n_valid, voxels beyond K)
+int frame_bits(int num_frames) {
+  int bits = 1;
+  while ((1 << bits) < num_frames + 1) ++bits;
+  return bits;
+}
+
 int build_grid(const float* xyz, const int32_t* frame_ptr, int num_frames, int64_t n, const GridSpec& spec,
                cudaStream_t s, BuiltGrid* out, const int32_t* n_valid = nullptr) {
   PG_REQUIRE(num_frames >= 1 && num_frames <= 65534, "num_frames=%d out of range [1,65534]", num_frames);
@@ -632,9 +606,7 @@ int build_grid(const float* xyz, const int32_t* frame_ptr, int num_frames, int64
                                                       out->err.as<int>());
   PG_LAUNCH_CHECK();
   // radix sort (key, original index); stable, so equal keys keep ascending point index
-  int frame_bits = 1;
-  while ((1 << frame_bits) < num_frames + 1) ++frame_bits;     // + 1: the key of rows beyond n_valid
-  const int end_bit = 48 + frame_bits;
+  const int end_bit = 48 + frame_bits(num_frames);
   size_t tmp_bytes = 0;
   PG_CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, out->keys_a.as<uint64_t>(), out->keys_b.as<uint64_t>(),
                                              out->vals_a.as<int32_t>(), out->vals_b.as<int32_t>(), int(n), 0, end_bit, s));
@@ -682,6 +654,47 @@ int graph_error(int err) {
   return PG_OK;
 }
 
+// ---- keypoint calls: voxel grid spec, and the end every keypoint call shares ----------------------------------
+int voxel_spec(const double* voxel_size_host, CellRule rule, GridSpec* spec) {
+  PG_REQUIRE(voxel_size_host[0] > 0 && voxel_size_host[1] > 0 && voxel_size_host[2] > 0, "voxel size must be positive");
+  *spec = GridSpec{};
+  for (int a = 0; a < 3; ++a) spec->cell[a] = voxel_size_host[a];
+  spec->rule = rule;
+  return PG_OK;
+}
+
+// kNumpyF64Shift: the per-frame shifts (host [num_frames][3]) copied to the device
+int upload_shift(const double* shift_host, int num_frames, cudaStream_t s, Temp* shift, GridSpec* spec) {
+  PG_REQUIRE(num_frames >= 1 && num_frames <= 65534, "num_frames=%d out of range [1,65534]", num_frames);
+  PG_CUDA_OK(shift->alloc(sizeof(double) * 3 * num_frames, s));
+  PG_CUDA_OK(cudaMemcpyAsync(shift->ptr, shift_host, sizeof(double) * 3 * num_frames, cudaMemcpyHostToDevice, s));
+  spec->shift = shift->as<double>();
+  return PG_OK;
+}
+
+// The keypoint frame ranges (frame field of the sorted `keys` at `frame_shift`), then the one host round trip of the
+// call: K and the error words of its grids (err1 may be null), their decoding, and the check of K against `capacity`.
+int finish_keypoints(const uint64_t* keys, int frame_shift, const int32_t* num_keys, int num_frames, const int* err0,
+                     const int* err1, int64_t capacity, const char* what, int32_t* out_frame_ptr, int64_t* out_num_host,
+                     cudaStream_t s) {
+  frame_ranges_kernel<<<ceil_div(num_frames + 1, 128), 128, 0, s>>>(keys, num_keys, num_frames, frame_shift, out_frame_ptr);
+  PG_LAUNCH_CHECK();
+  int32_t h[3] = {0, 0, 0};
+  PG_CUDA_OK(cudaMemcpyAsync(&h[0], num_keys, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  PG_CUDA_OK(cudaMemcpyAsync(&h[1], err0, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  if (err1 != nullptr) PG_CUDA_OK(cudaMemcpyAsync(&h[2], err1, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  PG_CUDA_OK(cudaStreamSynchronize(s));
+  if (int rc = graph_error(h[1])) return rc;
+  if (int rc = graph_error(h[2])) return rc;
+  *out_num_host = h[0];
+  if (h[0] > capacity) {
+    set_error("%s buffer too small: need %d, capacity %lld", what, h[0], (long long)capacity);
+    return PG_ERR_CAPACITY;
+  }
+  return PG_OK;
+}
+
+// ---- radius graphs ----------------------------------------------------------------------------
 struct RadiusPlan {
   BuiltGrid grid;
   GridSpec spec{};
@@ -689,11 +702,12 @@ struct RadiusPlan {
 };
 
 int radius_prepare(const float* points, const int32_t* point_frame_ptr, int num_frames, int64_t num_points,
-                   double radius, cudaStream_t s, RadiusPlan* plan, const double* scale_host = nullptr) {
+                   double radius, cudaStream_t s, RadiusPlan* plan, const double* scale_host = nullptr,
+                   const int32_t* n_valid = nullptr) {
   PG_REQUIRE(radius > 0.0, "radius must be positive");
   plan->spec = GridSpec{};
   plan->spec.cell[0] = plan->spec.cell[1] = plan->spec.cell[2] = radius * kCellSlack;
-  plan->spec.origin_off = 0.0;
+  plan->spec.rule = CellRule::kRadius;
   plan->spec.scale[0] = plan->spec.scale[1] = plan->spec.scale[2] = 1.0;
   if (scale_host != nullptr) {
     PG_REQUIRE(scale_host[0] > 0 && scale_host[1] > 0 && scale_host[2] > 0, "scale must be positive");
@@ -701,7 +715,131 @@ int radius_prepare(const float* points, const int32_t* point_frame_ptr, int num_
     for (int a = 0; a < 3; ++a) plan->spec.scale[a] = scale_host[a];
   }
   plan->r2 = radius * radius;
-  return build_grid(points, point_frame_ptr, num_frames, num_points, plan->spec, s, &plan->grid);
+  return build_grid(points, point_frame_ptr, num_frames, num_points, plan->spec, s, &plan->grid, n_valid);
+}
+
+// pass A: ranges [18 * num_centers_cap], cand [num_centers_cap + 1]
+int radius_candidates(RadiusPlan& plan, const float* centers, const int32_t* center_frame_ptr, int num_frames,
+                      int64_t num_centers_cap, const int32_t* num_centers_dev, int32_t* ranges, int32_t* cand,
+                      cudaStream_t s) {
+  radius_candidates_kernel<<<ceil_div(num_centers_cap + 1, 128), 128, 0, s>>>(
+      plan.grid.view, plan.spec, plan.grid.bounds.as<uint32_t>(), centers, center_frame_ptr, num_frames,
+      num_centers_cap, num_centers_dev, ranges, cand, plan.grid.err.as<int>());
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}
+
+int radius_collect(RadiusPlan& plan, const float* centers, int64_t num_centers_cap, const int32_t* num_centers_dev,
+                   const int32_t* ranges, const int32_t* out_off, int64_t out_capacity, int32_t* out, int32_t* counts,
+                   unsigned long long* total64, cudaStream_t s) {
+  auto kernel = plan.spec.scaled ? radius_collect_kernel<true> : radius_collect_kernel<false>;
+  kernel<<<ceil_div(num_centers_cap * 32, 256), 256, 0, s>>>(
+      plan.grid.view, plan.spec, centers, num_centers_cap, num_centers_dev, plan.r2, ranges, out_off,
+      out_capacity, out, counts, total64, plan.grid.err.as<int>());
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}
+
+// Sort every CSR row ascending and expand dst (`in` / `in_off` as sort_rows_warp_kernel); nothing happens when
+// row_ptr[num_rows] > capacity.
+int sort_rows(const int32_t* row_ptr, int64_t num_rows, int32_t* src, int32_t* dst, int64_t capacity,
+              const int32_t* in, const int32_t* in_off, cudaStream_t s) {
+  Temp has_long;
+  PG_CUDA_OK(has_long.alloc(sizeof(int), s));
+  PG_CUDA_OK(cudaMemsetAsync(has_long.ptr, 0, sizeof(int), s));
+  const int wblocks = int(std::min<int64_t>(ceil_div(num_rows, 8), int64_t(num_sms()) * 6));
+  sort_rows_warp_kernel<<<wblocks, 256, 0, s>>>(row_ptr, num_rows, src, dst, has_long.as<int>(), capacity, in, in_off);
+  PG_LAUNCH_CHECK();
+  // rows longer than kWarpRowMax (dense full-360 clouds): one block per row
+  const int blocks = int(std::min<int64_t>(num_rows, int64_t(num_sms()) * 4));
+  sort_rows_kernel<<<blocks, 256, kRowSortMax * sizeof(int32_t), s>>>(row_ptr, num_rows, src, dst, has_long.as<int>(),
+                                                                      capacity, in, in_off);
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}
+
+// Pass A of the stand-alone calls over all num_centers centres; `ranges` is kept by the caller for pass B.
+int radius_ranges(RadiusPlan& plan, const float* centers, const int32_t* center_frame_ptr, int num_frames,
+                  int64_t num_centers, Temp* ranges, cudaStream_t s) {
+  Temp cand;
+  PG_CUDA_OK(ranges->alloc(sizeof(int32_t) * 18 * num_centers, s));
+  PG_CUDA_OK(cand.alloc(sizeof(int32_t) * (num_centers + 1), s));
+  return radius_candidates(plan, centers, center_frame_ptr, num_frames, num_centers, nullptr, ranges->as<int32_t>(),
+                           cand.as<int32_t>(), s);
+}
+
+// Count half of the stand-alone radius graph: pass A, pass B counting only, out_row_ptr = exclusive scan of the row
+// lengths, then the one host round trip: E (64 bit) and the error word.
+int radius_count_rows(RadiusPlan& plan, const float* centers, const int32_t* center_frame_ptr, int num_frames,
+                      int64_t num_centers, Temp* ranges, int32_t* out_row_ptr, int64_t* out_num_edges_host,
+                      cudaStream_t s) {
+  Temp counts, tmp, total;
+  PG_CUDA_OK(counts.alloc(sizeof(int32_t) * (num_centers + 1), s));
+  PG_CUDA_OK(cudaMemsetAsync(counts.ptr, 0, sizeof(int32_t) * (num_centers + 1), s));
+  PG_CUDA_OK(total.alloc(sizeof(unsigned long long), s));
+  PG_CUDA_OK(cudaMemsetAsync(total.ptr, 0, sizeof(unsigned long long), s));
+  if (int rc = radius_ranges(plan, centers, center_frame_ptr, num_frames, num_centers, ranges, s)) return rc;
+  if (int rc = radius_collect(plan, centers, num_centers, nullptr, ranges->as<int32_t>(), nullptr, 0, nullptr,
+                              counts.as<int32_t>(), total.as<unsigned long long>(), s))
+    return rc;
+  size_t bytes = 0;
+  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, bytes, counts.as<int32_t>(), out_row_ptr, int(num_centers + 1), s));
+  PG_CUDA_OK(tmp.alloc(bytes, s));
+  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(tmp.ptr, bytes, counts.as<int32_t>(), out_row_ptr, int(num_centers + 1), s));
+  count_launch(2);
+  unsigned long long h_total = 0;
+  int32_t h_err = 0;
+  PG_CUDA_OK(cudaMemcpyAsync(&h_total, total.ptr, sizeof(h_total), cudaMemcpyDeviceToHost, s));
+  PG_CUDA_OK(cudaMemcpyAsync(&h_err, plan.grid.err.ptr, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  PG_CUDA_OK(cudaStreamSynchronize(s));
+  if (int rc = graph_error(h_err)) return rc;
+  *out_num_edges_host = int64_t(h_total);
+  if (h_total > 0x7fffffffull) {    // row_ptr is int32 (the reference's int32 edge arrays, train.py:131)
+    set_error("radius graph has %llu edges: more than int32 row_ptr can index; split the batch", h_total);
+    return PG_ERR_RANGE;
+  }
+  return PG_OK;
+}
+
+// Fill half (after pass A): pass B writing every row at row_ptr, then every row sorted in place.
+int radius_fill_rows(RadiusPlan& plan, const float* centers, int64_t num_centers, const int32_t* ranges,
+                     const int32_t* row_ptr, int64_t num_edges, int32_t* out_src, int32_t* out_dst, cudaStream_t s) {
+  if (int rc = radius_collect(plan, centers, num_centers, nullptr, ranges, row_ptr, num_edges, out_src, nullptr,
+                              nullptr, s))
+    return rc;
+  return sort_rows(row_ptr, num_centers, out_src, out_dst, num_edges, nullptr, nullptr, s);
+}
+
+// One radius level of pg_multi_level_graph: candidates -> scan -> collect into the parking buffer -> scan -> row sort,
+// the number of centres and the number of edges staying on the device (`num_centers_dev`; E = out_row_ptr[kp_capacity]).
+int radius_level_device(RadiusPlan& plan, const float* centers, const int32_t* center_frame_ptr, int num_frames,
+                        int64_t kp_capacity, const int32_t* num_centers_dev, int32_t* out_row_ptr, int32_t* out_src,
+                        int32_t* out_dst, int64_t capacity, unsigned long long* total64, cudaStream_t s) {
+  // candidates per row are ~6.5x the hits (27 cells of edge r against the ball of radius r); the parking buffer is
+  // sized from the caller's edge capacity and its overflow is reported like an edge-buffer overflow
+  const int64_t tmp_capacity = std::min<int64_t>(capacity * 10 + 4096, (int64_t(1) << 31) - 1);
+  Temp counts, cand, cand_off, ranges, parked, tmp;
+  PG_CUDA_OK(counts.alloc(sizeof(int32_t) * (kp_capacity + 1), s));
+  PG_CUDA_OK(cudaMemsetAsync(counts.ptr, 0, sizeof(int32_t) * (kp_capacity + 1), s));
+  PG_CUDA_OK(cand.alloc(sizeof(int32_t) * (kp_capacity + 1), s));
+  PG_CUDA_OK(cand_off.alloc(sizeof(int32_t) * (kp_capacity + 1), s));
+  PG_CUDA_OK(ranges.alloc(sizeof(int32_t) * 18 * kp_capacity, s));
+  PG_CUDA_OK(parked.alloc(sizeof(int32_t) * tmp_capacity, s));
+  if (int rc = radius_candidates(plan, centers, center_frame_ptr, num_frames, kp_capacity, num_centers_dev,
+                                 ranges.as<int32_t>(), cand.as<int32_t>(), s))
+    return rc;
+  size_t bytes = 0;
+  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, bytes, cand.as<int32_t>(), cand_off.as<int32_t>(), int(kp_capacity + 1), s));
+  PG_CUDA_OK(tmp.alloc(bytes, s));
+  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(tmp.ptr, bytes, cand.as<int32_t>(), cand_off.as<int32_t>(), int(kp_capacity + 1), s));
+  count_launch(2);
+  if (int rc = radius_collect(plan, centers, kp_capacity, num_centers_dev, ranges.as<int32_t>(), cand_off.as<int32_t>(),
+                              tmp_capacity, parked.as<int32_t>(), counts.as<int32_t>(), total64, s))
+    return rc;
+  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(tmp.ptr, bytes, counts.as<int32_t>(), out_row_ptr, int(kp_capacity + 1), s));
+  count_launch(2);
+  // rows beyond the real number of centres are empty, so row_ptr[c] == E for every c >= K
+  return sort_rows(out_row_ptr, kp_capacity, out_src, out_dst, capacity, parked.as<int32_t>(), cand_off.as<int32_t>(), s);
 }
 
 }  // namespace
@@ -715,12 +853,8 @@ extern "C" int pg_voxel_keypoints(const float* xyz, const int32_t* frame_ptr, in
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   PG_REQUIRE(xyz && frame_ptr && voxel_size_host && out_keypoint_idx && out_kp_frame_ptr && out_num_keypoints_host,
              "pg_voxel_keypoints: null argument");
-  PG_REQUIRE(voxel_size_host[0] > 0 && voxel_size_host[1] > 0 && voxel_size_host[2] > 0, "voxel size must be positive");
-  GridSpec spec{};
-  spec.cell[0] = voxel_size_host[0];
-  spec.cell[1] = voxel_size_host[1];
-  spec.cell[2] = voxel_size_host[2];
-  spec.origin_off = 0.5;  // Open3D: voxel_min_bound = min_bound - voxel_size * 0.5
+  GridSpec spec;
+  if (int rc = voxel_spec(voxel_size_host, CellRule::kVoxel, &spec)) return rc;
   BuiltGrid grid;
   if (int rc = build_grid(xyz, frame_ptr, num_frames, num_points, spec, s, &grid)) return rc;
   // K = number of occupied voxels <= N is only known on the device: launch for N, surplus threads exit;
@@ -728,20 +862,8 @@ extern "C" int pg_voxel_keypoints(const float* xyz, const int32_t* frame_ptr, in
   voxel_keypoint_kernel<<<ceil_div(num_points, 128), 128, 0, s>>>(grid.view, spec, grid.bounds.as<uint32_t>(),
                                                                     out_keypoint_idx, capacity);
   PG_LAUNCH_CHECK();
-  frame_ranges_kernel<<<ceil_div(num_frames + 1, 128), 128, 0, s>>>(grid.view.cell_key, grid.view.num_cells, num_frames,
-                                                                     out_kp_frame_ptr);
-  PG_LAUNCH_CHECK();
-  int32_t h[2] = {0, 0};   // the one host round trip of this call: K and the error word
-  PG_CUDA_OK(cudaMemcpyAsync(&h[0], grid.view.num_cells, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaMemcpyAsync(&h[1], grid.err.ptr, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaStreamSynchronize(s));
-  if (int rc = graph_error(h[1])) return rc;
-  *out_num_keypoints_host = h[0];
-  if (h[0] > capacity) {
-    set_error("keypoint buffer too small: need %d, capacity %lld", h[0], (long long)capacity);
-    return PG_ERR_CAPACITY;
-  }
-  return PG_OK;
+  return finish_keypoints(grid.view.cell_key, 48, grid.view.num_cells, num_frames, grid.err.as<int>(), nullptr, capacity,
+                          "keypoint", out_kp_frame_ptr, out_num_keypoints_host, s);
 }
 
 // multi_layer_downsampling for one scale (graph_gen.py:41-45): the fp64 voxel centroids themselves.
@@ -751,30 +873,14 @@ extern "C" int pg_voxel_centroids(const float* xyz, const int32_t* frame_ptr, in
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   PG_REQUIRE(xyz && frame_ptr && voxel_size_host && out_centroids && out_frame_ptr && out_num_host,
              "pg_voxel_centroids: null argument");
-  PG_REQUIRE(voxel_size_host[0] > 0 && voxel_size_host[1] > 0 && voxel_size_host[2] > 0, "voxel size must be positive");
-  GridSpec spec{};
-  spec.cell[0] = voxel_size_host[0];
-  spec.cell[1] = voxel_size_host[1];
-  spec.cell[2] = voxel_size_host[2];
-  spec.origin_off = 0.5;
+  GridSpec spec;
+  if (int rc = voxel_spec(voxel_size_host, CellRule::kVoxel, &spec)) return rc;
   BuiltGrid grid;
   if (int rc = build_grid(xyz, frame_ptr, num_frames, num_points, spec, s, &grid)) return rc;
   voxel_centroid_kernel<<<ceil_div(num_points, 128), 128, 0, s>>>(grid.view, out_centroids, nullptr, capacity);
   PG_LAUNCH_CHECK();
-  frame_ranges_kernel<<<ceil_div(num_frames + 1, 128), 128, 0, s>>>(grid.view.cell_key, grid.view.num_cells, num_frames,
-                                                                     out_frame_ptr);
-  PG_LAUNCH_CHECK();
-  int32_t h[2] = {0, 0};
-  PG_CUDA_OK(cudaMemcpyAsync(&h[0], grid.view.num_cells, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaMemcpyAsync(&h[1], grid.err.ptr, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaStreamSynchronize(s));
-  if (int rc = graph_error(h[1])) return rc;
-  *out_num_host = h[0];
-  if (h[0] > capacity) {
-    set_error("centroid buffer too small: need %d, capacity %lld", h[0], (long long)capacity);
-    return PG_ERR_CAPACITY;
-  }
-  return PG_OK;
+  return finish_keypoints(grid.view.cell_key, 48, grid.view.num_cells, num_frames, grid.err.as<int>(), nullptr, capacity,
+                          "centroid", out_frame_ptr, out_num_host, s);
 }
 
 // multi_layer_downsampling_select for a scale that differs from the previous level's (graph_gen.py:82-88):
@@ -788,12 +894,8 @@ extern "C" int pg_voxel_keypoints_select(const float* xyz, const int32_t* frame_
   PG_REQUIRE(xyz && frame_ptr && voxel_size_host && base_xyz && base_frame_ptr && out_keypoint_idx && out_kp_frame_ptr &&
                  out_num_keypoints_host,
              "pg_voxel_keypoints_select: null argument");
-  PG_REQUIRE(voxel_size_host[0] > 0 && voxel_size_host[1] > 0 && voxel_size_host[2] > 0, "voxel size must be positive");
-  GridSpec spec{};
-  spec.cell[0] = voxel_size_host[0];
-  spec.cell[1] = voxel_size_host[1];
-  spec.cell[2] = voxel_size_host[2];
-  spec.origin_off = 0.5;
+  GridSpec spec;
+  if (int rc = voxel_spec(voxel_size_host, CellRule::kVoxel, &spec)) return rc;
   BuiltGrid grid, base;
   if (int rc = build_grid(xyz, frame_ptr, num_frames, num_points, spec, s, &grid)) return rc;
   Temp cent, cframe;
@@ -802,30 +904,16 @@ extern "C" int pg_voxel_keypoints_select(const float* xyz, const int32_t* frame_
   voxel_centroid_kernel<<<ceil_div(num_points, 128), 128, 0, s>>>(grid.view, cent.as<double>(), cframe.as<int32_t>(),
                                                                     num_points);
   PG_LAUNCH_CHECK();
-  frame_ranges_kernel<<<ceil_div(num_frames + 1, 128), 128, 0, s>>>(grid.view.cell_key, grid.view.num_cells, num_frames,
-                                                                     out_kp_frame_ptr);
-  PG_LAUNCH_CHECK();
   GridSpec bspec = spec;       // search grid over the base vertices, same cell size
-  bspec.origin_off = 0.0;
+  bspec.rule = CellRule::kRadius;
   if (int rc = build_grid(base_xyz, base_frame_ptr, num_frames, num_base, bspec, s, &base)) return rc;
   nearest_point_kernel<<<ceil_div(num_points, 128), 128, 0, s>>>(base.view, bspec, base.bounds.as<uint32_t>(), base_frame_ptr,
                                                                    cent.as<double>(), cframe.as<int32_t>(),
                                                                    grid.view.num_cells, capacity, out_keypoint_idx,
                                                                    base.err.as<int>());
   PG_LAUNCH_CHECK();
-  int32_t h[3] = {0, 0, 0};
-  PG_CUDA_OK(cudaMemcpyAsync(&h[0], grid.view.num_cells, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaMemcpyAsync(&h[1], grid.err.ptr, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaMemcpyAsync(&h[2], base.err.ptr, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaStreamSynchronize(s));
-  if (int rc = graph_error(h[1])) return rc;
-  if (int rc = graph_error(h[2])) return rc;
-  *out_num_keypoints_host = h[0];
-  if (h[0] > capacity) {
-    set_error("keypoint buffer too small: need %d, capacity %lld", h[0], (long long)capacity);
-    return PG_ERR_CAPACITY;
-  }
-  return PG_OK;
+  return finish_keypoints(grid.view.cell_key, 48, grid.view.num_cells, num_frames, grid.err.as<int>(),
+                          base.err.as<int>(), capacity, "keypoint", out_kp_frame_ptr, out_num_keypoints_host, s);
 }
 
 // multi_layer_downsampling / multi_layer_downsampling_select with add_rnd3d (graph_gen.py:24-39 + :82-88): the voxel
@@ -842,15 +930,10 @@ extern "C" int pg_voxel_keypoints_rnd3d(const float* xyz, const int32_t* frame_p
              "pg_voxel_keypoints_rnd3d: null argument");
   PG_REQUIRE((base_xyz != nullptr) == (out_keypoint_idx != nullptr), "pg_voxel_keypoints_rnd3d: base_xyz and out_keypoint_idx go together");
   PG_REQUIRE(base_xyz == nullptr || base_frame_ptr != nullptr, "pg_voxel_keypoints_rnd3d: base_frame_ptr is null");
-  PG_REQUIRE(voxel_size_host[0] > 0 && voxel_size_host[1] > 0 && voxel_size_host[2] > 0, "voxel size must be positive");
+  GridSpec spec;
+  if (int rc = voxel_spec(voxel_size_host, CellRule::kNumpyF64Shift, &spec)) return rc;
   Temp shift;
-  PG_CUDA_OK(shift.alloc(sizeof(double) * 3 * num_frames, s));
-  PG_CUDA_OK(cudaMemcpyAsync(shift.ptr, shift_host, sizeof(double) * 3 * num_frames, cudaMemcpyHostToDevice, s));
-  GridSpec spec{};
-  spec.cell[0] = voxel_size_host[0];
-  spec.cell[1] = voxel_size_host[1];
-  spec.cell[2] = voxel_size_host[2];
-  spec.shift = shift.as<double>();
+  if (int rc = upload_shift(shift_host, num_frames, s, &shift, &spec)) return rc;
   BuiltGrid grid, base;
   if (int rc = build_grid(xyz, frame_ptr, num_frames, num_points, spec, s, &grid)) return rc;
   Temp cent, cframe;
@@ -863,87 +946,19 @@ extern "C" int pg_voxel_keypoints_rnd3d(const float* xyz, const int32_t* frame_p
   PG_CUDA_OK(cframe.alloc(sizeof(int32_t) * num_points, s));
   voxel_centroid_kernel<<<ceil_div(num_points, 128), 128, 0, s>>>(grid.view, cent_ptr, cframe.as<int32_t>(), cent_cap);
   PG_LAUNCH_CHECK();
-  frame_ranges_kernel<<<ceil_div(num_frames + 1, 128), 128, 0, s>>>(grid.view.cell_key, grid.view.num_cells, num_frames,
-                                                                     out_kp_frame_ptr);
-  PG_LAUNCH_CHECK();
-  int32_t h[3] = {0, 0, 0};
   if (base_xyz != nullptr) {
-    GridSpec bspec{};
-    bspec.cell[0] = voxel_size_host[0];
-    bspec.cell[1] = voxel_size_host[1];
-    bspec.cell[2] = voxel_size_host[2];
+    GridSpec bspec;
+    if (int rc = voxel_spec(voxel_size_host, CellRule::kRadius, &bspec)) return rc;
     if (int rc = build_grid(base_xyz, base_frame_ptr, num_frames, num_base, bspec, s, &base)) return rc;
     nearest_point_kernel<<<ceil_div(num_points, 128), 128, 0, s>>>(base.view, bspec, base.bounds.as<uint32_t>(),
                                                                      base_frame_ptr, cent_ptr, cframe.as<int32_t>(),
                                                                      grid.view.num_cells, std::min(capacity, cent_cap),
                                                                      out_keypoint_idx, base.err.as<int>());
     PG_LAUNCH_CHECK();
-    PG_CUDA_OK(cudaMemcpyAsync(&h[2], base.err.ptr, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
   }
-  PG_CUDA_OK(cudaMemcpyAsync(&h[0], grid.view.num_cells, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaMemcpyAsync(&h[1], grid.err.ptr, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaStreamSynchronize(s));
-  if (int rc = graph_error(h[1])) return rc;
-  if (int rc = graph_error(h[2])) return rc;
-  *out_num_keypoints_host = h[0];
-  if (h[0] > capacity) {
-    set_error("keypoint buffer too small: need %d, capacity %lld", h[0], (long long)capacity);
-    return PG_ERR_CAPACITY;
-  }
-  return PG_OK;
-}
-
-static int radius_count_impl(RadiusPlan& plan, const float* centers, const int32_t* center_frame_ptr, int num_frames,
-                             int64_t num_centers, int32_t* out_row_ptr, int64_t* out_num_edges_host, cudaStream_t s) {
-  Temp counts, tmp, total;
-  PG_CUDA_OK(counts.alloc(sizeof(int32_t) * (num_centers + 1), s));
-  PG_CUDA_OK(cudaMemsetAsync(counts.ptr, 0, sizeof(int32_t) * (num_centers + 1), s));
-  PG_CUDA_OK(total.alloc(sizeof(unsigned long long), s));
-  PG_CUDA_OK(cudaMemsetAsync(total.ptr, 0, sizeof(unsigned long long), s));
-  radius_query_kernel<false><<<ceil_div(num_centers * 32, 256), 256, 0, s>>>(
-      plan.grid.view, plan.spec, plan.grid.bounds.as<uint32_t>(), centers, center_frame_ptr, num_frames, num_centers,
-      nullptr, plan.r2, counts.as<int32_t>(), nullptr, nullptr, 0, plan.grid.err.as<int>(),
-      total.as<unsigned long long>());
-  PG_LAUNCH_CHECK();
-  size_t bytes = 0;
-  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, bytes, counts.as<int32_t>(), out_row_ptr, int(num_centers + 1), s));
-  PG_CUDA_OK(tmp.alloc(bytes, s));
-  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(tmp.ptr, bytes, counts.as<int32_t>(), out_row_ptr, int(num_centers + 1), s));
-  count_launch(2);
-  unsigned long long h_total = 0;   // the one host round trip of the graph build: E (64 bit) and the error word
-  int32_t h_err = 0;
-  PG_CUDA_OK(cudaMemcpyAsync(&h_total, total.ptr, sizeof(h_total), cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaMemcpyAsync(&h_err, plan.grid.err.ptr, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaStreamSynchronize(s));
-  if (int rc = graph_error(h_err)) return rc;
-  *out_num_edges_host = int64_t(h_total);
-  if (h_total > 0x7fffffffull) {    // row_ptr is int32 (the reference's int32 edge arrays, train.py:131)
-    set_error("radius graph has %llu edges: more than int32 row_ptr can index; split the batch", h_total);
-    return PG_ERR_RANGE;
-  }
-  return PG_OK;
-}
-
-static int radius_fill_impl(RadiusPlan& plan, const float* centers, const int32_t* center_frame_ptr, int num_frames,
-                            int64_t num_centers, const int32_t* row_ptr, int32_t* out_src, int32_t* out_dst,
-                            cudaStream_t s) {
-  radius_query_kernel<true><<<ceil_div(num_centers * 32, 256), 256, 0, s>>>(
-      plan.grid.view, plan.spec, plan.grid.bounds.as<uint32_t>(), centers, center_frame_ptr, num_frames, num_centers,
-      nullptr, plan.r2, nullptr, row_ptr, out_src, int64_t(1) << 40, nullptr, nullptr);
-  PG_LAUNCH_CHECK();
-  const int wblocks = int(std::min<int64_t>(ceil_div(num_centers, 8), int64_t(num_sms()) * 6));
-  Temp has_long;
-  PG_CUDA_OK(has_long.alloc(sizeof(int), s));
-  PG_CUDA_OK(cudaMemsetAsync(has_long.ptr, 0, sizeof(int), s));
-  sort_rows_warp_kernel<<<wblocks, 256, 0, s>>>(row_ptr, num_centers, out_src, out_dst, has_long.as<int>(),
-                                                int64_t(1) << 40);
-  PG_LAUNCH_CHECK();
-  // rows longer than kWarpRowMax (dense full-360 clouds): one block per row
-  const int blocks = int(std::min<int64_t>(num_centers, int64_t(num_sms()) * 4));
-  sort_rows_kernel<<<blocks, 256, kRowSortMax * sizeof(int32_t), s>>>(row_ptr, num_centers, out_src, out_dst,
-                                                                      has_long.as<int>(), int64_t(1) << 40);
-  PG_LAUNCH_CHECK();
-  return PG_OK;
+  // base.err is null when there is no base grid
+  return finish_keypoints(grid.view.cell_key, 48, grid.view.num_cells, num_frames, grid.err.as<int>(),
+                          base.err.as<int>(), capacity, "keypoint", out_kp_frame_ptr, out_num_keypoints_host, s);
 }
 
 extern "C" int pg_radius_graph_count(const float* points, const int32_t* point_frame_ptr, const float* centers,
@@ -956,7 +971,9 @@ extern "C" int pg_radius_graph_count(const float* points, const int32_t* point_f
   PG_REQUIRE(num_centers >= 1 && num_centers < (int64_t(1) << 31) - 1, "num_centers out of range");
   RadiusPlan plan;
   if (int rc = radius_prepare(points, point_frame_ptr, num_frames, num_points, radius, s, &plan)) return rc;
-  return radius_count_impl(plan, centers, center_frame_ptr, num_frames, num_centers, out_row_ptr, out_num_edges_host, s);
+  Temp ranges;
+  return radius_count_rows(plan, centers, center_frame_ptr, num_frames, num_centers, &ranges, out_row_ptr,
+                           out_num_edges_host, s);
 }
 
 extern "C" int pg_radius_graph_fill(const float* points, const int32_t* point_frame_ptr, const float* centers,
@@ -969,7 +986,9 @@ extern "C" int pg_radius_graph_fill(const float* points, const int32_t* point_fr
   if (num_edges == 0) return PG_OK;
   RadiusPlan plan;
   if (int rc = radius_prepare(points, point_frame_ptr, num_frames, num_points, radius, s, &plan)) return rc;
-  return radius_fill_impl(plan, centers, center_frame_ptr, num_frames, num_centers, row_ptr, out_src, out_dst, s);
+  Temp ranges;
+  if (int rc = radius_ranges(plan, centers, center_frame_ptr, num_frames, num_centers, &ranges, s)) return rc;
+  return radius_fill_rows(plan, centers, num_centers, ranges.as<int32_t>(), row_ptr, num_edges, out_src, out_dst, s);
 }
 
 extern "C" int pg_radius_graph(const float* points, const int32_t* point_frame_ptr, const float* centers,
@@ -991,7 +1010,8 @@ extern "C" int pg_radius_graph_scaled(const float* points, const int32_t* point_
   PG_REQUIRE(num_centers >= 1 && num_centers < (int64_t(1) << 31) - 1, "num_centers out of range");
   RadiusPlan plan;
   if (int rc = radius_prepare(points, point_frame_ptr, num_frames, num_points, radius, s, &plan, scale_host)) return rc;
-  if (int rc = radius_count_impl(plan, centers, center_frame_ptr, num_frames, num_centers, out_row_ptr,
+  Temp ranges;
+  if (int rc = radius_count_rows(plan, centers, center_frame_ptr, num_frames, num_centers, &ranges, out_row_ptr,
                                  out_num_edges_host, s))
     return rc;
   if (*out_num_edges_host > capacity) {
@@ -1000,54 +1020,8 @@ extern "C" int pg_radius_graph_scaled(const float* points, const int32_t* point_
   }
   if (*out_num_edges_host == 0) return PG_OK;
   PG_REQUIRE(out_src != nullptr, "pg_radius_graph: out_src is null");
-  return radius_fill_impl(plan, centers, center_frame_ptr, num_frames, num_centers, out_row_ptr, out_src, out_dst, s);
-}
-
-
-// One radius level of pg_multi_level_graph: count -> scan -> fill -> row sort, the number of centres and the number
-// of edges staying on the device (`num_centers_dev`; E = out_row_ptr[kp_capacity]).
-static int radius_level_device(RadiusPlan& plan, const float* centers, const int32_t* center_frame_ptr, int num_frames,
-                               int64_t kp_capacity, const int32_t* num_centers_dev, int32_t* out_row_ptr,
-                               int32_t* out_src, int32_t* out_dst, int64_t capacity, unsigned long long* total64,
-                               cudaStream_t s) {
-  // candidates per row are ~6.5x the hits (27 cells of edge r against the ball of radius r); the parking buffer is
-  // sized from the caller's edge capacity and its overflow is reported like an edge-buffer overflow
-  const int64_t tmp_capacity = std::min<int64_t>(capacity * 10 + 4096, (int64_t(1) << 31) - 1);
-  Temp counts, cand, cand_off, ranges, parked, tmp, has_long;
-  PG_CUDA_OK(counts.alloc(sizeof(int32_t) * (kp_capacity + 1), s));
-  PG_CUDA_OK(cudaMemsetAsync(counts.ptr, 0, sizeof(int32_t) * (kp_capacity + 1), s));
-  PG_CUDA_OK(cand.alloc(sizeof(int32_t) * (kp_capacity + 1), s));
-  PG_CUDA_OK(cand_off.alloc(sizeof(int32_t) * (kp_capacity + 1), s));
-  PG_CUDA_OK(ranges.alloc(sizeof(int32_t) * 18 * kp_capacity, s));
-  PG_CUDA_OK(parked.alloc(sizeof(int32_t) * tmp_capacity, s));
-  radius_candidates_kernel<<<ceil_div(kp_capacity + 1, 128), 128, 0, s>>>(
-      plan.grid.view, plan.spec, plan.grid.bounds.as<uint32_t>(), centers, center_frame_ptr, num_frames, kp_capacity,
-      num_centers_dev, ranges.as<int32_t>(), cand.as<int32_t>(), plan.grid.err.as<int>());
-  PG_LAUNCH_CHECK();
-  size_t bytes = 0;
-  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, bytes, cand.as<int32_t>(), cand_off.as<int32_t>(), int(kp_capacity + 1), s));
-  PG_CUDA_OK(tmp.alloc(bytes, s));
-  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(tmp.ptr, bytes, cand.as<int32_t>(), cand_off.as<int32_t>(), int(kp_capacity + 1), s));
-  count_launch(2);
-  radius_collect_kernel<<<ceil_div(kp_capacity * 32, 256), 256, 0, s>>>(
-      plan.grid.view, centers, kp_capacity, num_centers_dev, plan.r2, ranges.as<int32_t>(), cand_off.as<int32_t>(),
-      tmp_capacity, parked.as<int32_t>(), counts.as<int32_t>(), total64, plan.grid.err.as<int>());
-  PG_LAUNCH_CHECK();
-  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(tmp.ptr, bytes, counts.as<int32_t>(), out_row_ptr, int(kp_capacity + 1), s));
-  count_launch(2);
-  // rows beyond the real number of centres are empty, so row_ptr[c] == E for every c >= K
-  PG_CUDA_OK(has_long.alloc(sizeof(int), s));
-  PG_CUDA_OK(cudaMemsetAsync(has_long.ptr, 0, sizeof(int), s));
-  const int wblocks = int(std::min<int64_t>(ceil_div(kp_capacity, 8), int64_t(num_sms()) * 6));
-  sort_rows_warp_kernel<<<wblocks, 256, 0, s>>>(out_row_ptr, kp_capacity, out_src, out_dst, has_long.as<int>(), capacity,
-                                                parked.as<int32_t>(), cand_off.as<int32_t>());
-  PG_LAUNCH_CHECK();
-  const int blocks = int(std::min<int64_t>(kp_capacity, int64_t(num_sms()) * 4));
-  sort_rows_kernel<<<blocks, 256, kRowSortMax * sizeof(int32_t), s>>>(out_row_ptr, kp_capacity, out_src, out_dst,
-                                                                      has_long.as<int>(), capacity, parked.as<int32_t>(),
-                                                                      cand_off.as<int32_t>());
-  PG_LAUNCH_CHECK();
-  return PG_OK;
+  return radius_fill_rows(plan, centers, num_centers, ranges.as<int32_t>(), out_row_ptr, *out_num_edges_host, out_src,
+                          out_dst, s);
 }
 
 extern "C" int pg_multi_level_graph(const float* xyz, const int32_t* frame_ptr, int32_t num_frames, int64_t num_points,
@@ -1063,20 +1037,16 @@ extern "C" int pg_multi_level_graph(const float* xyz, const int32_t* frame_ptr, 
   PG_REQUIRE(out_src0 && out_dst0 && out_src1 && out_dst1 && capacity0 >= 1 && capacity1 >= 1,
              "pg_multi_level_graph: edge buffers are required");
   PG_REQUIRE(kp_capacity >= 1 && kp_capacity <= num_points, "pg_multi_level_graph: keypoint capacity out of range");
-  PG_REQUIRE(voxel_size_host[0] > 0 && voxel_size_host[1] > 0 && voxel_size_host[2] > 0, "voxel size must be positive");
   // ---- keypoints (multi_layer_downsampling_select, graph_gen.py:49-90) ---------------------------
-  GridSpec vspec{};
-  vspec.cell[0] = voxel_size_host[0];
-  vspec.cell[1] = voxel_size_host[1];
-  vspec.cell[2] = voxel_size_host[2];
-  vspec.origin_off = 0.5;
+  GridSpec vspec;
+  if (int rc = voxel_spec(voxel_size_host, CellRule::kVoxel, &vspec)) return rc;
   BuiltGrid vgrid;
   if (int rc = build_grid(xyz, frame_ptr, num_frames, num_points, vspec, s, &vgrid)) return rc;
   voxel_keypoint_kernel<<<ceil_div(num_points, 128), 128, 0, s>>>(vgrid.view, vspec, vgrid.bounds.as<uint32_t>(),
                                                                     out_keypoint_idx, kp_capacity);
   PG_LAUNCH_CHECK();
   frame_ranges_kernel<<<ceil_div(num_frames + 1, 128), 128, 0, s>>>(vgrid.view.cell_key, vgrid.view.num_cells, num_frames,
-                                                                     out_kp_frame_ptr);
+                                                                     48, out_kp_frame_ptr);
   PG_LAUNCH_CHECK();
   const int32_t* k_dev = vgrid.view.num_cells;      // K = number of occupied voxels, on the device
   gather_keypoints_kernel<<<ceil_div(kp_capacity, 256), 256, 0, s>>>(xyz, out_keypoint_idx, k_dev, kp_capacity, out_kp_xyz);
@@ -1092,11 +1062,8 @@ extern "C" int pg_multi_level_graph(const float* xyz, const int32_t* frame_ptr, 
     return rc;
   // ---- level 1: keypoints -> keypoints (same scale: graph_gen.py:76-81 makes level 2 = level 1) ------
   RadiusPlan plan1;
-  PG_REQUIRE(radius1 > 0.0, "radius must be positive");
-  plan1.spec.cell[0] = plan1.spec.cell[1] = plan1.spec.cell[2] = radius1 * kCellSlack;
-  plan1.spec.origin_off = 0.0;
-  plan1.r2 = radius1 * radius1;
-  if (int rc = build_grid(out_kp_xyz, out_kp_frame_ptr, num_frames, kp_capacity, plan1.spec, s, &plan1.grid, k_dev)) return rc;
+  if (int rc = radius_prepare(out_kp_xyz, out_kp_frame_ptr, num_frames, kp_capacity, radius1, s, &plan1, nullptr, k_dev))
+    return rc;
   if (int rc = radius_level_device(plan1, out_kp_xyz, out_kp_frame_ptr, num_frames, kp_capacity, k_dev, out_row_ptr1,
                                    out_src1, out_dst1, capacity1, totals.as<unsigned long long>() + 1, s))
     return rc;
@@ -1142,69 +1109,6 @@ extern "C" int pg_multi_level_graph(const float* xyz, const int32_t* frame_ptr, 
 namespace pg {
 namespace {
 
-// NumPy's floor_divide for floats (npy_floor_divide / npy_divmod): Python semantics
-template <typename T>
-__device__ inline T np_floor_divide(T a, T b) {
-  T mod = fmod(a, b);
-  T div = (a - mod) / b;
-  if (mod != T(0) && ((b < T(0)) != (mod < T(0)))) div -= T(1);
-  if (div != T(0)) {
-    T fl = floor(div);
-    if (div - fl > T(0.5)) fl += T(1);
-    return fl;
-  }
-  return copysign(T(0), a / b);
-}
-
-__device__ void shifted_cell_of(const GridSpec& g, const uint32_t* __restrict__ bounds, int f, float x, float y, float z,
-                                long long* ix, long long* iy, long long* iz) {
-  const float p[3] = {x, y, z};
-  long long idx[3];
-  for (int a = 0; a < 3; ++a) {
-    const float d = __fsub_rn(p[a], ordered_to_float(bounds[3 * f + a]));            // float32, as points_xyz - xyz_offset
-    const double t = __dadd_rn(double(d), __dmul_rn(g.cell[a], g.shift[3 * f + a]));
-    idx[a] = (long long)np_floor_divide<double>(t, g.cell[a]);
-  }
-  *ix = idx[0];
-  *iy = idx[1];
-  *iz = idx[2];
-}
-
-// graph_gen.py:124-131 voxel index of every point; shift == nullptr: float32 arithmetic (add_rnd3d False),
-// else float64 with the per-frame random shift fractions (add_rnd3d True)
-__global__ void random_voxel_keys_kernel(const float* __restrict__ xyz, const int32_t* __restrict__ frame_ptr, int num_frames,
-                                         int64_t n, double vx, double vy, double vz, const double* __restrict__ shift,
-                                         const uint32_t* __restrict__ bounds, uint64_t* __restrict__ keys,
-                                         int32_t* __restrict__ vals, int* __restrict__ err) {
-  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  if (i == 0 && (frame_ptr[0] != 0 || int64_t(frame_ptr[num_frames]) != n)) atomicOr(err, kErrFramePtr);
-  const int f = find_frame(frame_ptr, num_frames, i);
-  const float mn[3] = {ordered_to_float(bounds[3 * f]), ordered_to_float(bounds[3 * f + 1]), ordered_to_float(bounds[3 * f + 2])};
-  const double v[3] = {vx, vy, vz};
-  long long idx[3];
-  for (int a = 0; a < 3; ++a) {
-    const float d = __fsub_rn(xyz[3 * i + a], mn[a]);
-    if (shift == nullptr) {
-      idx[a] = (long long)np_floor_divide<float>(d, float(v[a]));
-    } else {
-      const double t = __dadd_rn(double(d), __dmul_rn(v[a], shift[3 * f + a]));
-      idx[a] = (long long)np_floor_divide<double>(t, v[a]);
-    }
-    if (idx[a] < 0 || idx[a] > kAxisMax) {
-      atomicOr(err, kErrRange);
-      idx[a] = 0;
-    }
-  }
-  keys[i] = make_key(uint32_t(f), uint32_t(idx[2]), uint32_t(idx[1]), uint32_t(idx[0]));
-  vals[i] = int32_t(i);
-}
-
-__global__ void head_flags_kernel(const uint64_t* __restrict__ keys, int64_t n, int32_t* __restrict__ head) {
-  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i < n) head[i] = (i == 0 || keys[i] != keys[i - 1]) ? 1 : 0;
-}
-
 // second sort key of every voxel: (frame, smallest original point index) = dict insertion order of graph_gen.py:133-139
 __global__ void voxel_first_keys_kernel(const uint64_t* __restrict__ cell_key, const int32_t* __restrict__ cell_start,
                                         const int32_t* __restrict__ sorted_idx, const int32_t* __restrict__ num_cells,
@@ -1226,13 +1130,6 @@ __global__ void random_pick_kernel(const int32_t* __restrict__ order, const int3
   int pick = int(uniform[o] * float(cnt));          // random.choice(seq) = seq[floor(u * len)], u in [0, 1)
   pick = min(max(pick, 0), cnt - 1);
   out_idx[o] = sorted_idx[s + pick];
-}
-
-__global__ void random_frame_ranges_kernel(const uint64_t* __restrict__ keys2_sorted, const int32_t* __restrict__ num_cells,
-                                           int num_frames, int32_t* __restrict__ out_frame_ptr) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  if (f > num_frames) return;
-  out_frame_ptr[f] = lower_bound_u64(keys2_sorted, *num_cells, uint64_t(f) << 32);
 }
 
 // ---- random neighbour cap ------------------------------------------------------------------------
@@ -1315,85 +1212,38 @@ extern "C" int pg_random_keypoints(const float* xyz, const int32_t* frame_ptr, i
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   PG_REQUIRE(xyz && frame_ptr && voxel_size_host && uniform && out_keypoint_idx && out_kp_frame_ptr && out_num_keypoints_host,
              "pg_random_keypoints: null argument");
-  PG_REQUIRE(voxel_size_host[0] > 0 && voxel_size_host[1] > 0 && voxel_size_host[2] > 0, "voxel size must be positive");
-  PG_REQUIRE(num_frames >= 1 && num_frames <= 65534, "num_frames=%d out of range [1,65534]", num_frames);
+  GridSpec spec;
+  if (int rc = voxel_spec(voxel_size_host, shift_host ? CellRule::kNumpyF64Shift : CellRule::kNumpyF32, &spec)) return rc;
+  Temp shift;
+  if (shift_host != nullptr)
+    if (int rc = upload_shift(shift_host, num_frames, s, &shift, &spec)) return rc;
+  BuiltGrid grid;
+  if (int rc = build_grid(xyz, frame_ptr, num_frames, num_points, spec, s, &grid)) return rc;
+  // second sort: the voxels in order of first appearance
   const int64_t n = num_points;
-  PG_REQUIRE(n >= 1 && n < (int64_t(1) << 31), "num_points=%lld out of range", (long long)n);
-  Temp bounds, keys_a, keys_b, vals_a, vals_b, head, head_scan, cell_key, cell_start, keys2a, keys2b, vals2a, vals2b, tmp, err,
-      shift;
-  PG_CUDA_OK(bounds.alloc(sizeof(uint32_t) * 3 * num_frames, s));
-  PG_CUDA_OK(keys_a.alloc(sizeof(uint64_t) * n, s));
-  PG_CUDA_OK(keys_b.alloc(sizeof(uint64_t) * n, s));
-  PG_CUDA_OK(vals_a.alloc(sizeof(int32_t) * n, s));
-  PG_CUDA_OK(vals_b.alloc(sizeof(int32_t) * n, s));
-  PG_CUDA_OK(head.alloc(sizeof(int32_t) * n, s));
-  PG_CUDA_OK(head_scan.alloc(sizeof(int32_t) * n, s));
-  PG_CUDA_OK(cell_key.alloc(sizeof(uint64_t) * n, s));
-  PG_CUDA_OK(cell_start.alloc(sizeof(int32_t) * (n + 1), s));
+  Temp keys2a, keys2b, vals2a, vals2b, tmp;
   PG_CUDA_OK(keys2a.alloc(sizeof(uint64_t) * n, s));
   PG_CUDA_OK(keys2b.alloc(sizeof(uint64_t) * n, s));
   PG_CUDA_OK(vals2a.alloc(sizeof(int32_t) * n, s));
   PG_CUDA_OK(vals2b.alloc(sizeof(int32_t) * n, s));
-  PG_CUDA_OK(err.alloc(sizeof(int), s));
-  PG_CUDA_OK(cudaMemsetAsync(err.ptr, 0, sizeof(int), s));
-  const double* shift_dev = nullptr;
-  if (shift_host != nullptr) {
-    PG_CUDA_OK(shift.alloc(sizeof(double) * 3 * num_frames, s));
-    PG_CUDA_OK(cudaMemcpyAsync(shift.ptr, shift_host, sizeof(double) * 3 * num_frames, cudaMemcpyHostToDevice, s));
-    shift_dev = shift.as<double>();
-  }
-  init_bounds_kernel<<<ceil_div(3 * num_frames, 256), 256, 0, s>>>(bounds.as<uint32_t>(), 3 * num_frames);
+  const int end_bit = 32 + frame_bits(num_frames);
+  size_t bytes = 0;
+  PG_CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, bytes, keys2a.as<uint64_t>(), keys2b.as<uint64_t>(), vals2a.as<int32_t>(),
+                                             vals2b.as<int32_t>(), int(n), 0, end_bit, s));
+  PG_CUDA_OK(tmp.alloc(bytes, s));
+  const int32_t* sorted_idx = grid.vals_b.as<int32_t>();
+  voxel_first_keys_kernel<<<ceil_div(n, 256), 256, 0, s>>>(grid.view.cell_key, grid.view.cell_start, sorted_idx,
+                                                            grid.view.num_cells, n, num_frames, keys2a.as<uint64_t>(),
+                                                            vals2a.as<int32_t>());
   PG_LAUNCH_CHECK();
-  const int blocks_per_frame = int(std::min<int64_t>(std::max<int64_t>(1, ceil_div(n / num_frames, 1024)), 64));
-  frame_min_kernel<<<dim3(blocks_per_frame, num_frames), 256, 0, s>>>(xyz, frame_ptr, n, bounds.as<uint32_t>());
-  PG_LAUNCH_CHECK();
-  random_voxel_keys_kernel<<<ceil_div(n, 256), 256, 0, s>>>(xyz, frame_ptr, num_frames, n, voxel_size_host[0], voxel_size_host[1],
-                                                            voxel_size_host[2], shift_dev, bounds.as<uint32_t>(),
-                                                            keys_a.as<uint64_t>(), vals_a.as<int32_t>(), err.as<int>());
-  PG_LAUNCH_CHECK();
-  int frame_bits = 1;
-  while ((1 << frame_bits) < num_frames + 1) ++frame_bits;
-  size_t b1 = 0, b2 = 0, b3 = 0;
-  PG_CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, b1, keys_a.as<uint64_t>(), keys_b.as<uint64_t>(), vals_a.as<int32_t>(),
-                                             vals_b.as<int32_t>(), int(n), 0, 48 + frame_bits, s));
-  PG_CUDA_OK(cub::DeviceScan::InclusiveSum(nullptr, b2, head.as<int32_t>(), head_scan.as<int32_t>(), int(n), s));
-  PG_CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, b3, keys2a.as<uint64_t>(), keys2b.as<uint64_t>(), vals2a.as<int32_t>(),
-                                             vals2b.as<int32_t>(), int(n), 0, 32 + frame_bits, s));
-  PG_CUDA_OK(tmp.alloc(std::max(b1, std::max(b2, b3)), s));
-  PG_CUDA_OK(cub::DeviceRadixSort::SortPairs(tmp.ptr, b1, keys_a.as<uint64_t>(), keys_b.as<uint64_t>(), vals_a.as<int32_t>(),
-                                             vals_b.as<int32_t>(), int(n), 0, 48 + frame_bits, s));
+  PG_CUDA_OK(cub::DeviceRadixSort::SortPairs(tmp.ptr, bytes, keys2a.as<uint64_t>(), keys2b.as<uint64_t>(), vals2a.as<int32_t>(),
+                                             vals2b.as<int32_t>(), int(n), 0, end_bit, s));
   count_launch(4);
-  head_flags_kernel<<<ceil_div(n, 256), 256, 0, s>>>(keys_b.as<uint64_t>(), n, head.as<int32_t>());
+  random_pick_kernel<<<ceil_div(n, 256), 256, 0, s>>>(vals2b.as<int32_t>(), grid.view.cell_start, sorted_idx,
+                                                       grid.view.num_cells, uniform, capacity, out_keypoint_idx);
   PG_LAUNCH_CHECK();
-  PG_CUDA_OK(cub::DeviceScan::InclusiveSum(tmp.ptr, b2, head.as<int32_t>(), head_scan.as<int32_t>(), int(n), s));
-  count_launch(2);
-  cell_table_kernel<<<ceil_div(n, 256), 256, 0, s>>>(keys_b.as<uint64_t>(), head_scan.as<int32_t>(), n, cell_key.as<uint64_t>(),
-                                                      cell_start.as<int32_t>());
-  PG_LAUNCH_CHECK();
-  const int32_t* num_cells = head_scan.as<int32_t>() + (n - 1);
-  voxel_first_keys_kernel<<<ceil_div(n, 256), 256, 0, s>>>(cell_key.as<uint64_t>(), cell_start.as<int32_t>(), vals_b.as<int32_t>(),
-                                                            num_cells, n, num_frames, keys2a.as<uint64_t>(), vals2a.as<int32_t>());
-  PG_LAUNCH_CHECK();
-  PG_CUDA_OK(cub::DeviceRadixSort::SortPairs(tmp.ptr, b3, keys2a.as<uint64_t>(), keys2b.as<uint64_t>(), vals2a.as<int32_t>(),
-                                             vals2b.as<int32_t>(), int(n), 0, 32 + frame_bits, s));
-  count_launch(4);
-  random_pick_kernel<<<ceil_div(n, 256), 256, 0, s>>>(vals2b.as<int32_t>(), cell_start.as<int32_t>(), vals_b.as<int32_t>(),
-                                                       num_cells, uniform, capacity, out_keypoint_idx);
-  PG_LAUNCH_CHECK();
-  random_frame_ranges_kernel<<<ceil_div(num_frames + 1, 128), 128, 0, s>>>(keys2b.as<uint64_t>(), num_cells, num_frames,
-                                                                            out_kp_frame_ptr);
-  PG_LAUNCH_CHECK();
-  int32_t h[2] = {0, 0};
-  PG_CUDA_OK(cudaMemcpyAsync(&h[0], num_cells, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaMemcpyAsync(&h[1], err.ptr, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaStreamSynchronize(s));
-  if (int rc = graph_error(h[1])) return rc;
-  *out_num_keypoints_host = h[0];
-  if (h[0] > capacity) {
-    set_error("keypoint buffer too small: need %d, capacity %lld", h[0], (long long)capacity);
-    return PG_ERR_CAPACITY;
-  }
-  return PG_OK;
+  return finish_keypoints(keys2b.as<uint64_t>(), 32, grid.view.num_cells, num_frames, grid.err.as<int>(), nullptr,
+                          capacity, "keypoint", out_kp_frame_ptr, out_num_keypoints_host, s);
 }
 
 extern "C" int pg_cap_neighbors(const int32_t* row_ptr, const int32_t* src, int64_t num_rows, int32_t num_neighbors,

@@ -277,3 +277,93 @@ def test_rnd3d_centroid_downsampling_vs_reference_golden():
     co, kpi, ed = graph_gen.gen_multi_level_local_graph_v3(xyz, 0.8, cfg, add_rnd3d=True)
     want_e = graph.gen_disjointed_rnn_local_graph_v3(co[0], co[1], 1.0, -1)
     assert np.array_equal(ed[0], want_e) and np.array_equal(co[1], xyz[kpi[0][:, 0]])
+
+
+def test_random_keypoints_vs_reference_golden():
+    """The training-time keypoints (graph_gen.py:92-153) fed the random numbers recorded in tests/golden/graph_random.npz
+    (the reference's own function with its generators patched to them): same voxels, first-appearance order, same
+    member, with the float32 voxel rule and with the shifted float64 one (add_rnd3d)."""
+    import os
+    from pointgnn_b200.models import graph_gen
+    g = np.load(os.path.join(os.path.dirname(__file__), 'golden', 'graph_random.npz'))
+    cloud = graph_gen._Cloud(torch.from_numpy(g['xyz']).cuda())
+    for tag, add in (('plain', False), ('rnd3d', True)):
+        u = torch.from_numpy(g['u_' + tag]).cuda()
+        coords, kp, fps = graph_gen._downsampling_random(cloud, 0.8, [1, 1], add, uniform=[u, None],
+                                                         shifts=[g['shift_' + tag], None])
+        want = g['kp_' + tag]
+        assert np.array_equal(_np(kp[0][:, 0]), want), tag
+        assert np.array_equal(_np(coords[1]), g['xyz'][want]), tag
+        assert _np(fps[1]).tolist() == [0, len(want)], tag
+        assert np.array_equal(_np(kp[1][:, 0]), np.arange(len(want))), tag
+
+
+def test_neighbor_cap_invariants_and_seed(car):
+    """The random neighbour cap (graph_gen.py:210-214) on a real level-0 radius graph: rows of at most num_neighbors
+    entries unchanged, longer rows exactly num_neighbors distinct true neighbours; the same seed gives the same edges."""
+    from pointgnn_b200.models import graph_gen
+    xyz, _ = synth.lidar_frame(17, 8000)
+    t = torch.from_numpy(xyz).cuda()
+    coords, _, _, fps = graph_gen.gen_multi_level_local_graph_v3(t, return_frame_ptr=True, **car.graph_kwargs)
+    r0 = car.graph_kwargs['level_configs'][0]['graph_gen_kwargs']['radius']
+    full = graph_gen._radius_edges(t, fps[0], coords[1], fps[1], r0, -1)
+    capped = graph_gen._radius_edges(t, fps[0], coords[1], fps[1], r0, 8, cap_seed=1234)
+    again = graph_gen._radius_edges(t, fps[0], coords[1], fps[1], r0, 8, cap_seed=1234)
+    full_np, capped_np = _np(full).astype(np.int64), _np(capped).astype(np.int64)
+    assert np.array_equal(full_np, graph.radius_graph(xyz, _np(coords[1]), r0))
+    assert graph.check_neighbor_cap(full_np, capped_np, 8) > 0
+    assert np.array_equal(_np(again), _np(capped))
+
+
+def test_radius_graph_capacity_contract():
+    """pg_radius_graph with an edge buffer that is too small: PG_ERR_CAPACITY, the exact E, and a valid row_ptr."""
+    import ctypes
+    from pointgnn_b200 import _lib
+    lib = _lib.load()
+    xyz, _ = synth.lidar_frame(12, 4000)
+    pts = torch.from_numpy(xyz).cuda()
+    ctr = pts[::5].contiguous()
+    fp = torch.tensor([0, pts.shape[0]], dtype=torch.int32, device='cuda')
+    cfp = torch.tensor([0, ctr.shape[0]], dtype=torch.int32, device='cuda')
+    row_ptr, edges = _lib.radius_graph(pts, fp, ctr, cfp, 1.0)
+    assert np.array_equal(_np(edges.t()).astype(np.int64), graph.radius_graph(xyz, xyz[::5], 1.0))
+    rp = torch.full_like(row_ptr, -1)
+    buf = torch.empty((2, 1), dtype=torch.int32, device='cuda')
+    e = ctypes.c_int64(0)
+    code = lib.pg_radius_graph(ctypes.c_void_p(pts.data_ptr()), ctypes.c_void_p(fp.data_ptr()),
+                               ctypes.c_void_p(ctr.data_ptr()), ctypes.c_void_p(cfp.data_ptr()), 1, pts.shape[0],
+                               ctr.shape[0], 1.0, ctypes.c_void_p(rp.data_ptr()), ctypes.c_void_p(buf[0].data_ptr()),
+                               ctypes.c_void_p(buf[1].data_ptr()), 1, ctypes.byref(e), _lib._stream())
+    assert code == _lib.PG_ERR_CAPACITY
+    assert e.value == edges.shape[1] > 1
+    assert torch.equal(rp, row_ptr)
+
+
+def test_multi_level_graph_capacity_retry(car):
+    """_lib.multi_level_graph started with a keypoint buffer below K, then with edge buffers below E0 / E1: the retry
+    loop must end with the result of a fresh call, which equals the oracle."""
+    from pointgnn_b200 import _lib
+    from pointgnn_b200.models import graph_gen
+    xyz, _ = synth.lidar_frame(13, 6000)
+    t = torch.from_numpy(xyz).cuda()
+    fp = torch.tensor([0, xyz.shape[0]], dtype=torch.int32, device='cuda')
+    kw = car.graph_kwargs
+    voxel = graph_gen._voxel_vector(kw['base_voxel_size'], kw['level_configs'][0]['graph_scale'])
+    r0, r1 = (c['graph_gen_kwargs']['radius'] for c in kw['level_configs'])
+    key = (t.device.index, int(xyz.shape[0]), tuple(float(v) for v in voxel), float(r0), float(r1))
+    _lib._graph_capacity.pop(key, None)
+    fresh = _lib.multi_level_graph(t, fp, voxel, r0, r1)
+    k, e0, e1 = fresh[0].numel(), fresh[3].shape[1], fresh[4].shape[1]
+    _, kp_o, edges_o = graph.gen_multi_level_local_graph_v3(xyz, **kw)
+    assert np.array_equal(_np(fresh[0]), kp_o[0][:, 0])
+    assert np.array_equal(_np(fresh[3].t()).astype(np.int64), edges_o[0])
+    assert np.array_equal(_np(fresh[4].t()).astype(np.int64), edges_o[1])
+    n = xyz.shape[0]
+    try:
+        for caps in ((k // 2, 32 * n, 48 * n), (k, e0 // 2, e1), (k, e0, e1 // 2)):
+            _lib._graph_capacity[key] = caps
+            got = _lib.multi_level_graph(t, fp, voxel, r0, r1)
+            for a, b in zip(got, fresh):
+                assert torch.equal(a, b), caps
+    finally:
+        _lib._graph_capacity.pop(key, None)

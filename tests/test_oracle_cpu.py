@@ -233,3 +233,17 @@ def test_oracle_rnd3d_centroids_match_reference_golden():
         assert np.array_equal(np.asarray(cents[i + 1], dtype=np.float64), g['centroids_%d' % (i + 1)])
         assert (kp[i][:, 0] == g['kp_%d' % i]).mean() > 0.97
     assert np.array_equal(kp[1][:, 0], np.arange(len(kp[0])))
+
+
+def test_oracle_random_downsampling_matches_reference_golden():
+    """multi_layer_downsampling_random (graph_gen.py:92-153) with its random sources given as arguments:
+    tests/golden/graph_random.npz is the reference's own function with np.random.random / random.choice patched to the
+    recorded numbers, with and without add_rnd3d."""
+    g = np.load(os.path.join(GOLDEN, 'graph_random.npz'))
+    for tag, add in (('plain', False), ('rnd3d', True)):
+        coords, kp = graph.multi_layer_downsampling_random(g['xyz'], 0.8, [1, 1], add_rnd3d=add,
+                                                           shifts=[g['shift_' + tag], None],
+                                                           uniforms=[g['u_' + tag], None])
+        assert np.array_equal(kp[0][:, 0], g['kp_' + tag]), tag
+        assert np.array_equal(coords[1], g['xyz'][g['kp_' + tag]]), tag
+        assert np.array_equal(kp[1][:, 0], np.arange(len(kp[0]))), tag
