@@ -404,17 +404,23 @@ def gather_rows(params, indices):
     return out
 
 
-def fully_connected(x, w, b, relu, residual=None, precision=0):
-    lib = load()
-    m, k = x.shape
-    if w.shape[0] != k:
-        raise ValueError('fully_connected: input width %d != weight rows %d' % (k, w.shape[0]))
-    n = w.shape[1]
-    if b.numel() != n:
-        raise ValueError('fully_connected: bias has %d entries, layer width is %d' % (b.numel(), n))
+def _check_fc_shapes(x, k, n, residual):
+    """x [m, k] into a layer chain of input width k and output width n; the optional residual must be [m, n]."""
+    m = x.shape[0]
+    if x.shape[1] != k:
+        raise ValueError('fully_connected: input width %d != weight rows %d' % (x.shape[1], k))
     if residual is not None and tuple(residual.shape) != (m, n):
         # the reference's tf add raises a shape error here (gnn.py:346, 372)
         raise ValueError('fully_connected: residual shape %s != output shape (%d, %d)' % (tuple(residual.shape), m, n))
+
+
+def fully_connected(x, w, b, relu, residual=None, precision=0):
+    lib = load()
+    m, k = x.shape
+    n = w.shape[1]
+    _check_fc_shapes(x, w.shape[0], n, residual)
+    if b.numel() != n:
+        raise ValueError('fully_connected: bias has %d entries, layer width is %d' % (b.numel(), n))
     out = torch.empty((m, n), dtype=torch.float32, device=x.device)
     _check(lib.pg_fully_connected(_ptr(x, torch.float32, 'x'), m, k, _ptr(w, torch.float32, 'w'),
                                   _ptr(b, torch.float32, 'b'), n, 1 if relu else 0,
@@ -485,13 +491,9 @@ class PreparedLayer(object):
 
     # multi_layer_neural_network_fn / multi_layer_fc_fn (gnn.py:34-104)
     def mlp(self, x, last_linear, residual=None):
-        m, k = x.shape
-        if k != self.dims[0]:
-            raise ValueError('fully_connected: input width %d != weight rows %d' % (k, self.dims[0]))
+        m, _ = x.shape
         n = self.dims[-1]
-        if residual is not None and tuple(residual.shape) != (m, n):
-            raise ValueError('fully_connected: residual shape %s != output shape (%d, %d)'
-                             % (tuple(residual.shape), m, n))
+        _check_fc_shapes(x, self.dims[0], n, residual)
         out = torch.empty((m, n), dtype=torch.float32, device=x.device)
         _check(load().pg_layer_mlp(self._handle, _ptr(x, torch.float32, 'x'), m, 1 if last_linear else 0,
                                    _ptr(residual, torch.float32, 'residual'), _ptr(out, torch.float32, 'out'),

@@ -16,9 +16,6 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
-static thread_local bool g_trusted = false;
-bool trusted_indices() { return g_trusted; }
-void set_trusted_indices(bool v) { g_trusted = v; }
 }  // namespace pg
 
 extern "C" {
@@ -33,6 +30,9 @@ int pg_device_is_sm90(void) {
   if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
   return major == 9 ? 1 : 0;
 }
+
+// the wgmma kernels are always built in, so the device decides
+int pg_tc_available(void) { return pg_device_is_sm90(); }
 
 int64_t pg_launch_count(void) { return pg::g_launches.load(std::memory_order_relaxed); }
 

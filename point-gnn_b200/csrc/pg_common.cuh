@@ -1,4 +1,5 @@
-// Shared helpers for libpointgnn_b200 (error plumbing, launch accounting, temp buffers).
+// Shared helpers for libpointgnn_b200 (error plumbing, launch accounting, temp buffers) and the internal functions
+// one source file calls in another.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -11,9 +12,6 @@ namespace pg {
 
 void set_error(const char* fmt, ...);
 void count_launch(int n = 1);
-// true while the current C-ABI call carries PG_FLAG_TRUSTED_INDICES (no range-error read-back, no sync)
-bool trusted_indices();
-void set_trusted_indices(bool v);
 
 #define PG_CUDA_OK(expr)                                                              \
   do {                                                                                \
@@ -71,6 +69,47 @@ struct Temp {
     if (ptr) cudaFreeAsync(ptr, stream);
   }
 };
+
+// Device word a kernel sets to nonzero when it meets an out-of-range index: allocated and zeroed on the stream;
+// read() returns its value after the stream's work.  trusted (PG_FLAG_TRUSTED_INDICES: the caller guarantees the
+// ranges) skips the read-back and the synchronisation and reports 0.
+struct ErrorWord {
+  Temp word;
+  int init(cudaStream_t s) {
+    PG_CUDA_OK(word.alloc(sizeof(int), s));
+    PG_CUDA_OK(cudaMemsetAsync(word.ptr, 0, sizeof(int), s));
+    return PG_OK;
+  }
+  int* ptr() const { return word.as<int>(); }
+  int read(int* value, bool trusted, cudaStream_t s) const {
+    *value = 0;
+    if (trusted) return PG_OK;
+    PG_CUDA_OK(cudaMemcpyAsync(value, word.ptr, sizeof(int), cudaMemcpyDeviceToHost, s));
+    PG_CUDA_OK(cudaStreamSynchronize(s));
+    return PG_OK;
+  }
+};
+
+// max(float) through integer atomics: valid for any finite values and any initial value.
+__device__ __forceinline__ void atomic_max_float(float* addr, float v) {
+  v += 0.0f;  // canonicalise -0.0f
+  if (v >= 0.0f)
+    atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
+  else
+    atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(v));
+}
+
+// pg_ops.cu
+int fill_async(float* p, int64_t n, float v, cudaStream_t s);
+// out [m, ldo] = act(x [m, k] @ w [k, n] + bias) (+ residual [m, n]); columns [n, ldo) are written as zeros
+int fc_fp32_launch(const float* x, int64_t m, int k, const float* w, const float* bias, int n, int act,
+                   const float* residual, float* out, int ldo, cudaStream_t s);
+// pg_edge_simt.cu: the fp32 FFMA edge MLP + segment max into out (already filled with -FLT_MAX); sets *err on an
+// out-of-range src / dst
+int edge_mlp_max_fp32(int mode, const float* features, int c_in, const float* xyz_src, const float* xyz_dst,
+                      const int32_t* dst_index, const int32_t* src, const int32_t* dst, int64_t num_edges,
+                      int64_t num_src, int64_t num_dst, const float* const* weights, const float* const* biases,
+                      const int32_t* dims, int num_layers, float* out, int* err, cudaStream_t s);
 
 inline int num_sms() {
   static int sms = 0;

@@ -15,19 +15,7 @@
 #include "pg_common.cuh"
 
 namespace pg {
-
-
-int fill_async(float* p, int64_t n, float v, cudaStream_t s);
-
 namespace {
-
-__device__ __forceinline__ void atomic_max_f(float* addr, float v) {
-  v += 0.0f;
-  if (v >= 0.0f)
-    atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
-  else
-    atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(v));
-}
 
 constexpr int kMaxLayers = 8;
 constexpr int kTileE = 64;   // edges per tile
@@ -152,13 +140,13 @@ __global__ void __launch_bounds__(kThreads, 1) edge_mlp_max_fp32_kernel(EdgeMlpP
       for (int r = 0; r < rows; ++r) {
         const int d = s_dst[r];
         if (d != cur) {
-          if (cur >= 0) atomic_max_f(p.out + int64_t(cur) * n_out + c, m);
+          if (cur >= 0) atomic_max_float(p.out + int64_t(cur) * n_out + c, m);
           cur = d;
           m = -FLT_MAX;
         }
         m = fmaxf(m, fin[size_t(r) * fstride + c]);
       }
-      if (cur >= 0) atomic_max_f(p.out + int64_t(cur) * n_out + c, m);
+      if (cur >= 0) atomic_max_float(p.out + int64_t(cur) * n_out + c, m);
     }
   }
 }
@@ -168,7 +156,7 @@ __global__ void __launch_bounds__(kThreads, 1) edge_mlp_max_fp32_kernel(EdgeMlpP
 int edge_mlp_max_fp32(int mode, const float* features, int c_in, const float* xyz_src, const float* xyz_dst,
                       const int32_t* dst_index, const int32_t* src, const int32_t* dst, int64_t num_edges,
                       int64_t num_src, int64_t num_dst, const float* const* weights, const float* const* biases,
-                      const int32_t* dims, int num_layers, float* out, cudaStream_t s) {
+                      const int32_t* dims, int num_layers, float* out, int* err, cudaStream_t s) {
   PG_REQUIRE(num_layers >= 1 && num_layers <= kMaxLayers, "edge MLP depth %d not in [1,%d]", num_layers, kMaxLayers);
   PG_REQUIRE(dims[0] == c_in + 3, "dims[0]=%d must equal feature channels + 3 = %d", dims[0], c_in + 3);
   EdgeMlpParams p{};
@@ -198,13 +186,9 @@ int edge_mlp_max_fp32(int mode, const float* features, int c_in, const float* xy
   p.stride0 = w0 + 1;
   p.stride1 = w1 + 1;
   p.out = out;
+  p.err = err;
   const size_t smem = size_t(kTileE) * (p.stride0 + p.stride1) * sizeof(float);
   PG_REQUIRE(smem <= 227 * 1024 - 1024, "edge MLP widths need %zu B of shared memory (> 226 KB)", smem);
-  Temp err;
-  PG_CUDA_OK(err.alloc(sizeof(int), s));
-  PG_CUDA_OK(cudaMemsetAsync(err.ptr, 0, sizeof(int), s));
-  p.err = err.as<int>();
-  if (int rc = fill_async(out, num_dst * dims[num_layers], -FLT_MAX, s)) return rc;
   if (num_edges > 0) {
     PG_CUDA_OK(cudaFuncSetAttribute(edge_mlp_max_fp32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
     const int64_t tiles = ceil_div(num_edges, kTileE);
@@ -212,47 +196,7 @@ int edge_mlp_max_fp32(int mode, const float* features, int c_in, const float* xy
     edge_mlp_max_fp32_kernel<<<grid, kThreads, smem, s>>>(p);
     PG_LAUNCH_CHECK();
   }
-  int h = 0;
-  if (!trusted_indices()) {   // PG_FLAG_TRUSTED_INDICES: no read-back, no synchronisation
-    PG_CUDA_OK(cudaMemcpyAsync(&h, err.ptr, sizeof(int), cudaMemcpyDeviceToHost, s));
-    PG_CUDA_OK(cudaStreamSynchronize(s));
-  }
-  PG_REQUIRE(h == 0, "edge index out of range (src in [0,%lld), dst in [0,%lld))", (long long)num_src,
-             (long long)num_dst);
   return PG_OK;
 }
 
-int edge_mlp_max_tc(int mode, const float* features, int c_in, const float* xyz_src, const float* xyz_dst,
-                    const int32_t* dst_index, const int32_t* src, const int32_t* dst, int64_t num_edges,
-                    int64_t num_src, int64_t num_dst, const float* const* weights, const float* const* biases,
-                    const int32_t* dims, int num_layers, float* out, cudaStream_t s);  // pg_tc.cu
-
 }  // namespace pg
-
-using namespace pg;
-
-extern "C" int pg_edge_mlp_max(int32_t mode, const float* features, int32_t num_feature_channels, const float* xyz_src,
-                               const float* xyz_dst, const int32_t* dst_index, const int32_t* src, const int32_t* dst,
-                               int64_t num_edges, int64_t num_src, int64_t num_dst, const float* const* weights_host,
-                               const float* const* biases_host, const int32_t* dims_host, int32_t num_layers, float* out,
-                               int32_t precision, void* stream) {
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  PG_REQUIRE(mode == PG_EDGE_POOL || mode == PG_EDGE_GNN, "pg_edge_mlp_max: unknown mode %d", mode);
-  PG_REQUIRE(weights_host && biases_host && dims_host, "pg_edge_mlp_max: null layer tables");
-  PG_REQUIRE(num_edges >= 0 && num_src >= 1 && num_dst >= 0, "pg_edge_mlp_max: bad sizes");
-  PG_REQUIRE(out != nullptr || num_dst == 0, "pg_edge_mlp_max: out is null");
-  PG_REQUIRE((features && xyz_src && xyz_dst && src && dst) || num_edges == 0, "pg_edge_mlp_max: null input");
-  PG_REQUIRE(mode == PG_EDGE_GNN || dst_index != nullptr || num_edges == 0,
-             "pg_edge_mlp_max: POOL mode needs keypoint indices");
-  struct TrustedScope {
-    explicit TrustedScope(bool v) { pg::set_trusted_indices(v); }
-    ~TrustedScope() { pg::set_trusted_indices(false); }
-  } scope((precision & PG_FLAG_TRUSTED_INDICES) != 0);
-  precision &= PG_PRECISION_MASK;
-  if (precision == 1)
-    return edge_mlp_max_tc(mode, features, num_feature_channels, xyz_src, xyz_dst, dst_index, src, dst, num_edges,
-                           num_src, num_dst, weights_host, biases_host, dims_host, num_layers, out, s);
-  PG_REQUIRE(precision == 0, "pg_edge_mlp_max: unknown precision %d", precision);
-  return edge_mlp_max_fp32(mode, features, num_feature_channels, xyz_src, xyz_dst, dst_index, src, dst, num_edges,
-                           num_src, num_dst, weights_host, biases_host, dims_host, num_layers, out, s);
-}

@@ -9,15 +9,6 @@
 
 namespace pg {
 
-// max(float) through integer atomics: valid for any finite values and any initial value.
-__device__ __forceinline__ void atomic_max_float(float* addr, float v) {
-  v += 0.0f;  // canonicalise -0.0f
-  if (v >= 0.0f)
-    atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
-  else
-    atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(v));
-}
-
 __global__ void fill_kernel(float* __restrict__ p, int64_t n, float v) {
   for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += int64_t(gridDim.x) * blockDim.x)
     p[i] = v;
@@ -264,9 +255,6 @@ int fc_fp32_launch(const float* x, int64_t m, int k, const float* w, const float
   return PG_OK;
 }
 
-int fc_tc_bf16x3(const float* x, int64_t m, int k, const float* w, const float* bias, int n, int act,
-                 const float* residual, float* out, cudaStream_t s);  // pg_tc.cu
-
 }  // namespace pg
 
 using namespace pg;
@@ -339,30 +327,16 @@ extern "C" int pg_gather_rows(const float* params, int64_t num_rows, int32_t num
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (num_indices == 0) return PG_OK;
   PG_REQUIRE(params && indices && out && num_channels >= 1, "pg_gather_rows: bad argument");
-  Temp err;
-  PG_CUDA_OK(err.alloc(sizeof(int), s));
-  PG_CUDA_OK(cudaMemsetAsync(err.ptr, 0, sizeof(int), s));
+  ErrorWord err;
+  if (int rc = err.init(s)) return rc;
   const int64_t total = num_indices * num_channels;
   const int blocks = int(std::min<int64_t>(ceil_div(total, 256), int64_t(num_sms()) * 16));
-  gather_rows_kernel<<<blocks, 256, 0, s>>>(params, num_rows, num_channels, indices, num_indices, out, err.as<int>());
+  gather_rows_kernel<<<blocks, 256, 0, s>>>(params, num_rows, num_channels, indices, num_indices, out, err.ptr());
   PG_LAUNCH_CHECK();
   int h = 0;
-  PG_CUDA_OK(cudaMemcpyAsync(&h, err.ptr, sizeof(int), cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaStreamSynchronize(s));
+  if (int rc = err.read(&h, false, s)) return rc;
   PG_REQUIRE(h == 0, "pg_gather_rows: index out of range [0,%lld)", (long long)num_rows);  // TF: InvalidArgumentError
   return PG_OK;
-}
-
-extern "C" int pg_fully_connected(const float* x, int64_t m, int32_t k, const float* w, const float* bias, int32_t n,
-                                  int32_t act, const float* residual, float* out, int32_t precision, void* stream) {
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  PG_REQUIRE(m >= 0 && k >= 1 && n >= 1, "pg_fully_connected: bad sizes m=%lld k=%d n=%d", (long long)m, k, n);
-  PG_REQUIRE(act == 0 || act == 1, "pg_fully_connected: act must be 0 (linear) or 1 (ReLU)");
-  if (m == 0) return PG_OK;
-  PG_REQUIRE(x && w && bias && out, "pg_fully_connected: null argument");
-  if (precision == 1) return fc_tc_bf16x3(x, m, k, w, bias, n, act, residual, out, s);
-  PG_REQUIRE(precision == 0, "pg_fully_connected: unknown precision %d", precision);
-  return fc_fp32_launch(x, m, k, w, bias, n, act, residual, out, n, s);
 }
 
 extern "C" int pg_check_edges(const int32_t* src, const int32_t* dst, int64_t num_edges, int64_t num_src,
@@ -370,15 +344,13 @@ extern "C" int pg_check_edges(const int32_t* src, const int32_t* dst, int64_t nu
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (num_edges == 0) return PG_OK;
   PG_REQUIRE(src && dst && num_edges > 0, "pg_check_edges: bad argument");
-  Temp err;
-  PG_CUDA_OK(err.alloc(sizeof(int), s));
-  PG_CUDA_OK(cudaMemsetAsync(err.ptr, 0, sizeof(int), s));
+  ErrorWord err;
+  if (int rc = err.init(s)) return rc;
   const int blocks = int(std::min<int64_t>(ceil_div(num_edges, 256), int64_t(num_sms()) * 8));
-  check_edges_kernel<<<blocks, 256, 0, s>>>(src, dst, num_edges, num_src, num_dst, err.as<int>());
+  check_edges_kernel<<<blocks, 256, 0, s>>>(src, dst, num_edges, num_src, num_dst, err.ptr());
   PG_LAUNCH_CHECK();
   int h = 0;
-  PG_CUDA_OK(cudaMemcpyAsync(&h, err.ptr, sizeof(int), cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaStreamSynchronize(s));
+  if (int rc = err.read(&h, false, s)) return rc;
   PG_REQUIRE(h == 0, "edge index out of range (src in [0,%lld), dst in [0,%lld))", (long long)num_src,
              (long long)num_dst);   // TF: InvalidArgumentError
   return PG_OK;

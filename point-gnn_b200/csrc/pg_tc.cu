@@ -28,17 +28,12 @@
 // for a 16-k chunk, core(row group g, k half kc) at g * 256 + kc * 128 (LBO = 128, SBO = 256).
 #include <atomic>
 #include <cstdlib>
+#include <memory>
+#include <utility>
 #include <vector>
 
 #include "pg_common.cuh"
 #include "pg_wgmma.cuh"
-
-extern "C" int pg_tc_available(void) {
-  int dev = 0, major = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
-  if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
-  return major == 9 ? 1 : 0;
-}
 
 namespace pg {
 static std::atomic<long long> g_tc_launches[2];   // [0] segment-max (edge) launches, [1] store (dense) launches
@@ -50,15 +45,6 @@ extern "C" int64_t pg_tc_launch_count(int32_t which) {
 }
 
 namespace pg {
-
-int fill_async(float* p, int64_t n, float v, cudaStream_t s);
-int fc_fp32_launch(const float* x, int64_t m, int k, const float* w, const float* bias, int n, int act,
-                   const float* residual, float* out, int ldo, cudaStream_t s);
-int edge_mlp_max_fp32(int mode, const float* features, int c_in, const float* xyz_src, const float* xyz_dst,
-                      const int32_t* dst_index, const int32_t* src, const int32_t* dst, int64_t num_edges,
-                      int64_t num_src, int64_t num_dst, const float* const* weights, const float* const* biases,
-                      const int32_t* dims, int num_layers, float* out, cudaStream_t s);
-
 namespace {
 using namespace wg;
 
@@ -380,7 +366,7 @@ WgShape wg_shape(int k, int n) {
   else if (t.np <= kMaxNT) { t.ni = 152; t.ns = 2; }
   t.nt = t.ni * t.ns;
   t.smem = size_t(kRing) * t.nt * 64 + 4 * kABytes + 2 * kRing * sizeof(uint64_t);
-  t.ok = pg_tc_available() && t.nt > 0 && k >= 1 && n >= 1;
+  t.ok = t.nt > 0 && k >= 1 && n >= 1;
   return t;
 }
 
@@ -453,9 +439,31 @@ std::vector<int> column_blocks(int n) {
 // =================================================================================================
 // Prepared layers.  Everything that depends only on the WEIGHTS is done once, when a layer is prepared:
 // the BF16 hi / lo operand images, padded biases, the hoisted first-layer matrices.  A forward pass then
-// launches compute kernels only.  The per-call entry points (pg_fully_connected, pg_edge_mlp_max) prepare
-// into stream-ordered temporaries and apply once; pg_layer_* keeps the prepared state in a handle.
+// launches compute kernels only.  pg_layer_* keeps the prepared state in a handle.  The per-call entry points
+// (pg_fully_connected, pg_edge_mlp_max) run a transient prepared layer: they prepare it on the stack (its
+// buffers are stream-ordered temporaries) and apply it once, so both forms share one dispatch path.  Whether an
+// edge call reads its range-error word back (PG_FLAG_TRUSTED_INDICES) is an argument of apply_edge.
 // =================================================================================================
+
+// W [k, n] with row stride ld as tensor-core GEMMs of at most kMaxNT output features, block b writing the columns
+// from col0[b]; only the first n_src columns of W are read, the pad columns past them get zero weights and bias
+int prepare_column_blocks(std::vector<PreparedGemm>& blocks, std::vector<int>& col0, const float* w, int ld,
+                          const float* bias, int k, int n_src, int n, cudaStream_t s) {
+  PG_REQUIRE(n >= 1, "no tensor-core shape for a %d x %d layer", k, n);
+  col0 = column_blocks(n);
+  blocks = std::vector<PreparedGemm>(col0.size());
+  for (size_t b = 0; b < col0.size(); ++b) {
+    const int wn = (b + 1 < col0.size() ? col0[b + 1] : n) - col0[b];
+    const int src_cols = std::max(0, std::min(wn, n_src - col0[b]));
+    PG_REQUIRE(src_cols > 0, "dense layer: column block beyond the weight matrix");
+    if (int rc = prepare_gemm(blocks[b], w + col0[b], ld, bias + col0[b], k, src_cols, s)) return rc;
+    blocks[b].n = wn;
+  }
+  return PG_OK;
+}
+
+// narrow / shallow layers (N < 8, K < 64: the 64->3, 64->4, 64->7 heads) stay on the fp32 FFMA kernel
+bool fc_uses_tc(int k, int n) { return (k & 3) == 0 && n >= 8 && (k + 15) / 16 * 16 >= 64; }
 
 // ---- one fully-connected layer -----------------------------------------------------------------
 struct PreparedFc {
@@ -479,21 +487,9 @@ int prepare_fc(PreparedFc& f, const float* w, int ld_src, const float* bias, int
   f.bias = bias;
   f.blocks.clear();
   f.col0.clear();
-  // narrow / shallow layers (N < 8, K < 64: the 64->3, 64->4, 64->7 heads) stay on the fp32 FFMA kernel
-  f.tc = want_tc && pg_tc_available() && (k & 3) == 0 && n >= 8 && (k + 15) / 16 * 16 >= 64;
+  f.tc = want_tc && fc_uses_tc(k, n);
   if (!f.tc) return PG_OK;
-  const std::vector<int> c0 = n <= kMaxNT ? std::vector<int>{0} : column_blocks(n);
-  f.blocks = std::vector<PreparedGemm>(c0.size());
-  for (size_t b = 0; b < c0.size(); ++b) {
-    const int wn = (b + 1 < c0.size() ? c0[b + 1] : n) - c0[b];
-    // the pad columns of a block past n_src get zero weights and bias
-    const int src_cols = std::max(0, std::min(wn, n_src - c0[b]));
-    PG_REQUIRE(src_cols > 0, "dense layer: column block beyond the weight matrix");
-    if (int rc = prepare_gemm(f.blocks[b], w + c0[b], ld_src, bias + c0[b], k, src_cols, s)) return rc;
-    f.blocks[b].n = wn;
-  }
-  f.col0 = c0;
-  return PG_OK;
+  return prepare_column_blocks(f.blocks, f.col0, w, ld_src, bias, k, n_src, n, s);
 }
 
 // out [m, ldo]: columns [0, n) = act(x @ W + b) (+ residual [m, n]); ldo >= n
@@ -540,17 +536,6 @@ struct PreparedEdge {
   int mid_width = 0;                  // widest stored per-edge activation (POOL)
 };
 
-int prepare_last(PreparedEdge& e, const float* w, const float* bias, int k, int n, cudaStream_t s) {
-  e.last_col0 = n <= kMaxNT ? std::vector<int>{0} : column_blocks(n);
-  e.last = std::vector<PreparedGemm>(e.last_col0.size());
-  for (size_t b = 0; b < e.last_col0.size(); ++b) {
-    const int c0 = e.last_col0[b];
-    const int wn = (b + 1 < e.last_col0.size() ? e.last_col0[b + 1] : n) - c0;
-    if (int rc = prepare_gemm(e.last[b], w + c0, n, bias + c0, k, wn, s)) return rc;
-  }
-  return PG_OK;
-}
-
 int prepare_edge(PreparedEdge& e, int mode, int c_in, const float* const* weights, const float* const* biases,
                  const int32_t* dims, int num_layers, bool want_tc, cudaStream_t s) {
   PG_REQUIRE(num_layers >= 1 && num_layers <= 8, "edge MLP depth %d not in [1, 8]", num_layers);
@@ -563,7 +548,7 @@ int prepare_edge(PreparedEdge& e, int mode, int c_in, const float* const* weight
   e.b.assign(biases, biases + num_layers);
   for (int l = 0; l < num_layers; ++l) PG_REQUIRE(weights[l] && biases[l], "null weight/bias for layer %d", l);
   e.path = EDGE_FP32;
-  if (!want_tc || !pg_tc_available() || num_layers < 2) return PG_OK;
+  if (!want_tc || num_layers < 2) return PG_OK;
   if (mode == PG_EDGE_POOL) {
     // PointSetPooling (one feature channel): layer 0 in fp32 inside the producer of layer 1; layers 1 .. L-2
     // store their per-edge activations (rows for the next layer); layer L-1 ends in the segment max
@@ -583,8 +568,9 @@ int prepare_edge(PreparedEdge& e, int mode, int c_in, const float* const* weight
       if (int rc = prepare_gemm(e.mid[l - 1], weights[l], dims[l + 1], biases[l], dims[l], dims[l + 1], s)) return rc;
       e.mid_width = std::max(e.mid_width, int(dims[l + 1]));
     }
-    if (int rc = prepare_last(e, weights[num_layers - 1], biases[num_layers - 1], dims[num_layers - 1],
-                              dims[num_layers], s))
+    const int n = dims[num_layers];
+    if (int rc = prepare_column_blocks(e.last, e.last_col0, weights[num_layers - 1], n, biases[num_layers - 1],
+                                       dims[num_layers - 1], n, n, s))
       return rc;
     e.path = EDGE_POOL;
     return PG_OK;
@@ -601,20 +587,8 @@ int prepare_edge(PreparedEdge& e, int mode, int c_in, const float* const* weight
   PG_CUDA_OK(e.w1x.alloc(sizeof(float) * 3 * e.kp, s));
   pad_rows_kernel<<<4, 256, 0, s>>>(weights[0] + int64_t(c_in) * d1, 3, d1, e.kp, e.w1x.as<float>());
   PG_LAUNCH_CHECK();
-  if (int rc = prepare_last(e, weights[1], biases[1], d1, n, s)) return rc;
+  if (int rc = prepare_column_blocks(e.last, e.last_col0, weights[1], n, biases[1], d1, n, n, s)) return rc;
   e.path = EDGE_GNN;
-  return PG_OK;
-}
-
-// read the range-error word back unless the caller vouched for the indices (PG_FLAG_TRUSTED_INDICES)
-int finish_index_check(const Temp& t_err, int64_t num_src, int64_t num_dst, cudaStream_t s) {
-  int h = 0;
-  if (!trusted_indices()) {
-    PG_CUDA_OK(cudaMemcpyAsync(&h, t_err.ptr, sizeof(int), cudaMemcpyDeviceToHost, s));
-    PG_CUDA_OK(cudaStreamSynchronize(s));
-  }
-  PG_REQUIRE(h == 0, "edge index out of range (src in [0,%lld), dst in [0,%lld))", (long long)num_src,
-             (long long)num_dst);
   return PG_OK;
 }
 
@@ -629,17 +603,15 @@ int apply_last(const PreparedEdge& e, WgParams p, int n, float* out, cudaStream_
   return PG_OK;
 }
 
-int apply_edge(const PreparedEdge& e, const float* features, const float* xyz_src, const float* xyz_dst,
-               const int32_t* dst_index, const int32_t* src, const int32_t* dst, int64_t num_edges, int64_t num_src,
-               int64_t num_dst, float* out, cudaStream_t s) {
+// the launches of one edge call: the segment max into out (pre-filled with -FLT_MAX); an out-of-range src / dst
+// sets *err
+int launch_edge(const PreparedEdge& e, const float* features, const float* xyz_src, const float* xyz_dst,
+                const int32_t* dst_index, const int32_t* src, const int32_t* dst, int64_t num_edges, int64_t num_src,
+                int64_t num_dst, float* out, int* err, cudaStream_t s) {
   const int n = e.dims[e.num_layers];
   if (e.path == EDGE_FP32 || num_edges == 0)
     return edge_mlp_max_fp32(e.mode, features, e.c_in, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst,
-                             e.w.data(), e.b.data(), e.dims.data(), e.num_layers, out, s);
-  Temp t_err;
-  PG_CUDA_OK(t_err.alloc(sizeof(int), s));
-  PG_CUDA_OK(cudaMemsetAsync(t_err.ptr, 0, sizeof(int), s));
-  if (int rc = fill_async(out, num_dst * n, -FLT_MAX, s)) return rc;
+                             e.w.data(), e.b.data(), e.dims.data(), e.num_layers, out, err, s);
   WgParams p{};
   p.xyz_src = xyz_src;
   p.xyz_dst = xyz_dst;
@@ -647,7 +619,7 @@ int apply_edge(const PreparedEdge& e, const float* features, const float* xyz_sr
   p.num_src = num_src;
   p.num_dst = num_dst;
   p.w1x = e.w1x.as<float>();
-  p.err = t_err.as<int>();
+  p.err = err;
   if (e.path == EDGE_POOL) {
     const int L = e.num_layers;
     p.feat = features;
@@ -655,8 +627,7 @@ int apply_edge(const PreparedEdge& e, const float* features, const float* xyz_sr
       p.src = src;
       p.dst = dst;
       p.num_rows = num_edges;
-      if (int rc = apply_last<PROD_POOL>(e, p, n, out, s)) return rc;
-      return finish_index_check(t_err, num_src, num_dst, s);
+      return apply_last<PROD_POOL>(e, p, n, out, s);
     }
     // the stored per-edge activations are bounded by slicing the edge list (a destination whose edges straddle
     // two slices is merged by the atomic max like any tile boundary)
@@ -682,7 +653,7 @@ int apply_edge(const PreparedEdge& e, const float* features, const float* xyz_sr
         r.num_rows = ne;
         r.dst = dst + e0;
         r.num_dst = num_dst;
-        r.err = t_err.as<int>();
+        r.err = err;
         if (l + 1 < L) {
           r.out = h[(l + 1) & 1].as<float>();
           r.ldo = e.dims[l + 1];
@@ -693,7 +664,7 @@ int apply_edge(const PreparedEdge& e, const float* features, const float* xyz_sr
         }
       }
     }
-    return finish_index_check(t_err, num_src, num_dst, s);
+    return PG_OK;
   }
   // GNN edge layer: hoisted per-vertex GEMM, then the fused gather / second layer / segment max kernel
   Temp t_p;
@@ -705,8 +676,25 @@ int apply_edge(const PreparedEdge& e, const float* features, const float* xyz_sr
   p.src = src;
   p.dst = dst;
   p.num_rows = num_edges;
-  if (int rc = apply_last<PROD_GNN>(e, p, n, out, s)) return rc;
-  return finish_index_check(t_err, num_src, num_dst, s);
+  return apply_last<PROD_GNN>(e, p, n, out, s);
+}
+
+// one edge call on either route: the error word, the -FLT_MAX fill of out, the launches, and the read-back of the
+// error word unless the caller vouched for the indices (trusted: no read-back, no synchronisation)
+int apply_edge(const PreparedEdge& e, const float* features, const float* xyz_src, const float* xyz_dst,
+               const int32_t* dst_index, const int32_t* src, const int32_t* dst, int64_t num_edges, int64_t num_src,
+               int64_t num_dst, bool trusted, float* out, cudaStream_t s) {
+  ErrorWord err;
+  if (int rc = err.init(s)) return rc;
+  if (int rc = fill_async(out, num_dst * e.dims[e.num_layers], -FLT_MAX, s)) return rc;
+  if (int rc = launch_edge(e, features, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst, out,
+                           err.ptr(), s))
+    return rc;
+  int h = 0;
+  if (int rc = err.read(&h, trusted, s)) return rc;
+  PG_REQUIRE(h == 0, "edge index out of range (src in [0,%lld), dst in [0,%lld))", (long long)num_src,
+             (long long)num_dst);
+  return PG_OK;
 }
 
 // ---- the class-aware predictor heads (gnn.py:133-163) ---------------------------------------------
@@ -829,50 +817,137 @@ __global__ void copy_block_kernel(const float* __restrict__ src, int64_t rows, i
 struct PreparedPredictor {
   int D = 0, H = 0, C = 0, box = 0, htot = 0;
   bool fused = false;
+  // fused route: the concatenated first layers on the tensor cores, then predictor_heads_kernel
   Temp wcat, bcat, wpack;                  // [D, htot] concatenated first layers, [htot], head weights
   std::vector<PreparedFc> first;           // column groups of the concatenated first layer (<= 256 wide each)
   std::vector<int> col0;
   int wfloats = 0;
   size_t smem = 0;
+  // per-layer route: every layer prepared on its own
+  std::vector<PreparedFc> layers;
 };
 
+// dims = {D, H, C, box_len}; layers = cls fc0, cls fc1, then per class c: fc0, fc1, fc2
+int prepare_predictor(PreparedPredictor& P, const float* const* weights, const float* const* biases,
+                      const int32_t* dims, int num_layers, bool want_tc, cudaStream_t s) {
+  P.D = dims[0];
+  P.H = dims[1];
+  P.C = dims[2];
+  P.box = dims[3];
+  PG_REQUIRE(num_layers == 2 + 3 * P.C && P.C >= 1 && P.C <= 16 && P.H >= 1 && P.box >= 1,
+             "pg_layer_create: predictor needs 2 + 3 C layers, 1 <= C <= 16");
+  P.htot = P.H * (P.C + 1);
+  auto pad4 = [](int v) { return (v + 3) & ~3; };
+  P.wfloats = pad4(P.H * P.C) + pad4(P.C) + P.C * (pad4(P.H * P.H) + pad4(P.H) + pad4(P.H * P.box) + pad4(P.box));
+  P.smem = (size_t((P.wfloats + 3) & ~3) + 2 * size_t(kHeadRows) * (kHeadH + 1) + size_t(kHeadRows) * 16) * sizeof(float);
+  // the heads kernel is built for H = kHeadH and keeps every head weight in shared memory; the first-layer groups
+  // read column slices of the concatenated matrix, which only the tensor-core path can (every group is >= H wide,
+  // so all of them qualify when one H-wide group does)
+  P.fused = want_tc && P.H == kHeadH && P.smem <= 227 * 1024 && fc_uses_tc(P.D, P.H);
+  if (P.fused) {
+    PG_CUDA_OK(P.wcat.alloc(sizeof(float) * size_t(P.D) * P.htot, s));
+    PG_CUDA_OK(P.bcat.alloc(sizeof(float) * P.htot, s));
+    PG_CUDA_OK(P.wpack.alloc(sizeof(float) * P.wfloats, s));
+    // concatenated first layers: column block h = 0 is the cls head, h = 1 + c the loc head of class c
+    for (int h = 0; h <= P.C; ++h) {
+      const int l = h == 0 ? 0 : 2 + 3 * (h - 1);
+      copy_block_kernel<<<32, 256, 0, s>>>(weights[l], P.D, P.H, P.htot, P.wcat.as<float>() + h * P.H);
+      PG_LAUNCH_CHECK();
+      PG_CUDA_OK(cudaMemcpyAsync(P.bcat.as<float>() + h * P.H, biases[l], sizeof(float) * P.H, cudaMemcpyDeviceToDevice, s));
+    }
+    // the heads' weight pack, sections in the order predictor_heads_kernel reads them, each on a 16-byte boundary
+    std::vector<std::pair<const float*, size_t>> sections = {{weights[1], size_t(P.H) * P.C}, {biases[1], size_t(P.C)}};
+    for (int c = 0; c < P.C; ++c) {
+      sections.push_back({weights[2 + 3 * c + 1], size_t(P.H) * P.H});
+      sections.push_back({biases[2 + 3 * c + 1], size_t(P.H)});
+      sections.push_back({weights[2 + 3 * c + 2], size_t(P.H) * P.box});
+      sections.push_back({biases[2 + 3 * c + 2], size_t(P.box)});
+    }
+    float* wp = P.wpack.as<float>();
+    PG_CUDA_OK(cudaMemsetAsync(wp, 0, sizeof(float) * P.wfloats, s));
+    size_t off = 0;
+    for (const auto& sec : sections) {
+      PG_CUDA_OK(cudaMemcpyAsync(wp + off, sec.first, sizeof(float) * sec.second, cudaMemcpyDeviceToDevice, s));
+      off += (sec.second + 3) & ~size_t(3);
+    }
+    // column groups of at most 256 (whole heads) -> one tensor-core GEMM each
+    const int heads_per_group = std::max(1, 256 / P.H);
+    for (int h0 = 0; h0 <= P.C; h0 += heads_per_group) {
+      const int nh = std::min(heads_per_group, P.C + 1 - h0);
+      P.first.emplace_back();
+      P.col0.push_back(h0 * P.H);
+      if (int rc = prepare_fc(P.first.back(), P.wcat.as<float>() + h0 * P.H, P.htot, P.bcat.as<float>() + h0 * P.H, P.D,
+                              nh * P.H, nh * P.H, want_tc, s))
+        return rc;
+      if (!P.first.back().tc) P.fused = false;   // FFMA kernel needs contiguous weights: per-layer route
+    }
+  }
+  if (P.fused) return PG_OK;
+  P.first.clear();
+  P.layers.resize(num_layers);
+  for (int l = 0; l < num_layers; ++l) {
+    const int pos = l < 2 ? l : (l - 2) % 3;
+    const int k = pos == 0 ? P.D : P.H;
+    const int n = l == 1 ? P.C : (l >= 2 && pos == 2 ? P.box : P.H);
+    if (int rc = prepare_fc(P.layers[l], weights[l], n, biases[l], k, n, n, want_tc, s)) return rc;
+  }
+  return PG_OK;
+}
+
 }  // namespace
+}  // namespace pg
 
+using namespace pg;
 
 // ---------------------------------------------------------------------------------------------------
-// per-call entry points (prepare into temporaries, apply once)
+// per-call entry points: a transient prepared layer on the stack, applied once
 // ---------------------------------------------------------------------------------------------------
-int fc_tc_bf16x3(const float* x, int64_t m, int k, const float* w, const float* bias, int n, int act,
-                 const float* residual, float* out, cudaStream_t s) {
+extern "C" int pg_fully_connected(const float* x, int64_t m, int32_t k, const float* w, const float* bias, int32_t n,
+                                  int32_t act, const float* residual, float* out, int32_t precision, void* stream) {
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  PG_REQUIRE(m >= 0 && k >= 1 && n >= 1, "pg_fully_connected: bad sizes m=%lld k=%d n=%d", (long long)m, k, n);
+  PG_REQUIRE(act == 0 || act == 1, "pg_fully_connected: act must be 0 (linear) or 1 (ReLU)");
+  if (m == 0) return PG_OK;
+  PG_REQUIRE(x && w && bias && out, "pg_fully_connected: null argument");
+  PG_REQUIRE(precision == 0 || precision == 1, "pg_fully_connected: unknown precision %d", precision);
   PreparedFc f;
-  if (int rc = prepare_fc(f, w, n, bias, k, n, n, m >= 1, s)) return rc;
+  if (int rc = prepare_fc(f, w, n, bias, k, n, n, precision == 1 && pg_tc_available(), s)) return rc;
   return apply_fc(f, x, m, act, residual, out, n, s);
 }
 
-int edge_mlp_max_tc(int mode, const float* features, int c_in, const float* xyz_src, const float* xyz_dst,
-                    const int32_t* dst_index, const int32_t* src, const int32_t* dst, int64_t num_edges,
-                    int64_t num_src, int64_t num_dst, const float* const* weights, const float* const* biases,
-                    const int32_t* dims, int num_layers, float* out, cudaStream_t s) {
+extern "C" int pg_edge_mlp_max(int32_t mode, const float* features, int32_t num_feature_channels, const float* xyz_src,
+                               const float* xyz_dst, const int32_t* dst_index, const int32_t* src, const int32_t* dst,
+                               int64_t num_edges, int64_t num_src, int64_t num_dst, const float* const* weights_host,
+                               const float* const* biases_host, const int32_t* dims_host, int32_t num_layers, float* out,
+                               int32_t precision, void* stream) {
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  PG_REQUIRE(mode == PG_EDGE_POOL || mode == PG_EDGE_GNN, "pg_edge_mlp_max: unknown mode %d", mode);
+  PG_REQUIRE(weights_host && biases_host && dims_host, "pg_edge_mlp_max: null layer tables");
+  PG_REQUIRE(num_edges >= 0 && num_src >= 1 && num_dst >= 0, "pg_edge_mlp_max: bad sizes");
+  PG_REQUIRE(out != nullptr || num_dst == 0, "pg_edge_mlp_max: out is null");
+  PG_REQUIRE((features && xyz_src && xyz_dst && src && dst) || num_edges == 0, "pg_edge_mlp_max: null input");
+  PG_REQUIRE(mode == PG_EDGE_GNN || dst_index != nullptr || num_edges == 0,
+             "pg_edge_mlp_max: POOL mode needs keypoint indices");
+  const bool trusted = (precision & PG_FLAG_TRUSTED_INDICES) != 0;
+  precision &= PG_PRECISION_MASK;
+  PG_REQUIRE(precision == 0 || precision == 1, "pg_edge_mlp_max: unknown precision %d", precision);
   PreparedEdge e;
-  if (int rc = prepare_edge(e, mode, c_in, weights, biases, dims, num_layers, num_edges > 0, s)) return rc;
-  return apply_edge(e, features, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst, out, s);
+  if (int rc = prepare_edge(e, mode, num_feature_channels, weights_host, biases_host, dims_host, num_layers,
+                            precision == 1 && num_edges > 0 && pg_tc_available(), s))
+    return rc;
+  return apply_edge(e, features, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst, trusted, out, s);
 }
-
-}  // namespace pg
 
 // ---------------------------------------------------------------------------------------------------
 // pg_layer: prepared layers behind the C ABI
 // ---------------------------------------------------------------------------------------------------
 struct pg_layer {
-  int kind = 0, precision = 0, num_layers = 0;
+  int kind = 0, num_layers = 0;
   std::vector<int32_t> dims;
-  std::vector<pg::PreparedFc> fcs;      // PG_LAYER_MLP
-  pg::PreparedEdge edge;                // PG_LAYER_EDGE_POOL / PG_LAYER_EDGE_GNN
-  pg::PreparedPredictor pred;           // PG_LAYER_PREDICTOR
-  std::vector<const float*> w, b;
+  std::vector<PreparedFc> fcs;          // PG_LAYER_MLP
+  PreparedEdge edge;                    // PG_LAYER_EDGE_POOL / PG_LAYER_EDGE_GNN
+  PreparedPredictor pred;               // PG_LAYER_PREDICTOR
 };
-
-using namespace pg;
 
 extern "C" int pg_layer_create(int32_t kind, const float* const* weights_host, const float* const* biases_host,
                                const int32_t* dims_host, int32_t num_layers, int32_t precision, void* stream,
@@ -885,98 +960,27 @@ extern "C" int pg_layer_create(int32_t kind, const float* const* weights_host, c
   PG_REQUIRE(kind == PG_LAYER_MLP || kind == PG_LAYER_EDGE_POOL || kind == PG_LAYER_EDGE_GNN || kind == PG_LAYER_PREDICTOR,
              "pg_layer_create: unknown kind %d", kind);
   for (int l = 0; l < num_layers; ++l) PG_REQUIRE(weights_host[l] && biases_host[l], "pg_layer_create: null weight/bias %d", l);
-  pg_layer* L = new pg_layer();
+  auto L = std::make_unique<pg_layer>();
   L->kind = kind;
-  L->precision = precision;
   L->num_layers = num_layers;
-  L->w.assign(weights_host, weights_host + num_layers);
-  L->b.assign(biases_host, biases_host + num_layers);
-  int rc = PG_OK;
-  const bool tc = precision == 1 && pg_tc_available();
+  const bool want_tc = precision == 1 && pg_tc_available();
   if (kind == PG_LAYER_MLP) {
     L->dims.assign(dims_host, dims_host + num_layers + 1);
     L->fcs.resize(num_layers);
-    for (int l = 0; l < num_layers && rc == PG_OK; ++l)
-      rc = prepare_fc(L->fcs[l], weights_host[l], dims_host[l + 1], biases_host[l], dims_host[l], dims_host[l + 1],
-                      dims_host[l + 1], tc, s);
+    for (int l = 0; l < num_layers; ++l)
+      if (int rc = prepare_fc(L->fcs[l], weights_host[l], dims_host[l + 1], biases_host[l], dims_host[l],
+                              dims_host[l + 1], dims_host[l + 1], want_tc, s))
+        return rc;
   } else if (kind == PG_LAYER_EDGE_POOL || kind == PG_LAYER_EDGE_GNN) {
     L->dims.assign(dims_host, dims_host + num_layers + 1);
-    rc = prepare_edge(L->edge, kind == PG_LAYER_EDGE_POOL ? PG_EDGE_POOL : PG_EDGE_GNN, dims_host[0] - 3, weights_host,
-                      biases_host, dims_host, num_layers, tc, s);
+    if (int rc = prepare_edge(L->edge, kind == PG_LAYER_EDGE_POOL ? PG_EDGE_POOL : PG_EDGE_GNN, dims_host[0] - 3,
+                              weights_host, biases_host, dims_host, num_layers, want_tc, s))
+      return rc;
   } else {
-    // predictor: dims = {D, H, C, box_len}; layers = cls fc0, cls fc1, then per class c: fc0, fc1, fc2
     L->dims.assign(dims_host, dims_host + 4);
-    PreparedPredictor& P = L->pred;
-    P.D = dims_host[0];
-    P.H = dims_host[1];
-    P.C = dims_host[2];
-    P.box = dims_host[3];
-    if (num_layers != 2 + 3 * P.C || P.C < 1 || P.C > 16 || P.H < 1 || P.box < 1) {
-      delete L;
-      PG_REQUIRE(false, "pg_layer_create: predictor needs 2 + 3 C layers, 1 <= C <= 16");
-    }
-    P.htot = P.H * (P.C + 1);
-    auto pad4 = [](int v) { return (v + 3) & ~3; };
-    P.wfloats = pad4(P.H * P.C) + pad4(P.C) + P.C * (pad4(P.H * P.H) + pad4(P.H) + pad4(P.H * P.box) + pad4(P.box));
-    P.smem = (size_t((P.wfloats + 3) & ~3) + 2 * size_t(kHeadRows) * (kHeadH + 1) + size_t(kHeadRows) * 16) * sizeof(float);
-    P.fused = P.H == kHeadH && P.smem <= 227 * 1024;
-    if (P.fused) {
-      auto cuda_ok = [&](cudaError_t e) { if (e != cudaSuccess && rc == PG_OK) { pg::set_error("predictor prepare: %s", cudaGetErrorString(e)); rc = PG_ERR_CUDA; } };
-      cuda_ok(P.wcat.alloc(sizeof(float) * size_t(P.D) * P.htot, s));
-      cuda_ok(P.bcat.alloc(sizeof(float) * P.htot, s));
-      cuda_ok(P.wpack.alloc(sizeof(float) * P.wfloats, s));
-      if (rc == PG_OK) {
-        // concatenated first layers: column block h = 0 is the cls head, h = 1 + c the loc head of class c
-        for (int h = 0; h <= P.C; ++h) {
-          const int l = h == 0 ? 0 : 2 + 3 * (h - 1);
-          copy_block_kernel<<<32, 256, 0, s>>>(weights_host[l], P.D, P.H, P.htot, P.wcat.as<float>() + h * P.H);
-          count_launch();
-          cuda_ok(cudaMemcpyAsync(P.bcat.as<float>() + h * P.H, biases_host[l], sizeof(float) * P.H, cudaMemcpyDeviceToDevice, s));
-        }
-        float* wp = P.wpack.as<float>();
-        size_t off = 0;
-        cuda_ok(cudaMemsetAsync(wp, 0, sizeof(float) * P.wfloats, s));
-        auto put = [&](const float* src, size_t count) {     // sections start on 16-byte boundaries
-          cuda_ok(cudaMemcpyAsync(wp + off, src, sizeof(float) * count, cudaMemcpyDeviceToDevice, s));
-          off += (count + 3) & ~size_t(3);
-        };
-        put(weights_host[1], size_t(P.H) * P.C);
-        put(biases_host[1], P.C);
-        for (int c = 0; c < P.C; ++c) {
-          put(weights_host[2 + 3 * c + 1], size_t(P.H) * P.H);
-          put(biases_host[2 + 3 * c + 1], P.H);
-          put(weights_host[2 + 3 * c + 2], size_t(P.H) * P.box);
-          put(biases_host[2 + 3 * c + 2], P.box);
-        }
-        // column groups of at most 256 (whole heads) -> one tensor-core GEMM each
-        const int heads_per_group = std::max(1, 256 / P.H);
-        for (int h0 = 0; h0 <= P.C && rc == PG_OK; h0 += heads_per_group) {
-          const int nh = std::min(heads_per_group, P.C + 1 - h0);
-          P.first.emplace_back();
-          P.col0.push_back(h0 * P.H);
-          rc = prepare_fc(P.first.back(), P.wcat.as<float>() + h0 * P.H, P.htot, P.bcat.as<float>() + h0 * P.H, P.D,
-                          nh * P.H, nh * P.H, tc, s);
-          if (rc == PG_OK && !P.first.back().tc) P.fused = false;   // FFMA kernel needs contiguous weights: per-layer path
-        }
-      }
-    }
-    if (!P.fused && rc == PG_OK) {
-      // generic route: every layer prepared on its own (used for shapes the heads kernel is not built for)
-      P.first.clear();
-      L->fcs.resize(num_layers);
-      for (int l = 0; l < num_layers && rc == PG_OK; ++l) {
-        const int pos = l < 2 ? l : (l - 2) % 3;
-        const int k = pos == 0 ? P.D : P.H;
-        const int n = l == 1 ? P.C : (l >= 2 && pos == 2 ? P.box : P.H);
-        rc = prepare_fc(L->fcs[l], weights_host[l], n, biases_host[l], k, n, n, tc, s);
-      }
-    }
+    if (int rc = prepare_predictor(L->pred, weights_host, biases_host, dims_host, num_layers, want_tc, s)) return rc;
   }
-  if (rc != PG_OK) {
-    delete L;
-    return rc;
-  }
-  *out_layer = L;
+  *out_layer = L.release();
   return PG_OK;
 }
 
@@ -1022,11 +1026,8 @@ extern "C" int pg_layer_edge_mlp_max(const pg_layer* layer, const float* feature
   PG_REQUIRE((features && xyz_src && xyz_dst && src && dst) || num_edges == 0, "pg_layer_edge_mlp_max: null input");
   PG_REQUIRE(layer->kind == PG_LAYER_EDGE_GNN || dst_index != nullptr || num_edges == 0,
              "pg_layer_edge_mlp_max: POOL mode needs keypoint indices");
-  struct TrustedScope {
-    explicit TrustedScope(bool v) { pg::set_trusted_indices(v); }
-    ~TrustedScope() { pg::set_trusted_indices(false); }
-  } scope((flags & PG_FLAG_TRUSTED_INDICES) != 0);
-  return apply_edge(layer->edge, features, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst, out, s);
+  return apply_edge(layer->edge, features, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst,
+                    (flags & PG_FLAG_TRUSTED_INDICES) != 0, out, s);
 }
 
 extern "C" int pg_layer_predictor(const pg_layer* layer, const float* x, int64_t m, float* logits, float* boxes,
@@ -1062,20 +1063,20 @@ extern "C" int pg_layer_predictor(const pg_layer* layer, const float* x, int64_t
     PG_LAUNCH_CHECK();
     return PG_OK;
   }
-  // generic route: layer by layer
+  // per-layer route
   Temp h1, h2, tmp;
   PG_CUDA_OK(h1.alloc(sizeof(float) * m * P.H, s));
   PG_CUDA_OK(h2.alloc(sizeof(float) * m * P.H, s));
   PG_CUDA_OK(tmp.alloc(sizeof(float) * m * P.box, s));
-  if (int rc = apply_fc(layer->fcs[0], x, m, 1, nullptr, h1.as<float>(), P.H, s)) return rc;
-  if (int rc = apply_fc(layer->fcs[1], h1.as<float>(), m, 0, nullptr, logits, P.C, s)) return rc;
+  if (int rc = apply_fc(P.layers[0], x, m, 1, nullptr, h1.as<float>(), P.H, s)) return rc;
+  if (int rc = apply_fc(P.layers[1], h1.as<float>(), m, 0, nullptr, logits, P.C, s)) return rc;
   if (probs != nullptr)
     if (int rc = pg_softmax_rows(logits, m, P.C, probs, stream)) return rc;
   for (int c = 0; c < P.C; ++c) {
     const int l = 2 + 3 * c;
-    if (int rc = apply_fc(layer->fcs[l], x, m, 1, nullptr, h1.as<float>(), P.H, s)) return rc;
-    if (int rc = apply_fc(layer->fcs[l + 1], h1.as<float>(), m, 1, nullptr, h2.as<float>(), P.H, s)) return rc;
-    if (int rc = apply_fc(layer->fcs[l + 2], h2.as<float>(), m, 0, nullptr, tmp.as<float>(), P.box, s)) return rc;
+    if (int rc = apply_fc(P.layers[l], x, m, 1, nullptr, h1.as<float>(), P.H, s)) return rc;
+    if (int rc = apply_fc(P.layers[l + 1], h1.as<float>(), m, 1, nullptr, h2.as<float>(), P.H, s)) return rc;
+    if (int rc = apply_fc(P.layers[l + 2], h2.as<float>(), m, 0, nullptr, tmp.as<float>(), P.box, s)) return rc;
     copy_block_kernel<<<64, 256, 0, s>>>(tmp.as<float>(), m, P.box, P.C * P.box, boxes + c * P.box);
     PG_LAUNCH_CHECK();
   }

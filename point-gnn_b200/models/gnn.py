@@ -21,9 +21,6 @@ import torch
 from .. import _lib
 from .. import get_precision
 
-_PG_EDGE_POOL = 0
-_PG_EDGE_GNN = 1
-
 
 # ---------------------------------------------------------------------------------------------
 # variable scoping (stand-in for tf.variable_scope + slim's layer naming)
@@ -143,11 +140,6 @@ def _check_types(normalization_type, activation_type):
                                   '(SURVEY fact 3); batch/instance norm are not built' % normalization_type)
     if activation_fn_dict[activation_type] not in ('ReLU',):
         raise NotImplementedError('activation %r: every shipped config uses "ReLU"' % activation_type)
-
-
-def _fully_connected(features, relu, residual=None):
-    w, b = _next_fully_connected()
-    return _lib.fully_connected(features, w, b, relu, residual=residual, precision=get_precision())
 
 
 def multi_layer_fc_fn(sv, mask=None, Ks=(64, 32, 64), num_classes=4, is_logits=False, num_layer=4,

@@ -532,3 +532,110 @@ def test_scatter_sum_and_mean_vs_numpy(car):
     for n in ('layer1/combined_features/fully_connected', 'layer1/combined_features/fully_connected_1'):
         agg = np.maximum(agg @ w[n + '/weights'] + w[n + '/biases'], 0)
     assert np.abs(got - agg).max() < 1e-3 * max(1.0, np.abs(agg).max())
+
+
+# edge layer shapes: (mode, feature channels, layer widths) - a GNN iteration (two layers) and a pooling MLP (three)
+EDGE_SHAPES = {'gnn': (1, 32, (64, 64)), 'pool': (0, 1, (32, 64, 128))}
+
+
+def _edge_layer_inputs(shape, seed):
+    """Random weights and a destination-sorted edge list for one EDGE_SHAPES entry."""
+    from pointgnn_b200 import _lib
+    mode, c_in, widths = EDGE_SHAPES[shape]
+    rng = np.random.default_rng(seed)
+    nv, e = 700, 3000
+    dims = [c_in + 3] + list(widths)
+    ws = [_cuda((rng.standard_normal((dims[i], dims[i + 1])) / np.sqrt(dims[i])).astype(np.float32))
+          for i in range(len(widths))]
+    bs = [_cuda((rng.standard_normal(dims[i + 1]) * 0.1).astype(np.float32)) for i in range(len(widths))]
+    f = _cuda((rng.standard_normal((nv, c_in)) * 0.5).astype(np.float32))
+    x = _cuda((rng.standard_normal((nv, 3)) * 20).astype(np.float32))
+    if mode == 1:      # GNN: the destinations are the vertices, xyz_dst the offset coordinates
+        nd, xd, kp = nv, x + _cuda((rng.standard_normal((nv, 3)) * 0.1).astype(np.float32)), None
+    else:              # pooling: the destinations are keypoints, indirected into xyz_dst
+        nd, xd = 300, x
+        kp = _cuda(rng.integers(0, nv, nd).astype(np.int32))
+    src = _cuda(rng.integers(0, nv, e).astype(np.int32))
+    dst = _cuda(np.sort(rng.integers(0, nd, e)).astype(np.int32))
+    kind = _lib.PG_LAYER_EDGE_GNN if mode == 1 else _lib.PG_LAYER_EDGE_POOL
+    return mode, kind, dims, ws, bs, (f, x, xd, kp), src, dst, nd
+
+
+def _counted(fn):
+    """fn() and the number of kernel launches it made."""
+    from pointgnn_b200 import _lib
+    before = _lib.launch_count()
+    out = fn()
+    return out, _lib.launch_count() - before
+
+
+@pytest.mark.parametrize('precision', [0, 1])
+def test_per_call_equals_prepared(precision):
+    """pg_fully_connected / pg_edge_mlp_max equal pg_layer_create + pg_layer_mlp / pg_layer_edge_mlp_max bit for bit
+    and launch as many kernels (the segment max is an exact max, so the order of its atomics does not matter)."""
+    if precision == 1:
+        _need('bf16x3')
+    from pointgnn_b200 import _lib
+    rng = np.random.default_rng(12)
+    # 600 features run as two column blocks on the tensor cores
+    for m, k, n in ((1000, 300, 300), (513, 4, 32), (257, 300, 600)):
+        x = _cuda(rng.standard_normal((m, k)).astype(np.float32))
+        w = _cuda((rng.standard_normal((k, n)) / np.sqrt(k)).astype(np.float32))
+        b = _cuda(rng.standard_normal(n).astype(np.float32))
+        r = _cuda(rng.standard_normal((m, n)).astype(np.float32))
+        for relu in (True, False):
+            for res in (None, r):
+                dense0 = _lib.tc_launch_count(1)
+                per, per_launches = _counted(
+                    lambda: _lib.fully_connected(x, w, b, relu, residual=res, precision=precision))
+                if precision == 1 and n == 600:
+                    assert _lib.tc_launch_count(1) - dense0 == 2
+                layer, create_launches = _counted(
+                    lambda: _lib.PreparedLayer(_lib.PG_LAYER_MLP, [w], [b], [k, n], precision))
+                prep, apply_launches = _counted(lambda: layer.mlp(x, last_linear=not relu, residual=res))
+                assert torch.equal(per, prep), (m, k, n, relu, res is not None)
+                assert per_launches == create_launches + apply_launches, (m, k, n, relu, res is not None)
+    for shape in EDGE_SHAPES:
+        mode, kind, dims, ws, bs, (f, x, xd, kp), src, dst, nd = _edge_layer_inputs(shape, 13)
+        per, per_launches = _counted(
+            lambda: _lib.edge_mlp_max(mode, f, x, xd, kp, src, dst, nd, ws, bs, precision=precision))
+        layer, create_launches = _counted(lambda: _lib.PreparedLayer(kind, ws, bs, dims, precision))
+        prep, apply_launches = _counted(lambda: layer.edge_mlp_max(f, x, xd, kp, src, dst, nd))
+        assert torch.equal(per, prep), shape
+        assert per_launches == create_launches + apply_launches, shape
+
+
+@pytest.mark.parametrize('shape', list(EDGE_SHAPES))
+@pytest.mark.parametrize('precision', [0, 1])
+@pytest.mark.parametrize('route', ['per_call', 'prepared'])
+def test_edge_index_errors_on_every_route(route, precision, shape):
+    """An out-of-range src or dst raises on every edge route, and a trusted call (no read-back) does not stop a
+    later untrusted call on the same thread from checking its indices."""
+    if precision == 1:
+        _need('bf16x3')
+    from pointgnn_b200 import _lib
+    mode, kind, dims, ws, bs, (f, x, xd, kp), src, dst, nd = _edge_layer_inputs(shape, 14)
+    if route == 'prepared':
+        layer = _lib.PreparedLayer(kind, ws, bs, dims, precision)
+
+        def call(s, d, trusted=False):
+            return layer.edge_mlp_max(f, x, xd, kp, s, d, nd, trusted=trusted)
+    else:
+        def call(s, d, trusted=False):
+            return _lib.edge_mlp_max(mode, f, x, xd, kp, s, d, nd, ws, bs, precision=precision, trusted=trusted)
+    good = call(src, dst)
+    bad = []
+    for pos, value in ((src.numel() // 2, f.shape[0] + 7), (0, -1)):
+        s = src.clone()
+        s[pos] = value
+        bad.append((s, dst))
+    for pos, value in ((-1, nd + 3), (0, -1)):          # dst stays non-decreasing
+        d = dst.clone()
+        d[pos] = value
+        bad.append((src, d))
+    for s, d in bad:
+        with pytest.raises(_lib.PointGNNError, match='out of range'):
+            call(s, d)
+    assert torch.equal(call(src, dst, trusted=True), good)
+    with pytest.raises(_lib.PointGNNError, match='out of range'):
+        call(bad[0][0], dst)
