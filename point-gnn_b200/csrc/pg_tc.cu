@@ -1,7 +1,8 @@
 // Hopper tensor-core kernels (wgmma): the fast path (precision = 1, "BF16x3").
 //
-// wg_gemm_kernel - one persistent kernel for every tensor-core layer of the network:
-//   out = epilogue(A @ W + b), A produced on the fly in shared memory by the consumer warpgroups.
+// wg_gemm_kernel - one persistent, warp-specialised kernel for every tensor-core layer of the network:
+//   out = epilogue(A @ W + b), W streamed by a producer warpgroup, A produced on the fly in shared memory by the
+//   two consumer warpgroups that also run the wgmmas.
 //
 //   producers  PROD_ROWS  A = rows of an fp32 matrix (dense layers, the later layers of the pooling MLP)
 //              PROD_GNN   one GNN iteration's edge MLP (/root/reference/models/gnn.py:338-365) after hoisting:
@@ -16,13 +17,16 @@
 //                         16 rows with shuffles and each partial max is flushed with one atomicMax
 //   precision  every fp32 operand is split x = hi + lo (two BF16), and hi*hi' + lo*hi' + hi*lo' is
 //              accumulated in fp32 registers: ~2^-16 relative per product (fp32-class accuracy)
-//   mapping    CTA = two consumer warpgroups, 128 rows per tile (64 per warpgroup), the whole padded N
-//              (<= 304: two m64nNk16 instructions) in registers.  W (hi and lo images, pre-packed in the
-//              no-swizzle K-major core-matrix layout, one contiguous block per 16-k chunk) streams from L2
-//              through a ring of shared-memory stages filled by cp.async.bulk with mbarrier completion;
-//              each warpgroup produces A into a double buffer, issuing the global loads of chunk k + 2
-//              before the wgmmas of chunk k + 1.  (ptxas serialises the wgmmas here, C7518, because of the
-//              divergent refill and epilogue code, so producing chunk k + 1 does not overlap chunk k's MMAs.)
+//   mapping    CTA = 3 warpgroups.  Warpgroup 0 is the W producer (setmaxnreg down to 24 registers): one thread
+//              streams W (hi and lo images, pre-packed in the no-swizzle K-major core-matrix layout, one
+//              contiguous block per 16-k chunk) from L2 through a ring of shared-memory stages with
+//              cp.async.bulk, each stage tracked by a "full" (bytes landed) and an "empty" (both consumers done)
+//              mbarrier.  Warpgroups 1 and 2 are the consumers (setmaxnreg up to 240): 128 rows per tile (64 per
+//              warpgroup), the whole padded N (<= 304: two m64nNk16 instructions) in registers.  Each produces
+//              A into a double buffer, issuing the global loads of chunk k + 2 before the wgmmas of chunk k + 1,
+//              and splits and stores chunk k + 1 while chunk k's wgmmas run.  A consumer only arrives on "empty";
+//              it never waits on it or issues a copy: such divergent code in the k-loop makes ptxas serialise
+//              the wgmmas (C7518), and the two consumers would wait for each other on every chunk.
 //
 // Operand layout (no swizzle, K-major): 8-row x 16-byte core matrices, 128 contiguous bytes each;
 // for a 16-k chunk, core(row group g, k half kc) at g * 256 + kc * 128 (LBO = 128, SBO = 256).
@@ -48,11 +52,26 @@ namespace pg {
 namespace {
 using namespace wg;
 
-constexpr int kWgThreads = 256;     // two consumer warpgroups
-constexpr int kTileRows = 128;      // rows per tile (64 per warpgroup)
-constexpr int kRing = 4;            // W stages in shared memory
+constexpr int kWgThreads = 384;     // warpgroup 0 streams W, warpgroups 1 and 2 compute
+constexpr int kProducerRegs = 24;   // 2 x 128 x 240 + 128 x 24 = 384 x 168, the launch bound's budget
+constexpr int kConsumerRegs = 240;  // 232 spills 8 bytes in the 152 x 2 segment-max instances
+constexpr int kTileRows = 128;      // rows per tile (64 per consumer warpgroup)
+// 4 W stages beat 8 on H100: the ring is deep enough for the copies, and the smaller shared-memory carve-out leaves
+// more L1 for the gathered rows (GNN edge layer at the benchmark shape: 7.7 vs 8.0 ms, H100 SXM at a 400 W limit)
+constexpr int kMaxRing = 4;
 constexpr int kMaxNT = 304;         // widest padded N one launch covers
 constexpr uint32_t kABytes = 4096;  // one warpgroup's A chunk: hi (2048) + lo (2048), 64 rows x 16 k
+
+// W stages in shared memory for an NT-wide layer: the deepest power of two up to kMaxRing (so the stage of a chunk
+// is a mask) whose ring, A buffers and barriers fit the 227 KB a CTA may use
+constexpr size_t wg_smem_bytes(int nt, int ring) {
+  return size_t(ring) * nt * 64 + 4 * kABytes + 2 * ring * sizeof(uint64_t);
+}
+constexpr int ring_stages(int nt) {
+  int r = kMaxRing;
+  while (r > 1 && wg_smem_bytes(nt, r) > 227 * 1024) r /= 2;
+  return r;
+}
 
 enum { PROD_ROWS = 0, PROD_GNN = 1, PROD_POOL = 2 };
 enum { EPI_STORE = 0, EPI_SEGMAX = 1 };
@@ -97,44 +116,57 @@ __device__ __forceinline__ void seg_flush(const WgParams& p, int d, int col, flo
   atomicMax(reinterpret_cast<int*>(p.out + int64_t(d) * p.ldo + col), __float_as_int(fmaxf(m + __ldg(p.bias + col), 0.0f) + 0.0f));
 }
 
+// w[0 .. 8) = ptr[0 .. 8); ptr is 32-byte aligned
+__device__ __forceinline__ void ldg8(const float* ptr, float (&w)[8]) {
+  const float4 a = __ldg(reinterpret_cast<const float4*>(ptr)), b = __ldg(reinterpret_cast<const float4*>(ptr) + 1);
+  w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w;
+  w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
+}
+
 template <int kProd, int kEpi, int NI, int NS>
 __global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
   constexpr int NT = NI * NS;
+  constexpr int kRing = ring_stages(NT);
   constexpr uint32_t kChunkBytes = uint32_t(NT) * 64u;   // hi + lo, 16 k
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t* bring = smem;
-  uint8_t* abuf = smem + kRing * kChunkBytes;            // [warpgroup][buffer][hi | lo]
+  uint8_t* abuf = smem + kRing * kChunkBytes;            // [consumer warpgroup][buffer][hi | lo]
   uint64_t* full = reinterpret_cast<uint64_t*>(abuf + 4 * kABytes);
   uint64_t* empty = full + kRing;
-  const int tid = threadIdx.x, wgi = tid >> 7, t = tid & 127, warp = t >> 5, lane = tid & 31;
+  const int tid = threadIdx.x;
+  const int role = __shfl_sync(0xffffffffu, tid >> 7, 0);   // warpgroup, warp-uniform by construction
   if (tid == 0) {
     for (int s = 0; s < kRing; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 8);     // lane 0 of each of the 8 warps
+      mbar_init(&empty[s], 8);     // lane 0 of each of the 8 consumer warps
     }
     fence_barrier_init();
   }
   __syncthreads();
   const int64_t my_tiles = (p.num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x;
   const int nk = p.nchunks;
-  const int64_t total = my_tiles * nk;
-  auto issue = [&](int64_t g) {
-    const uint32_t stage = uint32_t(g % kRing);
-    mbar_arrive_expect_tx(&full[stage], kChunkBytes);
-    bulk_g2s(bring + stage * kChunkBytes, p.bimg + size_t(g % nk) * kChunkBytes, kChunkBytes, &full[stage]);
-  };
-  // chunk g's stage is free again: the refill of chunk g + kRing (issued by thread 0 once both warpgroups let go)
+  if (role == 0) {
+    // W producer: one thread streams the CTA's chunks in the order the consumers use them, refilling a stage as
+    // soon as both consumer warpgroups have released it
+    setmaxnreg_dec<kProducerRegs>();
+    if (tid != 0) return;
+    const int64_t total = my_tiles * nk;
+    for (int64_t g = 0; g < total; ++g) {
+      const uint32_t stage = uint32_t(g % kRing);
+      if (g >= kRing) mbar_wait(&empty[stage], uint32_t((g / kRing - 1) & 1));
+      mbar_arrive_expect_tx(&full[stage], kChunkBytes);
+      bulk_g2s(bring + stage * kChunkBytes, p.bimg + size_t(g % nk) * kChunkBytes, kChunkBytes, &full[stage]);
+    }
+    return;
+  }
+  setmaxnreg_inc<kConsumerRegs>();
+  const int wgi = role - 1, t = tid & 127, warp = t >> 5, lane = tid & 31;
+  // chunk g's W stage is free again
   auto release = [&](int64_t g) {
     if (lane == 0) mbar_arrive(&empty[g % kRing]);
-    if (tid == 0 && g + kRing < total) {
-      mbar_wait(&empty[g % kRing], uint32_t((g / kRing) & 1));
-      issue(g + kRing);
-    }
   };
-  if (tid == 0)
-    for (int64_t g = 0; g < total && g < kRing; ++g) issue(g);
 
-  // producer geometry: thread t writes 8 consecutive k (half kh) of row pr of its warpgroup's 64
+  // A geometry: thread t writes 8 consecutive k (half kh) of row pr of its warpgroup's 64
   const int pr = t >> 1, kh = t & 1;
   const uint32_t a_off = uint32_t(pr >> 3) * 256u + uint32_t(kh) * 128u + uint32_t(pr & 7) * 16u;
   uint8_t* my_a = abuf + wgi * 2 * kABytes;
@@ -173,21 +205,28 @@ __global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
     auto put = [&](int buf, const float4 (&q)[2], int kc) {
       const int k0 = kc * 16 + kh * 8;
       float v[8] = {q[0].x, q[0].y, q[0].z, q[0].w, q[1].x, q[1].y, q[1].z, q[1].w};
+      // w1x rows are kp (a multiple of 16) floats long, so this thread's 8 k of every row are 32-byte aligned
       if (kProd == PROD_GNN) {
+        float wx[8], wy[8], wz[8];
+        ldg8(p.w1x + k0, wx);
+        ldg8(p.w1x + p.kp + k0, wy);
+        ldg8(p.w1x + 2 * p.kp + k0, wz);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int k = k0 + i;
-          v[i] = fmaxf(fmaf(rz, __ldg(p.w1x + 2 * p.kp + k), fmaf(ry, __ldg(p.w1x + p.kp + k), fmaf(rx, __ldg(p.w1x + k), v[i]))), 0.0f);
-        }
+        for (int i = 0; i < 8; ++i) v[i] = fmaxf(fmaf(rz, wz[i], fmaf(ry, wy[i], fmaf(rx, wx[i], v[i]))), 0.0f);
       } else if (kProd == PROD_POOL) {
+        float wf[8], wx[8], wy[8], wz[8], b0[8];
+        ldg8(p.w1x + k0, wf);
+        ldg8(p.w1x + p.kp + k0, wx);
+        ldg8(p.w1x + 2 * p.kp + k0, wy);
+        ldg8(p.w1x + 3 * p.kp + k0, wz);
+        ldg8(p.w1x + 4 * p.kp + k0, b0);
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          const int k = k0 + i;
-          float a = __ldg(p.w1x + 4 * p.kp + k);
-          a = fmaf(f0, __ldg(p.w1x + k), a);
-          a = fmaf(rx, __ldg(p.w1x + p.kp + k), a);
-          a = fmaf(ry, __ldg(p.w1x + 2 * p.kp + k), a);
-          a = fmaf(rz, __ldg(p.w1x + 3 * p.kp + k), a);
+          float a = b0[i];
+          a = fmaf(f0, wf[i], a);
+          a = fmaf(rx, wx[i], a);
+          a = fmaf(ry, wy[i], a);
+          a = fmaf(rz, wz[i], a);
           v[i] = fmaxf(a, 0.0f);
         }
       }
@@ -222,17 +261,17 @@ __global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
         wgmma_bf16<NI>(acc[i], a_hi, b_lo, 1);
       }
       wgmma_commit();
+      // every iteration leaves exactly chunk kc in flight: a wait on a path of its own (the last chunk's) would make
+      // ptxas drain the wgmmas at the end of every iteration
+      wgmma_wait<1>();                    // chunk kc - 1 complete: its A buffer and W stage are free
+      if (kc > 0) release(g - 1);
       if (kc + 1 < nk) {
-        wgmma_wait<1>();                  // chunk kc - 1 complete: its A buffer and W stage are free
-        if (kc > 0) release(g - 1);
         put((kc + 1) & 1, q, kc + 1);
         if (kc + 2 < nk) load(kc + 2, q);
-      } else {
-        wgmma_wait<0>();
-        if (kc > 0) release(g - 1);
-        release(g);
       }
     }
+    wgmma_wait<0>();
+    release(g - 1);
     // ---- epilogue ----------------------------------------------------------------------------------
     const int64_t r0 = tile * kTileRows + wgi * 64 + warp * 16 + (lane >> 2);
     const int cq = (lane & 3) * 2;
@@ -365,7 +404,7 @@ WgShape wg_shape(int k, int n) {
   else if (t.np <= 256) { t.ni = 128; t.ns = 2; }
   else if (t.np <= kMaxNT) { t.ni = 152; t.ns = 2; }
   t.nt = t.ni * t.ns;
-  t.smem = size_t(kRing) * t.nt * 64 + 4 * kABytes + 2 * kRing * sizeof(uint64_t);
+  t.smem = wg_smem_bytes(t.nt, ring_stages(t.nt));
   t.ok = t.nt > 0 && k >= 1 && n >= 1;
   return t;
 }

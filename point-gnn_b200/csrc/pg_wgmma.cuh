@@ -61,6 +61,17 @@ __device__ __forceinline__ void warpgroup_sync(int id) {
   asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory");
 }
 
+// ---- per-warpgroup register budget ---------------------------------------------------------------
+// Every thread of the warpgroup executes the same one; the CTA's register pool must hold what .inc asks for.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+
 // ---- wgmma -------------------------------------------------------------------------------------
 // Shared-memory matrix descriptor, K-major operand, no swizzle ("interleave"): the operand is a grid of
 // 8-row x 16-byte core matrices (128 contiguous bytes each, row r of the core at +16*r).

@@ -1,6 +1,6 @@
 #!/bin/bash
 # Experiment build of the library: tools/build_variant.sh NAME [-DFLAG ...]  ->  lab/NAME.so (git-ignored, travels to
-# the GPU machine).  Used with PG_LIB_VARIANT=NAME tools/prof_pool.py / tools/prof_graph.py.
+# the GPU machine).  Used with PG_LIB_VARIANT=NAME tools/prof_edge.py / tools/prof_pool.py / tools/prof_graph.py.
 set -e
 name=$1; shift
 cd "$(dirname "$0")/../point-gnn_b200/csrc"
