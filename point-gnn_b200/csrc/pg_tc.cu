@@ -311,20 +311,42 @@ __global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
       }
       const int dw = __shfl_sync(0xffffffffu, d[0], 0);
       if (__all_sync(0xffffffffu, d[0] == dw && d[1] == dw) && dw >= 0) {
-        // the warp's 16 rows are one destination: combine the halves, then the 8 lanes sharing columns
+        // the warp's 16 rows are one destination.  Value v of a thread is column (v / 2) * 8 + cq + v % 2; the 8
+        // lanes sharing cq (lane bits 4, 3, 2) reduce-scatter their V values in three halving exchanges, after which
+        // every lane holds the full maxima of V / 8 (rounded up or down) of them and all 32 lanes flush
+        constexpr int V = NT / 4, L1 = V / 2, L2 = V / 4, L3 = (L2 + 1) / 2;
+        static_assert(V % 4 == 0, "the first two exchanges halve evenly");
+        float m[V];
 #pragma unroll
         for (int i = 0; i < NS; ++i)
 #pragma unroll
           for (int jj = 0; jj < NI / 8; ++jj)
 #pragma unroll
-            for (int c = 0; c < 2; ++c) {
-              float m = fmaxf(acc[i][4 * jj + c], acc[i][4 * jj + 2 + c]);
-              m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
-              m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 8));
-              m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 16));
-              const int col = i * NI + jj * 8 + cq + c;
-              if (lane < 4 && col < p.n) seg_flush(p, dw, col, m);
-            }
+            for (int c = 0; c < 2; ++c) m[(i * (NI / 8) + jj) * 2 + c] = fmaxf(acc[i][4 * jj + c], acc[i][4 * jj + 2 + c]);
+        const bool b4 = lane & 16, b3 = lane & 8, b2 = lane & 4;
+        // a lane with the bit set keeps the upper part, its partner the lower; each sends the part it gives up
+#pragma unroll
+        for (int k = 0; k < L1; ++k) {
+          const float keep = b4 ? m[k + L1] : m[k], give = b4 ? m[k] : m[k + L1];
+          m[k] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, give, 16));
+        }
+#pragma unroll
+        for (int k = 0; k < L2; ++k) {
+          const float keep = b3 ? m[k + L2] : m[k], give = b3 ? m[k] : m[k + L2];
+          m[k] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, give, 8));
+        }
+#pragma unroll
+        for (int k = 0; k < L3; ++k) {
+          const float up = k + L3 < L2 ? m[k + L3] : m[k];   // L2 odd: the upper part is one value shorter
+          const float keep = b2 ? up : m[k], give = b2 ? m[k] : up;
+          m[k] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, give, 4));
+        }
+        const int v0 = (b4 ? L1 : 0) + (b3 ? L2 : 0) + (b2 ? L3 : 0), nv = b2 ? L2 - L3 : L3;
+#pragma unroll
+        for (int k = 0; k < L3; ++k) {
+          const int v = v0 + k, col = (v >> 1) * 8 + cq + (v & 1);
+          if (k < nv && col < p.n) seg_flush(p, dw, col, m[k]);
+        }
       } else {
         // segmented max down each 8-row half (rows of one destination are contiguous); the first row of
         // every run flushes the run's max
