@@ -99,6 +99,32 @@ __device__ __forceinline__ void atomic_max_float(float* addr, float v) {
     atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(v));
 }
 
+// float <-> order-preserving uint: a < b iff float_to_ordered(a) < float_to_ordered(b), for any non-NaN values
+__device__ inline uint32_t float_to_ordered(float f) {
+  uint32_t b = __float_as_uint(f);
+  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+__device__ inline float ordered_to_float(uint32_t u) {
+  uint32_t b = (u & 0x80000000u) ? (u & 0x7fffffffu) : ~u;
+  return __uint_as_float(b);
+}
+
+// the frame f with frame_ptr[f] <= row < frame_ptr[f + 1] (rows past the end fall into the last frame)
+__device__ inline int find_frame(const int32_t* __restrict__ frame_ptr, int num_frames, int64_t row) {
+  int lo = 0, hi = num_frames;  // invariant: frame_ptr[lo] <= row < frame_ptr[hi]
+  while (hi - lo > 1) {
+    int mid = (lo + hi) >> 1;
+    if (frame_ptr[mid] <= row) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
+// pg_api.cu: CUB device-wide scans and the stable radix sort of (key, value) pairs over bits [0, end_bit), each with
+// a stream-ordered temporary; they count their launches (scan 2, sort 4)
+int exclusive_sum(const int32_t* in, int32_t* out, int64_t n, cudaStream_t s);
+int inclusive_sum(const int32_t* in, int32_t* out, int64_t n, cudaStream_t s);
+int sort_pairs(const uint64_t* keys_in, uint64_t* keys_out, const int32_t* vals_in, int32_t* vals_out, int64_t n,
+               int end_bit, cudaStream_t s);
 // pg_ops.cu
 int fill_async(float* p, int64_t n, float v, cudaStream_t s);
 // out [m, ldo] = act(x [m, k] @ w [k, n] + bias) (+ residual [m, n]); columns [n, ldo) are written as zeros

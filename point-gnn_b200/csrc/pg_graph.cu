@@ -14,8 +14,6 @@
 // nearest point, radius test) are evaluated in fp64 with explicitly rounded mul/add
 // (no FMA contraction), which is what makes the edge lists bit-exact against the reference's
 // scikit-learn float64 trees.
-#include <cub/cub.cuh>
-
 #include "pg_common.cuh"
 
 namespace pg {
@@ -32,25 +30,6 @@ constexpr int kErrParking = 8;     // pg_multi_level_graph: hit parking buffer t
 
 __host__ __device__ inline uint64_t make_key(uint32_t frame, uint32_t iz, uint32_t iy, uint32_t ix) {
   return (uint64_t(frame) << 48) | (uint64_t(iz) << 32) | (uint64_t(iy) << 16) | uint64_t(ix);
-}
-
-// float <-> order-preserving uint (for atomicMin on floats)
-__device__ inline uint32_t float_to_ordered(float f) {
-  uint32_t b = __float_as_uint(f);
-  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__device__ inline float ordered_to_float(uint32_t u) {
-  uint32_t b = (u & 0x80000000u) ? (u & 0x7fffffffu) : ~u;
-  return __uint_as_float(b);
-}
-
-__device__ inline int find_frame(const int32_t* __restrict__ frame_ptr, int num_frames, int64_t row) {
-  int lo = 0, hi = num_frames;  // invariant: frame_ptr[lo] <= row < frame_ptr[hi]
-  while (hi - lo > 1) {
-    int mid = (lo + hi) >> 1;
-    if (frame_ptr[mid] <= row) lo = mid; else hi = mid;
-  }
-  return lo;
 }
 
 // ---- per-frame bounding-box minimum ---------------------------------------------------------
@@ -567,7 +546,7 @@ __global__ void gather_keypoints_kernel(const float* __restrict__ xyz, const int
 
 // ---- host-side building blocks ----------------------------------------------------------------
 struct BuiltGrid {
-  Temp bounds, keys_a, keys_b, vals_a, vals_b, sorted_pts, head, head_scan, cell_key, cell_start, cub_tmp, err;
+  Temp bounds, keys_a, keys_b, vals_a, vals_b, sorted_pts, head, head_scan, cell_key, cell_start, err;
   SortedGrid view{};
 };
 
@@ -606,21 +585,13 @@ int build_grid(const float* xyz, const int32_t* frame_ptr, int num_frames, int64
                                                       out->err.as<int>());
   PG_LAUNCH_CHECK();
   // radix sort (key, original index); stable, so equal keys keep ascending point index
-  const int end_bit = 48 + frame_bits(num_frames);
-  size_t tmp_bytes = 0;
-  PG_CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, out->keys_a.as<uint64_t>(), out->keys_b.as<uint64_t>(),
-                                             out->vals_a.as<int32_t>(), out->vals_b.as<int32_t>(), int(n), 0, end_bit, s));
-  size_t scan_bytes = 0;
-  PG_CUDA_OK(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, out->head.as<int32_t>(), out->head_scan.as<int32_t>(), int(n), s));
-  PG_CUDA_OK(out->cub_tmp.alloc(std::max(tmp_bytes, scan_bytes), s));
-  PG_CUDA_OK(cub::DeviceRadixSort::SortPairs(out->cub_tmp.ptr, tmp_bytes, out->keys_a.as<uint64_t>(), out->keys_b.as<uint64_t>(),
-                                             out->vals_a.as<int32_t>(), out->vals_b.as<int32_t>(), int(n), 0, end_bit, s));
-  count_launch(4);
+  if (int rc = sort_pairs(out->keys_a.as<uint64_t>(), out->keys_b.as<uint64_t>(), out->vals_a.as<int32_t>(),
+                          out->vals_b.as<int32_t>(), n, 48 + frame_bits(num_frames), s))
+    return rc;
   gather_sorted_kernel<<<ceil_div(n, 256), 256, 0, s>>>(xyz, out->keys_b.as<uint64_t>(), out->vals_b.as<int32_t>(), n,
                                                          out->sorted_pts.as<float4>(), out->head.as<int32_t>());
   PG_LAUNCH_CHECK();
-  PG_CUDA_OK(cub::DeviceScan::InclusiveSum(out->cub_tmp.ptr, scan_bytes, out->head.as<int32_t>(), out->head_scan.as<int32_t>(), int(n), s));
-  count_launch(2);
+  if (int rc = inclusive_sum(out->head.as<int32_t>(), out->head_scan.as<int32_t>(), n, s)) return rc;
   cell_table_kernel<<<ceil_div(n, 256), 256, 0, s>>>(out->keys_b.as<uint64_t>(), out->head_scan.as<int32_t>(), n,
                                                       out->cell_key.as<uint64_t>(), out->cell_start.as<int32_t>());
   PG_LAUNCH_CHECK();
@@ -773,7 +744,7 @@ int radius_ranges(RadiusPlan& plan, const float* centers, const int32_t* center_
 int radius_count_rows(RadiusPlan& plan, const float* centers, const int32_t* center_frame_ptr, int num_frames,
                       int64_t num_centers, Temp* ranges, int32_t* out_row_ptr, int64_t* out_num_edges_host,
                       cudaStream_t s) {
-  Temp counts, tmp, total;
+  Temp counts, total;
   PG_CUDA_OK(counts.alloc(sizeof(int32_t) * (num_centers + 1), s));
   PG_CUDA_OK(cudaMemsetAsync(counts.ptr, 0, sizeof(int32_t) * (num_centers + 1), s));
   PG_CUDA_OK(total.alloc(sizeof(unsigned long long), s));
@@ -782,11 +753,7 @@ int radius_count_rows(RadiusPlan& plan, const float* centers, const int32_t* cen
   if (int rc = radius_collect(plan, centers, num_centers, nullptr, ranges->as<int32_t>(), nullptr, 0, nullptr,
                               counts.as<int32_t>(), total.as<unsigned long long>(), s))
     return rc;
-  size_t bytes = 0;
-  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, bytes, counts.as<int32_t>(), out_row_ptr, int(num_centers + 1), s));
-  PG_CUDA_OK(tmp.alloc(bytes, s));
-  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(tmp.ptr, bytes, counts.as<int32_t>(), out_row_ptr, int(num_centers + 1), s));
-  count_launch(2);
+  if (int rc = exclusive_sum(counts.as<int32_t>(), out_row_ptr, num_centers + 1, s)) return rc;
   unsigned long long h_total = 0;
   int32_t h_err = 0;
   PG_CUDA_OK(cudaMemcpyAsync(&h_total, total.ptr, sizeof(h_total), cudaMemcpyDeviceToHost, s));
@@ -818,7 +785,7 @@ int radius_level_device(RadiusPlan& plan, const float* centers, const int32_t* c
   // candidates per row are ~6.5x the hits (27 cells of edge r against the ball of radius r); the parking buffer is
   // sized from the caller's edge capacity and its overflow is reported like an edge-buffer overflow
   const int64_t tmp_capacity = std::min<int64_t>(capacity * 10 + 4096, (int64_t(1) << 31) - 1);
-  Temp counts, cand, cand_off, ranges, parked, tmp;
+  Temp counts, cand, cand_off, ranges, parked;
   PG_CUDA_OK(counts.alloc(sizeof(int32_t) * (kp_capacity + 1), s));
   PG_CUDA_OK(cudaMemsetAsync(counts.ptr, 0, sizeof(int32_t) * (kp_capacity + 1), s));
   PG_CUDA_OK(cand.alloc(sizeof(int32_t) * (kp_capacity + 1), s));
@@ -828,16 +795,11 @@ int radius_level_device(RadiusPlan& plan, const float* centers, const int32_t* c
   if (int rc = radius_candidates(plan, centers, center_frame_ptr, num_frames, kp_capacity, num_centers_dev,
                                  ranges.as<int32_t>(), cand.as<int32_t>(), s))
     return rc;
-  size_t bytes = 0;
-  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, bytes, cand.as<int32_t>(), cand_off.as<int32_t>(), int(kp_capacity + 1), s));
-  PG_CUDA_OK(tmp.alloc(bytes, s));
-  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(tmp.ptr, bytes, cand.as<int32_t>(), cand_off.as<int32_t>(), int(kp_capacity + 1), s));
-  count_launch(2);
+  if (int rc = exclusive_sum(cand.as<int32_t>(), cand_off.as<int32_t>(), kp_capacity + 1, s)) return rc;
   if (int rc = radius_collect(plan, centers, kp_capacity, num_centers_dev, ranges.as<int32_t>(), cand_off.as<int32_t>(),
                               tmp_capacity, parked.as<int32_t>(), counts.as<int32_t>(), total64, s))
     return rc;
-  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(tmp.ptr, bytes, counts.as<int32_t>(), out_row_ptr, int(kp_capacity + 1), s));
-  count_launch(2);
+  if (int rc = exclusive_sum(counts.as<int32_t>(), out_row_ptr, kp_capacity + 1, s)) return rc;
   // rows beyond the real number of centres are empty, so row_ptr[c] == E for every c >= K
   return sort_rows(out_row_ptr, kp_capacity, out_src, out_dst, capacity, parked.as<int32_t>(), cand_off.as<int32_t>(), s);
 }
@@ -1221,24 +1183,19 @@ extern "C" int pg_random_keypoints(const float* xyz, const int32_t* frame_ptr, i
   if (int rc = build_grid(xyz, frame_ptr, num_frames, num_points, spec, s, &grid)) return rc;
   // second sort: the voxels in order of first appearance
   const int64_t n = num_points;
-  Temp keys2a, keys2b, vals2a, vals2b, tmp;
+  Temp keys2a, keys2b, vals2a, vals2b;
   PG_CUDA_OK(keys2a.alloc(sizeof(uint64_t) * n, s));
   PG_CUDA_OK(keys2b.alloc(sizeof(uint64_t) * n, s));
   PG_CUDA_OK(vals2a.alloc(sizeof(int32_t) * n, s));
   PG_CUDA_OK(vals2b.alloc(sizeof(int32_t) * n, s));
-  const int end_bit = 32 + frame_bits(num_frames);
-  size_t bytes = 0;
-  PG_CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, bytes, keys2a.as<uint64_t>(), keys2b.as<uint64_t>(), vals2a.as<int32_t>(),
-                                             vals2b.as<int32_t>(), int(n), 0, end_bit, s));
-  PG_CUDA_OK(tmp.alloc(bytes, s));
   const int32_t* sorted_idx = grid.vals_b.as<int32_t>();
   voxel_first_keys_kernel<<<ceil_div(n, 256), 256, 0, s>>>(grid.view.cell_key, grid.view.cell_start, sorted_idx,
                                                             grid.view.num_cells, n, num_frames, keys2a.as<uint64_t>(),
                                                             vals2a.as<int32_t>());
   PG_LAUNCH_CHECK();
-  PG_CUDA_OK(cub::DeviceRadixSort::SortPairs(tmp.ptr, bytes, keys2a.as<uint64_t>(), keys2b.as<uint64_t>(), vals2a.as<int32_t>(),
-                                             vals2b.as<int32_t>(), int(n), 0, end_bit, s));
-  count_launch(4);
+  if (int rc = sort_pairs(keys2a.as<uint64_t>(), keys2b.as<uint64_t>(), vals2a.as<int32_t>(), vals2b.as<int32_t>(), n,
+                          32 + frame_bits(num_frames), s))
+    return rc;
   random_pick_kernel<<<ceil_div(n, 256), 256, 0, s>>>(vals2b.as<int32_t>(), grid.view.cell_start, sorted_idx,
                                                        grid.view.num_cells, uniform, capacity, out_keypoint_idx);
   PG_LAUNCH_CHECK();
@@ -1252,15 +1209,11 @@ extern "C" int pg_cap_neighbors(const int32_t* row_ptr, const int32_t* src, int6
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   PG_REQUIRE(row_ptr && out_row_ptr && out_num_edges_host && num_rows >= 1 && num_neighbors >= 1,
              "pg_cap_neighbors: bad argument");
-  Temp counts, tmp;
+  Temp counts;
   PG_CUDA_OK(counts.alloc(sizeof(int32_t) * (num_rows + 1), s));
   capped_counts_kernel<<<ceil_div(num_rows + 1, 256), 256, 0, s>>>(row_ptr, num_rows, num_neighbors, counts.as<int32_t>());
   PG_LAUNCH_CHECK();
-  size_t bytes = 0;
-  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, bytes, counts.as<int32_t>(), out_row_ptr, int(num_rows + 1), s));
-  PG_CUDA_OK(tmp.alloc(bytes, s));
-  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(tmp.ptr, bytes, counts.as<int32_t>(), out_row_ptr, int(num_rows + 1), s));
-  count_launch(2);
+  if (int rc = exclusive_sum(counts.as<int32_t>(), out_row_ptr, num_rows + 1, s)) return rc;
   int32_t h_e = 0;
   PG_CUDA_OK(cudaMemcpyAsync(&h_e, out_row_ptr + num_rows, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
   PG_CUDA_OK(cudaStreamSynchronize(s));

@@ -11,8 +11,6 @@
 // are ([M, 4] float32) and everything after that runs here.  Output order = input order (stable compaction).
 #include <vector>
 
-#include <cub/cub.cuh>
-
 #include "pg_common.cuh"
 
 namespace pg {
@@ -123,7 +121,7 @@ extern "C" int pg_cam_points_in_image(const float* velo_points, const int32_t* f
     h[f].height = image_size_host[2 * f + 1];
     PG_REQUIRE(h[f].width > 0 && h[f].height > 0, "pg_cam_points_in_image: bad image size of frame %d", f);
   }
-  Temp calib, cam, uv, flags, slot, tmp, offs;
+  Temp calib, cam, uv, flags, slot, offs;
   PG_CUDA_OK(calib.alloc(sizeof(FrameCalib) * num_frames, s));
   PG_CUDA_OK(cudaMemcpyAsync(calib.ptr, h.data(), sizeof(FrameCalib) * num_frames, cudaMemcpyHostToDevice, s));
   if (attr_channels == 4) {
@@ -138,11 +136,7 @@ extern "C" int pg_cam_points_in_image(const float* velo_points, const int32_t* f
                                                            calib.as<FrameCalib>(), cam.as<float>(), uv.as<float>(),
                                                            flags.as<int32_t>());
   PG_LAUNCH_CHECK();
-  size_t bytes = 0;
-  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, bytes, flags.as<int32_t>(), slot.as<int32_t>(), int(num_points + 1), s));
-  PG_CUDA_OK(tmp.alloc(bytes, s));
-  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(tmp.ptr, bytes, flags.as<int32_t>(), slot.as<int32_t>(), int(num_points + 1), s));
-  count_launch(2);
+  if (int rc = exclusive_sum(flags.as<int32_t>(), slot.as<int32_t>(), num_points + 1, s)) return rc;
   cam_compact_kernel<<<ceil_div(std::max<int64_t>(num_points, num_frames + 1), 256), 256, 0, s>>>(
       velo_points, frame_ptr, num_frames, num_points, calib.as<FrameCalib>(), cam.as<float>(), uv.as<float>(),
       flags.as<int32_t>(), slot.as<int32_t>(), images, offs.as<int64_t>(), attr_channels, capacity, out_xyz, out_attr,

@@ -13,15 +13,15 @@
 //                             score grows by sum_j score_j * IoU(median box, box_j) (rescore)
 //
 // The reference's loop is sequential over boxes; here only the cheap part is:
-//   1. flag + exclusive scan + decode/scatter   candidates in ascending (vertex, class) order per frame
-//   2. stable radix sort by (frame, score desc)  = bboxes_sort, ties in ascending flat index
+//   1. candidates: pg_postprocess flags, scans, decodes (decode_box, the rule pg_decode_boxes uses) and scatters them
+//      in ascending (vertex, class) order per frame; pg_nms_boxes_3d takes the caller's boxes as they are.  Either
+//      way the result is one Candidates set that nms_stage runs stages 2-6 on.
+//   2. stable radix sort by (frame, score desc)  = bboxes_sort, ties in ascending candidate position
 //   3. geometry per candidate (corners, extents) and the pairwise same-class "IoU > threshold" bit matrix,
 //      all pairs of a frame in parallel over the whole GPU
 //   4. sweep: one warp per frame walks the sorted list with bit operations only (who is kept, whom it removes)
 //   5. merge + rescore: one block per kept box (median by rank selection, IoU with the merged box)
 //   6. compaction of the kept boxes per frame
-#include <cub/cub.cuh>
-
 #include "pg_common.cuh"
 
 namespace pg {
@@ -47,16 +47,34 @@ __global__ void flag_candidates_kernel(const float* __restrict__ probs, int64_t 
   flags[i] = (c > 0 && c < num_classes - 1 && double(probs[i]) > 1.0 / double(num_classes)) ? 1 : 0;
 }
 
-__device__ inline int find_frame_of(const int32_t* __restrict__ frame_ptr, int num_frames, int64_t row) {
-  int lo = 0, hi = num_frames;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (frame_ptr[mid] <= row) lo = mid; else hi = mid;
+// classaware_all_class_box_decoding of (vertex, class c): the encoding e [7] at the vertex position p [3] -> b [7]
+// (box_encoding.py:276-298, float32 arithmetic in NumPy's order)
+__device__ __forceinline__ void decode_box(const float* __restrict__ e, const float* __restrict__ p, const ClassTable& tab,
+                                           int c, float* b) {
+#pragma unroll
+  for (int j = 0; j < kBoxLen; ++j) b[j] = e[j];
+  if (tab.decoded[c]) {
+    const float pi4 = float(M_PI * 0.25), pi2 = float(0.5 * M_PI);
+    b[0] = __fmul_rn(e[0], tab.l[c]);
+    b[1] = __fmul_rn(e[1], tab.h[c]);
+    b[2] = __fmul_rn(e[2], tab.w[c]);
+    b[3] = __fmul_rn(expf(e[3]), tab.l[c]);
+    b[4] = __fmul_rn(expf(e[4]), tab.h[c]);
+    b[5] = __fmul_rn(expf(e[5]), tab.w[c]);
+    b[6] = __fmul_rn(e[6], pi4);
+    if (tab.yaw0[c] != 0.0f) b[6] = __fadd_rn(b[6], pi2);
   }
-  return lo;
+  b[0] = __fadd_rn(b[0], p[0]);
+  b[1] = __fadd_rn(b[1], p[1]);
+  b[2] = __fadd_rn(b[2], p[2]);
 }
 
-// decode + scatter in flat (vertex, class) order; also the sort key (frame | descending score)
+// sort key of a candidate: frame, then score descending
+__device__ __forceinline__ uint64_t sort_key(int frame, float score) {
+  return (uint64_t(uint32_t(frame)) << 32) | uint64_t(~float_to_ordered(score));
+}
+
+// decode + scatter in flat (vertex, class) order, with the sort key
 __global__ void decode_scatter_kernel(const float* __restrict__ probs, const float* __restrict__ enc,
                                       const float* __restrict__ xyz, const int32_t* __restrict__ frame_ptr,
                                       int num_frames, int64_t num_vertices, int num_classes, ClassTable tab,
@@ -71,34 +89,30 @@ __global__ void decode_scatter_kernel(const float* __restrict__ probs, const flo
   const int64_t v = i / num_classes;
   const int c = int(i - v * num_classes);
   const int s = slot_of[i];
-  const float* e = enc + i * kBoxLen;
   float b[kBoxLen];
-#pragma unroll
-  for (int j = 0; j < kBoxLen; ++j) b[j] = e[j];
-  if (tab.decoded[c]) {    // box_encoding.py:276-291, float32 arithmetic
-    const float pi4 = float(M_PI * 0.25), pi2 = float(0.5 * M_PI);
-    b[0] = __fmul_rn(e[0], tab.l[c]);
-    b[1] = __fmul_rn(e[1], tab.h[c]);
-    b[2] = __fmul_rn(e[2], tab.w[c]);
-    b[3] = __fmul_rn(expf(e[3]), tab.l[c]);
-    b[4] = __fmul_rn(expf(e[4]), tab.h[c]);
-    b[5] = __fmul_rn(expf(e[5]), tab.w[c]);
-    b[6] = __fmul_rn(e[6], pi4);
-    if (tab.yaw0[c] != 0.0f) b[6] = __fadd_rn(b[6], pi2);
-  }
-  b[0] = __fadd_rn(b[0], xyz[3 * v + 0]);   // box_encoding.py:293-298
-  b[1] = __fadd_rn(b[1], xyz[3 * v + 1]);
-  b[2] = __fadd_rn(b[2], xyz[3 * v + 2]);
+  decode_box(enc + i * kBoxLen, xyz + 3 * v, tab, c, b);
 #pragma unroll
   for (int j = 0; j < kBoxLen; ++j) cand_box[int64_t(s) * kBoxLen + j] = b[j];
   const float p = probs[i];
   cand_score[s] = p;
   cand_label[s] = fold_label(c);
   cand_index[s] = int32_t(i);
-  const int f = find_frame_of(frame_ptr, num_frames, v);
-  // probabilities are positive: the bit pattern (sign bit set, as in candidate_keys_kernel) is monotonic
-  keys[s] = (uint64_t(uint32_t(f)) << 32) | uint64_t(~(__float_as_uint(p) | 0x80000000u));
+  const int f = find_frame(frame_ptr, num_frames, v);
+  keys[s] = sort_key(f, p);
   vals[s] = s;
+  atomicAdd(&frame_count[f], 1);
+}
+
+// sort keys of caller-provided candidates (pg_nms_boxes_3d), value = position
+__global__ void candidate_keys_kernel(const float* __restrict__ score, const int32_t* __restrict__ frame_ptr, int num_frames,
+                                      int64_t n, uint64_t* __restrict__ keys, int32_t* __restrict__ vals,
+                                      int32_t* __restrict__ frame_count, int32_t* __restrict__ index) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int f = find_frame(frame_ptr, num_frames, i);
+  keys[i] = sort_key(f, score[i]);
+  vals[i] = int32_t(i);
+  index[i] = int32_t(i);
   atomicAdd(&frame_count[f], 1);
 }
 
@@ -109,24 +123,8 @@ __global__ void decode_all_kernel(const float* __restrict__ enc, const float* __
   if (i >= num_vertices * num_classes) return;
   const int64_t v = i / num_classes;
   const int c = int(i - v * num_classes);
-  const float* e = enc + i * kBoxLen;
   float b[kBoxLen];
-#pragma unroll
-  for (int j = 0; j < kBoxLen; ++j) b[j] = e[j];
-  if (tab.decoded[c]) {
-    const float pi4 = float(M_PI * 0.25), pi2 = float(0.5 * M_PI);
-    b[0] = __fmul_rn(e[0], tab.l[c]);
-    b[1] = __fmul_rn(e[1], tab.h[c]);
-    b[2] = __fmul_rn(e[2], tab.w[c]);
-    b[3] = __fmul_rn(expf(e[3]), tab.l[c]);
-    b[4] = __fmul_rn(expf(e[4]), tab.h[c]);
-    b[5] = __fmul_rn(expf(e[5]), tab.w[c]);
-    b[6] = __fmul_rn(e[6], pi4);
-    if (tab.yaw0[c] != 0.0f) b[6] = __fadd_rn(b[6], pi2);
-  }
-  b[0] = __fadd_rn(b[0], xyz[3 * v + 0]);
-  b[1] = __fadd_rn(b[1], xyz[3 * v + 1]);
-  b[2] = __fadd_rn(b[2], xyz[3 * v + 2]);
+  decode_box(enc + i * kBoxLen, xyz + 3 * v, tab, c, b);
 #pragma unroll
   for (int j = 0; j < kBoxLen; ++j) out[i * kBoxLen + j] = b[j];
 }
@@ -137,6 +135,20 @@ __global__ void fill_tail_keys_kernel(const int32_t* __restrict__ total, int64_t
   if (i >= capacity || i < *total) return;
   keys[i] = ~0ull;
   vals[i] = int32_t(i);
+}
+
+// ---- 2. sort ---------------------------------------------------------------------------------------
+// one thread: ptr = exclusive scan of the per-frame counts (ptr[num_frames] = all candidates), and
+// counts[num_frames] = the largest count
+__global__ void frame_ptr_kernel(int32_t* __restrict__ counts, int num_frames, int32_t* __restrict__ ptr) {
+  int acc = 0, widest = 0;
+  for (int f = 0; f < num_frames; ++f) {
+    ptr[f] = acc;
+    acc += counts[f];
+    widest = max(widest, counts[f]);
+  }
+  ptr[num_frames] = acc;
+  counts[num_frames] = widest;
 }
 
 // ---- 3. geometry -----------------------------------------------------------------------------------
@@ -310,7 +322,7 @@ __global__ void __launch_bounds__(kMergeThreads) merge_rescore_kernel(
   for (int i = blockIdx.x; i < *total; i += gridDim.x) {
     __syncthreads();
     if (!kept[i]) continue;                                   // uniform
-    const int f = find_frame_of(cand_frame_ptr, num_frames, i);
+    const int f = find_frame(cand_frame_ptr, num_frames, i);
     const int begin = cand_frame_ptr[f];
     const int li = i - begin;
     const uint32_t* row = adj + int64_t(i) * words;
@@ -403,14 +415,6 @@ __global__ void compact_kernel(const int32_t* __restrict__ total, const int32_t*
   for (int j = 0; j < kBoxLen; ++j) det_box[int64_t(o) * kBoxLen + j] = out_box[int64_t(i) * kBoxLen + j];
 }
 
-__global__ void frame_ptr_from_counts_kernel(const int32_t* __restrict__ counts, int num_frames, int32_t* __restrict__ ptr) {
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    int acc = 0;
-    for (int f = 0; f < num_frames; ++f) { ptr[f] = acc; acc += counts[f]; }
-    ptr[num_frames] = acc;
-  }
-}
-
 __global__ void det_frame_ptr_kernel(const int32_t* __restrict__ cand_frame_ptr, int num_frames,
                                      const int32_t* __restrict__ kept_scan, int32_t* __restrict__ det_frame_ptr) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
@@ -418,71 +422,74 @@ __global__ void det_frame_ptr_kernel(const int32_t* __restrict__ cand_frame_ptr,
   det_frame_ptr[f] = kept_scan[cand_frame_ptr[f]];     // kept_scan has total + 1 entries (exclusive scan)
 }
 
-// sort keys of caller-provided candidates (pg_nms_boxes_3d): (frame | descending score), value = position
-__global__ void candidate_keys_kernel(const float* __restrict__ score, const int32_t* __restrict__ frame_ptr, int num_frames,
-                                      int64_t n, uint64_t* __restrict__ keys, int32_t* __restrict__ vals,
-                                      int32_t* __restrict__ frame_count, int32_t* __restrict__ index) {
-  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const int f = find_frame_of(frame_ptr, num_frames, i);
-  // any finite score: order-preserving map of the float bits, complemented for descending order
-  const uint32_t b = __float_as_uint(score[i]);
-  const uint32_t ordered = (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-  keys[i] = (uint64_t(uint32_t(f)) << 32) | uint64_t(~ordered);
-  vals[i] = int32_t(i);
-  index[i] = int32_t(i);
-  atomicAdd(&frame_count[f], 1);
-}
+// The candidate boxes of a batch: the input of stages 2-6.  box / score / label / index are indexed by candidate
+// position (frame by frame); the sort runs over sort_n entries, the keys of any entries past the candidates sort last.
+struct Candidates {
+  const float* box = nullptr;            // [n, 7]
+  const float* score = nullptr;          // [n]
+  const int32_t* label = nullptr;        // [n]
+  Temp index;                            // int32 [n]: flat (vertex, class) index, or the position in the caller's arrays
+  Temp keys_a, keys_b, vals_a, vals_b;   // sort input and output: sort_key -> candidate position
+  Temp frame_count;                      // int32 [num_frames + 1]: candidates per frame, then the largest count
+  Temp frame_ptr;                        // int32 [num_frames + 1]: frame_ptr[num_frames] = number of candidates
+  int64_t sort_n = 0;
+  int num_frames = 0;
 
-__global__ void max_frame_count_kernel(const int32_t* __restrict__ counts, int num_frames, int32_t* __restrict__ out) {
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    int m = 0;
-    for (int f = 0; f < num_frames; ++f) m = max(m, counts[f]);
-    *out = m;
+  // n sort entries and index slots; frame_count zeroed
+  int alloc(int64_t n, int frames, cudaStream_t s) {
+    sort_n = n;
+    num_frames = frames;
+    PG_CUDA_OK(index.alloc(sizeof(int32_t) * n, s));
+    PG_CUDA_OK(keys_a.alloc(sizeof(uint64_t) * n, s));
+    PG_CUDA_OK(keys_b.alloc(sizeof(uint64_t) * n, s));
+    PG_CUDA_OK(vals_a.alloc(sizeof(int32_t) * n, s));
+    PG_CUDA_OK(vals_b.alloc(sizeof(int32_t) * n, s));
+    PG_CUDA_OK(frame_count.alloc(sizeof(int32_t) * (frames + 1), s));
+    PG_CUDA_OK(frame_ptr.alloc(sizeof(int32_t) * (frames + 1), s));
+    PG_CUDA_OK(cudaMemsetAsync(frame_count.ptr, 0, sizeof(int32_t) * (frames + 1), s));
+    return PG_OK;
   }
-}
+};
+
+// The caller's outputs
+struct Detections {
+  int32_t* label; float* box; float* score; int32_t* index;   // [capacity] kept boxes
+  int64_t capacity;
+  int32_t* frame_ptr;                                         // [num_frames + 1] into the kept boxes
+  int32_t* cand_index; int32_t* cand_frame_ptr;               // the candidate list, or null when not wanted
+  int64_t* sizes_host;                                        // {kept boxes, candidates}
+};
 
 }  // namespace
 }  // namespace pg
 
 using namespace pg;
 
-// Stages 2b-6 on candidate arrays that are contiguous per frame (cfp = candidate frame_ptr, fcount = per-frame counts,
-// total_dev = number of candidates, all on the device; keys_a / vals_a hold the sort input of `cap` entries).
-static int nms_stage(Temp& cbox, Temp& cscore, Temp& clabel, Temp& cindex, Temp& keys_a, Temp& keys_b, Temp& vals_a,
-                     Temp& vals_b, Temp& fcount, Temp& cfp, const int32_t* total_dev, int64_t cap, int num_frames,
-                     double overlapped_thres, double appr_factor, int32_t flags, int64_t max_candidates_per_frame, int32_t* out_label,
-                     float* out_box, float* out_score, int32_t* out_index, int64_t capacity, int32_t* out_det_frame_ptr,
-                     int32_t* out_cand_index, int32_t* out_cand_frame_ptr, int64_t* out_sizes_host, cudaStream_t s) {
-  void* stream = static_cast<void*>(s);
-  (void)stream;
-  Temp tmp;
-  size_t sort_bytes = 0;
-  PG_CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, keys_a.as<uint64_t>(), keys_b.as<uint64_t>(),
-                                             vals_a.as<int32_t>(), vals_b.as<int32_t>(), int(cap), 0, 64, s));
-  PG_CUDA_OK(tmp.alloc(sort_bytes, s));
-  frame_ptr_from_counts_kernel<<<1, 32, 0, s>>>(fcount.as<int32_t>(), num_frames, cfp.as<int32_t>());
+// Stages 2-6 on candidates whose sort input (keys_a, vals_a) and per-frame counts are filled.  Two host round trips:
+// the widest frame (to size the bit matrix), then the number of kept boxes.
+static int nms_stage(Candidates& c, const Detections& out, double overlapped_thres, double appr_factor, int32_t flags,
+                     int64_t max_candidates_per_frame, cudaStream_t s) {
+  const int num_frames = c.num_frames;
+  const int32_t* cfp = c.frame_ptr.as<int32_t>();
+  const int32_t* total_dev = cfp + num_frames;     // number of candidates
+  frame_ptr_kernel<<<1, 1, 0, s>>>(c.frame_count.as<int32_t>(), num_frames, c.frame_ptr.as<int32_t>());
   PG_LAUNCH_CHECK();
-  // bboxes_sort (nms.py:90-107): score descending inside a frame; stable, so ties keep ascending input order
-  PG_CUDA_OK(cub::DeviceRadixSort::SortPairs(tmp.ptr, sort_bytes, keys_a.as<uint64_t>(), keys_b.as<uint64_t>(),
-                                             vals_a.as<int32_t>(), vals_b.as<int32_t>(), int(cap), 0, 64, s));
-  count_launch(4);
+  // bboxes_sort (nms.py:90-107): score descending inside a frame; stable, so ties keep ascending candidate position
+  if (int rc = sort_pairs(c.keys_a.as<uint64_t>(), c.keys_b.as<uint64_t>(), c.vals_a.as<int32_t>(), c.vals_b.as<int32_t>(),
+                          c.sort_n, 64, s))
+    return rc;
 
   // the widest frame decides the bit-matrix row width; it must be known on the host to size the matrix
-  Temp maxc;
-  PG_CUDA_OK(maxc.alloc(sizeof(int32_t), s));
-  max_frame_count_kernel<<<1, 32, 0, s>>>(fcount.as<int32_t>(), num_frames, maxc.as<int32_t>());
-  PG_LAUNCH_CHECK();
   int32_t h_max = 0, h_total = 0;
-  PG_CUDA_OK(cudaMemcpyAsync(&h_max, maxc.ptr, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  PG_CUDA_OK(cudaMemcpyAsync(&h_max, c.frame_count.as<int32_t>() + num_frames, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
   PG_CUDA_OK(cudaMemcpyAsync(&h_total, total_dev, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
   PG_CUDA_OK(cudaStreamSynchronize(s));
-  out_sizes_host[0] = 0;
-  out_sizes_host[1] = h_total;
-  if (out_cand_frame_ptr)
-    PG_CUDA_OK(cudaMemcpyAsync(out_cand_frame_ptr, cfp.ptr, sizeof(int32_t) * (num_frames + 1), cudaMemcpyDeviceToDevice, s));
+  out.sizes_host[0] = 0;
+  out.sizes_host[1] = h_total;
+  if (out.cand_frame_ptr)
+    PG_CUDA_OK(cudaMemcpyAsync(out.cand_frame_ptr, cfp, sizeof(int32_t) * (num_frames + 1), cudaMemcpyDeviceToDevice, s));
   if (h_total == 0) {
-    PG_CUDA_OK(cudaMemsetAsync(out_det_frame_ptr, 0, sizeof(int32_t) * (num_frames + 1), s));
+    PG_CUDA_OK(cudaMemsetAsync(out.frame_ptr, 0, sizeof(int32_t) * (num_frames + 1), s));
     return PG_OK;
   }
   if (h_max > max_candidates_per_frame) {
@@ -505,47 +512,41 @@ static int nms_stage(Temp& cbox, Temp& cscore, Temp& clabel, Temp& cindex, Temp&
   PG_CUDA_OK(obox.alloc(sizeof(float) * h_total * kBoxLen, s));
   PG_CUDA_OK(oscore.alloc(sizeof(float) * h_total, s));
   sorted_geometry_kernel<<<ceil_div(h_total, 128), 128, 0, s>>>(
-      vals_b.as<int32_t>(), total_dev, cbox.as<float>(), cscore.as<float>(), clabel.as<int32_t>(), cindex.as<int32_t>(),
-      sbox.as<float>(), sscore.as<float>(), slabel.as<int32_t>(), sindex.as<int32_t>(), geom.as<BoxGeom>(),
-      (flags & 4) ? appr_factor : 0.0);
+      c.vals_b.as<int32_t>(), total_dev, c.box, c.score, c.label, c.index.as<int32_t>(), sbox.as<float>(),
+      sscore.as<float>(), slabel.as<int32_t>(), sindex.as<int32_t>(), geom.as<BoxGeom>(),
+      (flags & PG_NMS_INT_CORNERS) ? appr_factor : 0.0);
   PG_LAUNCH_CHECK();
   {
     dim3 grid(std::max(1, std::min(words / 4 + 1, 16)), std::min(h_max, 4096), num_frames);
-    adjacency_kernel<<<grid, 128, 0, s>>>(geom.as<BoxGeom>(), slabel.as<int32_t>(), cfp.as<int32_t>(), num_frames, words,
+    adjacency_kernel<<<grid, 128, 0, s>>>(geom.as<BoxGeom>(), slabel.as<int32_t>(), cfp, num_frames, words,
                                           overlapped_thres, adj.as<uint32_t>());
     PG_LAUNCH_CHECK();
   }
-  sweep_kernel<<<num_frames, 32, 0, s>>>(cfp.as<int32_t>(), words, adj.as<uint32_t>(), valid.as<uint32_t>(), kept.as<int32_t>());
+  sweep_kernel<<<num_frames, 32, 0, s>>>(cfp, words, adj.as<uint32_t>(), valid.as<uint32_t>(), kept.as<int32_t>());
   PG_LAUNCH_CHECK();
   const int mblocks = std::min(h_total, num_sms() * 4);
   PG_CUDA_OK(scratch.alloc(sizeof(int32_t) * int64_t(mblocks) * (int64_t(words) * 32 + 1), s));
   merge_rescore_kernel<<<mblocks, kMergeThreads, 0, s>>>(
-      cfp.as<int32_t>(), num_frames, total_dev, words, adj.as<uint32_t>(), kept.as<int32_t>(), geom.as<BoxGeom>(),
-      sbox.as<float>(), sscore.as<float>(), (flags & 1) ? 1 : 0, (flags & 2) ? 1 : 0, obox.as<float>(), oscore.as<float>(),
-      scratch.as<int32_t>());
+      cfp, num_frames, total_dev, words, adj.as<uint32_t>(), kept.as<int32_t>(), geom.as<BoxGeom>(), sbox.as<float>(),
+      sscore.as<float>(), (flags & PG_NMS_MERGE) ? 1 : 0, (flags & PG_NMS_RESCORE) ? 1 : 0, obox.as<float>(),
+      oscore.as<float>(), scratch.as<int32_t>());
   PG_LAUNCH_CHECK();
   PG_CUDA_OK(cudaMemsetAsync(kept.as<int32_t>() + h_total, 0, sizeof(int32_t), s));
-  size_t ks_bytes = 0;
-  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, ks_bytes, kept.as<int32_t>(), kept_scan.as<int32_t>(), h_total + 1, s));
-  Temp tmp2;
-  PG_CUDA_OK(tmp2.alloc(ks_bytes, s));
-  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(tmp2.ptr, ks_bytes, kept.as<int32_t>(), kept_scan.as<int32_t>(), h_total + 1, s));
-  count_launch(2);
+  if (int rc = exclusive_sum(kept.as<int32_t>(), kept_scan.as<int32_t>(), h_total + 1, s)) return rc;
   compact_kernel<<<ceil_div(h_total, 256), 256, 0, s>>>(total_dev, kept.as<int32_t>(), kept_scan.as<int32_t>(), obox.as<float>(),
-                                                        oscore.as<float>(), slabel.as<int32_t>(), sindex.as<int32_t>(), capacity,
-                                                        out_label, out_box, out_score, out_index);
+                                                        oscore.as<float>(), slabel.as<int32_t>(), sindex.as<int32_t>(),
+                                                        out.capacity, out.label, out.box, out.score, out.index);
   PG_LAUNCH_CHECK();
-  det_frame_ptr_kernel<<<ceil_div(num_frames + 1, 64), 64, 0, s>>>(cfp.as<int32_t>(), num_frames, kept_scan.as<int32_t>(),
-                                                                    out_det_frame_ptr);
+  det_frame_ptr_kernel<<<ceil_div(num_frames + 1, 64), 64, 0, s>>>(cfp, num_frames, kept_scan.as<int32_t>(), out.frame_ptr);
   PG_LAUNCH_CHECK();
-  if (out_cand_index)   // all candidates in ascending (vertex, class) order: run.py:284 box_indices, per frame
-    PG_CUDA_OK(cudaMemcpyAsync(out_cand_index, cindex.ptr, sizeof(int32_t) * h_total, cudaMemcpyDeviceToDevice, s));
+  if (out.cand_index)   // all candidates in ascending (vertex, class) order: run.py:284 box_indices, per frame
+    PG_CUDA_OK(cudaMemcpyAsync(out.cand_index, c.index.ptr, sizeof(int32_t) * h_total, cudaMemcpyDeviceToDevice, s));
   int32_t h_det = 0;
   PG_CUDA_OK(cudaMemcpyAsync(&h_det, kept_scan.as<int32_t>() + h_total, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
   PG_CUDA_OK(cudaStreamSynchronize(s));
-  out_sizes_host[0] = h_det;
-  if (h_det > capacity) {
-    set_error("detection buffer too small: need %d, capacity %lld", h_det, (long long)capacity);
+  out.sizes_host[0] = h_det;
+  if (h_det > out.capacity) {
+    set_error("detection buffer too small: need %d, capacity %lld", h_det, (long long)out.capacity);
     return PG_ERR_CAPACITY;
   }
   return PG_OK;
@@ -604,40 +605,34 @@ extern "C" int pg_postprocess(const float* probs, const float* box_encodings, co
   make_class_table(class_table_host, num_classes, &tab);
   const int64_t cap = num_vertices * (num_classes - 2);      // at most C - 2 candidate classes per vertex
   const int64_t pairs = num_vertices * num_classes;
-  Temp flags_b, slots, tmp, cbox, cscore, clabel, cindex, keys_a, keys_b, vals_a, vals_b, fcount, total, cfp;
+  Candidates cand;
+  if (int rc = cand.alloc(cap, num_frames, s)) return rc;
+  Temp flags_b, slots, cbox, cscore, clabel;
   PG_CUDA_OK(flags_b.alloc(sizeof(int32_t) * (pairs + 1), s));
   PG_CUDA_OK(slots.alloc(sizeof(int32_t) * (pairs + 1), s));
   PG_CUDA_OK(cbox.alloc(sizeof(float) * cap * kBoxLen, s));
   PG_CUDA_OK(cscore.alloc(sizeof(float) * cap, s));
   PG_CUDA_OK(clabel.alloc(sizeof(int32_t) * cap, s));
-  PG_CUDA_OK(cindex.alloc(sizeof(int32_t) * cap, s));
-  PG_CUDA_OK(keys_a.alloc(sizeof(uint64_t) * cap, s));
-  PG_CUDA_OK(keys_b.alloc(sizeof(uint64_t) * cap, s));
-  PG_CUDA_OK(vals_a.alloc(sizeof(int32_t) * cap, s));
-  PG_CUDA_OK(vals_b.alloc(sizeof(int32_t) * cap, s));
-  PG_CUDA_OK(fcount.alloc(sizeof(int32_t) * (num_frames + 1), s));
-  PG_CUDA_OK(cfp.alloc(sizeof(int32_t) * (num_frames + 1), s));
-  PG_CUDA_OK(cudaMemsetAsync(fcount.ptr, 0, sizeof(int32_t) * (num_frames + 1), s));
   PG_CUDA_OK(cudaMemsetAsync(flags_b.as<int32_t>() + pairs, 0, sizeof(int32_t), s));
+  cand.box = cbox.as<float>();
+  cand.score = cscore.as<float>();
+  cand.label = clabel.as<int32_t>();
 
   flag_candidates_kernel<<<ceil_div(pairs, 256), 256, 0, s>>>(probs, num_vertices, num_classes, flags_b.as<int32_t>());
   PG_LAUNCH_CHECK();
-  size_t scan_bytes = 0;
-  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, flags_b.as<int32_t>(), slots.as<int32_t>(), int(pairs + 1), s));
-  PG_CUDA_OK(tmp.alloc(scan_bytes, s));
-  PG_CUDA_OK(cub::DeviceScan::ExclusiveSum(tmp.ptr, scan_bytes, flags_b.as<int32_t>(), slots.as<int32_t>(), int(pairs + 1), s));
-  count_launch(2);
-  const int32_t* total_dev = slots.as<int32_t>() + pairs;      // number of candidates
+  if (int rc = exclusive_sum(flags_b.as<int32_t>(), slots.as<int32_t>(), pairs + 1, s)) return rc;
   decode_scatter_kernel<<<ceil_div(pairs, 256), 256, 0, s>>>(
       probs, box_encodings, xyz, frame_ptr, num_frames, num_vertices, num_classes, tab, flags_b.as<int32_t>(),
-      slots.as<int32_t>(), cbox.as<float>(), cscore.as<float>(), clabel.as<int32_t>(), cindex.as<int32_t>(),
-      keys_a.as<uint64_t>(), vals_a.as<int32_t>(), fcount.as<int32_t>());
+      slots.as<int32_t>(), cbox.as<float>(), cscore.as<float>(), clabel.as<int32_t>(), cand.index.as<int32_t>(),
+      cand.keys_a.as<uint64_t>(), cand.vals_a.as<int32_t>(), cand.frame_count.as<int32_t>());
   PG_LAUNCH_CHECK();
-  fill_tail_keys_kernel<<<ceil_div(cap, 256), 256, 0, s>>>(total_dev, cap, keys_a.as<uint64_t>(), vals_a.as<int32_t>());
+  // slots[pairs] = number of candidates
+  fill_tail_keys_kernel<<<ceil_div(cap, 256), 256, 0, s>>>(slots.as<int32_t>() + pairs, cap, cand.keys_a.as<uint64_t>(),
+                                                          cand.vals_a.as<int32_t>());
   PG_LAUNCH_CHECK();
-  return nms_stage(cbox, cscore, clabel, cindex, keys_a, keys_b, vals_a, vals_b, fcount, cfp, total_dev, cap, num_frames,
-                   overlapped_thres, 0.0, flags, max_candidates_per_frame, out_label, out_box, out_score, out_index, capacity,
-                   out_det_frame_ptr, out_cand_index, out_cand_frame_ptr, out_sizes_host, s);
+  const Detections out{out_label, out_box, out_score, out_index, capacity, out_det_frame_ptr, out_cand_index,
+                       out_cand_frame_ptr, out_sizes_host};
+  return nms_stage(cand, out, overlapped_thres, 0.0, flags, max_candidates_per_frame, s);
 }
 
 extern "C" int pg_nms_boxes_3d(const int32_t* class_labels, const float* boxes, const float* scores,
@@ -650,29 +645,15 @@ extern "C" int pg_nms_boxes_3d(const int32_t* class_labels, const float* boxes, 
   PG_REQUIRE(out_label && out_box && out_score && out_index && capacity >= 1, "pg_nms_boxes_3d: output buffers are required");
   PG_REQUIRE(num_frames >= 1 && num_frames <= 65535 && num_boxes >= 1 && num_boxes < (int64_t(1) << 31), "pg_nms_boxes_3d: bad sizes");
   PG_REQUIRE(max_candidates_per_frame >= 32, "pg_nms_boxes_3d: max_candidates_per_frame must be >= 32");
-  Temp cbox, cscore, clabel, cindex, keys_a, keys_b, vals_a, vals_b, fcount, cfp, total;
-  PG_CUDA_OK(cbox.alloc(sizeof(float) * num_boxes * kBoxLen, s));
-  PG_CUDA_OK(cscore.alloc(sizeof(float) * num_boxes, s));
-  PG_CUDA_OK(clabel.alloc(sizeof(int32_t) * num_boxes, s));
-  PG_CUDA_OK(cindex.alloc(sizeof(int32_t) * num_boxes, s));
-  PG_CUDA_OK(keys_a.alloc(sizeof(uint64_t) * num_boxes, s));
-  PG_CUDA_OK(keys_b.alloc(sizeof(uint64_t) * num_boxes, s));
-  PG_CUDA_OK(vals_a.alloc(sizeof(int32_t) * num_boxes, s));
-  PG_CUDA_OK(vals_b.alloc(sizeof(int32_t) * num_boxes, s));
-  PG_CUDA_OK(fcount.alloc(sizeof(int32_t) * (num_frames + 1), s));
-  PG_CUDA_OK(cfp.alloc(sizeof(int32_t) * (num_frames + 1), s));
-  PG_CUDA_OK(total.alloc(sizeof(int32_t), s));
-  PG_CUDA_OK(cudaMemsetAsync(fcount.ptr, 0, sizeof(int32_t) * (num_frames + 1), s));
-  PG_CUDA_OK(cudaMemcpyAsync(cbox.ptr, boxes, sizeof(float) * num_boxes * kBoxLen, cudaMemcpyDeviceToDevice, s));
-  PG_CUDA_OK(cudaMemcpyAsync(cscore.ptr, scores, sizeof(float) * num_boxes, cudaMemcpyDeviceToDevice, s));
-  PG_CUDA_OK(cudaMemcpyAsync(clabel.ptr, class_labels, sizeof(int32_t) * num_boxes, cudaMemcpyDeviceToDevice, s));
-  const int32_t h_n = int32_t(num_boxes);
-  PG_CUDA_OK(cudaMemcpyAsync(total.ptr, &h_n, sizeof(int32_t), cudaMemcpyHostToDevice, s));
-  candidate_keys_kernel<<<ceil_div(num_boxes, 256), 256, 0, s>>>(scores, frame_ptr, num_frames, num_boxes, keys_a.as<uint64_t>(),
-                                                                  vals_a.as<int32_t>(), fcount.as<int32_t>(), cindex.as<int32_t>());
+  Candidates cand;
+  if (int rc = cand.alloc(num_boxes, num_frames, s)) return rc;
+  cand.box = boxes;
+  cand.score = scores;
+  cand.label = class_labels;
+  candidate_keys_kernel<<<ceil_div(num_boxes, 256), 256, 0, s>>>(scores, frame_ptr, num_frames, num_boxes,
+                                                                  cand.keys_a.as<uint64_t>(), cand.vals_a.as<int32_t>(),
+                                                                  cand.frame_count.as<int32_t>(), cand.index.as<int32_t>());
   PG_LAUNCH_CHECK();
-  PG_CUDA_OK(cudaStreamSynchronize(s));     // h_n is a stack variable
-  return nms_stage(cbox, cscore, clabel, cindex, keys_a, keys_b, vals_a, vals_b, fcount, cfp, total.as<int32_t>(), num_boxes,
-                   num_frames, overlapped_thres, appr_factor, flags, max_candidates_per_frame, out_label, out_box, out_score, out_index,
-                   capacity, out_det_frame_ptr, nullptr, nullptr, out_sizes_host, s);
+  const Detections out{out_label, out_box, out_score, out_index, capacity, out_det_frame_ptr, nullptr, nullptr, out_sizes_host};
+  return nms_stage(cand, out, overlapped_thres, appr_factor, flags, max_candidates_per_frame, s);
 }
