@@ -436,6 +436,38 @@ PG_API int pg_nms_boxes_3d(const int32_t* class_labels, const float* boxes, cons
                     float* out_box, float* out_score, int32_t* out_index, int64_t capacity,
                     int32_t* out_det_frame_ptr, int64_t* out_sizes_host, void* stream);
 
+/* ------------------------------------------------------------------------ *
+ * KITTI object evaluation (reference kitti_native_evaluation/src/evaluate_object_3d_offline.cpp)
+ * ------------------------------------------------------------------------ */
+
+/*
+ * eval_class (:639-739) for every metric m (0 image :224-258, 1 bird's-eye view :291-311, 2 3D :314-341), class c
+ * (0 car, 1 pedestrian, 2 cyclist) and difficulty d (0 easy, 1 moderate, 2 hard) on a batch of frames: cleanData
+ * (:378-451), computeStatistics (:453-633) without and with false positives, getThresholds (:343-376) and the
+ * precision / orientation-similarity curves with their suffix max (:703-734).  fp64 throughout.
+ *   gt        [G, 14] device, the label-file columns after the type: truncation, occlusion, alpha, x1, y1, x2, y2,
+ *             h, w, l, t1, t2, t3, ry (loadGroundtruth :175-199)
+ *   det       [D, 15] device, the result-file columns after the type: two unused, alpha, x1, y1, x2, y2, h, w, l,
+ *             t1, t2, t3, ry, score (loadDetections :128-173)
+ *   gt_class / det_class [G] / [D] device: the type, case-insensitively, as 0 car, 1 pedestrian, 2 cyclist, 3 van,
+ *             4 person_sitting, 5 dontcare, 6 anything else
+ *   gt_frame_ptr_host / det_frame_ptr_host [num_frames + 1] (host): the rows of each frame
+ *   flags     PG_KITTI_EVAL_AOS: the image metric also computes AOS (no detection has alpha = -10, :152-154);
+ *             the other two always compute the heading similarity (AHS) from |gt.ry - det.ry|
+ * Outputs (host), segment s = (m * 3 + c) * 3 + d:
+ *   out_precision / out_aos / out_ahs [27][41]   the curves eval_class returns (zeros where not computed)
+ *   out_num_thresholds [27]                      score thresholds of each segment, at most 41: where the
+ *                                                reference would write past its 41-entry arrays (undefined
+ *                                                behaviour), the thresholds after the 41st are dropped
+ *   out_tp / out_fp / out_fn [27][41]            summed over frames per threshold (zeros past the count)
+ * No limit on boxes per frame.  One host round trip (the final read-back).
+ */
+#define PG_KITTI_EVAL_AOS 1
+PG_API int pg_kitti_eval(const double* gt, const int32_t* gt_class, const double* det, const int32_t* det_class,
+                  const int64_t* gt_frame_ptr_host, const int64_t* det_frame_ptr_host, int32_t num_frames,
+                  int32_t flags, double* out_precision, double* out_aos, double* out_ahs,
+                  int32_t* out_num_thresholds, int32_t* out_tp, int32_t* out_fp, int32_t* out_fn, void* stream);
+
 /* wgmma kernel launches so far (which: 0 = segment-max launches of the edge layers, 1 = store launches:
  * dense layers and the stored per-edge layers of point-set pooling);
  * lets callers and tests verify that the tensor-core path, not the FFMA path, actually ran. */

@@ -80,6 +80,11 @@ SIGNATURES = {
     'pg_nms_boxes_3d': (ctypes.c_int, [c_i32p, c_f32p, c_f32p, c_i32p, c_i32, c_i64, ctypes.c_double,
                                        ctypes.c_double, c_i32, c_i64, c_i32p, c_f32p, c_f32p, c_i32p, c_i64, c_i32p,
                                        ctypes.POINTER(c_i64), ctypes.c_void_p]),
+    'pg_kitti_eval': (ctypes.c_int, [ctypes.c_void_p, c_i32p, ctypes.c_void_p, c_i32p, ctypes.POINTER(c_i64),
+                                     ctypes.POINTER(c_i64), c_i32, c_i32, ctypes.POINTER(ctypes.c_double),
+                                     ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double),
+                                     ctypes.POINTER(c_i32), ctypes.POINTER(c_i32), ctypes.POINTER(c_i32),
+                                     ctypes.POINTER(c_i32), ctypes.c_void_p]),
     'pg_layer_create': (ctypes.c_int, [c_i32, ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_void_p),
                                        ctypes.POINTER(c_i32), c_i32, c_i32, ctypes.c_void_p,
                                        ctypes.POINTER(ctypes.c_void_p)]),
@@ -646,3 +651,32 @@ def cam_points_in_image(velo, frame_ptr, velo_to_cam, cam_to_image, image_sizes,
         _ptr(out_attr, torch.float32, 'out_attr'), channels, m, _ptr(out_fp, torch.int32, 'out_fp'), ctypes.byref(n),
         _stream()))
     return out_xyz[:n.value], out_attr[:n.value], out_fp
+
+
+# ---------------------------------------------------------------------------------------------
+# KITTI object evaluation
+# ---------------------------------------------------------------------------------------------
+PG_KITTI_EVAL_AOS = 1
+
+
+def kitti_eval(gt, gt_class, det, det_class, gt_frame_ptr, det_frame_ptr, compute_aos):
+    """pg_kitti_eval.  gt [G,14] / det [D,15] CUDA float64, gt_class / det_class CUDA int32, frame pointers [F+1] host
+    int64 arrays.  -> dict of host arrays: precision / aos / ahs [3,3,3,41] float64, num_thresholds [3,3,3],
+    tp / fp / fn [3,3,3,41] int32 (axes: metric, class, difficulty, threshold)."""
+    import numpy as np
+    gfp = np.ascontiguousarray(gt_frame_ptr, dtype=np.int64)
+    dfp = np.ascontiguousarray(det_frame_ptr, dtype=np.int64)
+    num_frames = len(gfp) - 1
+    out = {k: np.zeros((3, 3, 3, 41), np.float64) for k in ('precision', 'aos', 'ahs')}
+    out.update({k: np.zeros((3, 3, 3, 41), np.int32) for k in ('tp', 'fp', 'fn')})
+    out['num_thresholds'] = np.zeros((3, 3, 3), np.int32)
+
+    def p(a, t):
+        return a.ctypes.data_as(ctypes.POINTER(t))
+    _check(load().pg_kitti_eval(
+        _ptr(gt, torch.float64, 'gt'), _ptr(gt_class, torch.int32, 'gt_class'), _ptr(det, torch.float64, 'det'),
+        _ptr(det_class, torch.int32, 'det_class'), p(gfp, c_i64), p(dfp, c_i64), num_frames,
+        PG_KITTI_EVAL_AOS if compute_aos else 0, p(out['precision'], ctypes.c_double), p(out['aos'], ctypes.c_double),
+        p(out['ahs'], ctypes.c_double), p(out['num_thresholds'], c_i32), p(out['tp'], c_i32), p(out['fp'], c_i32),
+        p(out['fn'], c_i32), _stream()))
+    return out

@@ -23,6 +23,7 @@
 //   5. merge + rescore: one block per kept box (median by rank selection, IoU with the merged box)
 //   6. compaction of the kept boxes per frame
 #include "pg_common.cuh"
+#include "pg_geom.cuh"
 
 namespace pg {
 namespace {
@@ -152,21 +153,6 @@ __global__ void frame_ptr_kernel(int32_t* __restrict__ counts, int num_frames, i
 }
 
 // ---- 3. geometry -----------------------------------------------------------------------------------
-struct BoxGeom {
-  double fx[4], fz[4];   // footprint corners (x, z), nms.py:17-20 order
-  double ymin, ymax, xmin, xmax, zmin, zmax;
-  double area;
-};
-
-__device__ inline double shoelace(const double* x, const double* z, int n) {
-  double a = 0.0;
-  for (int i = 0; i < n; ++i) {
-    const int j = (i + 1 == n) ? 0 : i + 1;
-    a += x[i] * z[j] - z[i] * x[j];
-  }
-  return 0.5 * a;
-}
-
 // nms.py:9-27: trigonometry and the half extents in float32 (the box dtype), the rest in float64
 // appr > 0: the corners are converted to integer "pixels" first, np.int32(corners * appr) (bboxes_nms, nms.py:114)
 __device__ inline void make_geom(const float* b, BoxGeom* g, double appr = 0.0) {
@@ -196,36 +182,6 @@ __device__ inline void make_geom(const float* b, BoxGeom* g, double appr = 0.0) 
   g->ymax = fmax(y_top, y_bot);
   g->ymin = fmin(y_top, y_bot);
   g->area = fabs(shoelace(g->fx, g->fz, 4));
-}
-
-// area of (convex subject) clipped by (convex clip), Sutherland-Hodgman
-__device__ inline double clipped_area(const BoxGeom& subj, const BoxGeom& clip) {
-  double px[12], pz[12], qx[12], qz[12];
-  int n = 4;
-  for (int i = 0; i < 4; ++i) { px[i] = subj.fx[i]; pz[i] = subj.fz[i]; }
-  const bool ccw = shoelace(clip.fx, clip.fz, 4) >= 0.0;
-  for (int e = 0; e < 4 && n > 0; ++e) {
-    // walk the clip polygon counter-clockwise
-    const int ia = ccw ? e : (4 - e) & 3, ib = ccw ? (e + 1) & 3 : (3 - e);
-    const double ax = clip.fx[ia], az = clip.fz[ia];
-    const double ex = clip.fx[ib] - ax, ez = clip.fz[ib] - az;
-    int m = 0;
-    for (int j = 0; j < n; ++j) {
-      const int k = (j + 1 == n) ? 0 : j + 1;
-      const double sp = ex * (pz[j] - az) - ez * (px[j] - ax);
-      const double sq = ex * (pz[k] - az) - ez * (px[k] - ax);
-      if (sp >= 0.0) { qx[m] = px[j]; qz[m] = pz[j]; ++m; }
-      if ((sp >= 0.0) != (sq >= 0.0)) {
-        const double t = sp / (sp - sq);
-        qx[m] = px[j] + t * (px[k] - px[j]);
-        qz[m] = pz[j] + t * (pz[k] - pz[j]);
-        ++m;
-      }
-    }
-    n = m;
-    for (int j = 0; j < n; ++j) { px[j] = qx[j]; pz[j] = qz[j]; }
-  }
-  return n >= 3 ? fabs(shoelace(px, pz, n)) : 0.0;
 }
 
 // nms.py:64-88: IoU of `a` (single_box) against `b` (an element of box_list)

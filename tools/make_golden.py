@@ -376,6 +376,47 @@ def checkpoint_fixtures():
         print('checkpoint fixture', name)
 
 
+KITTI_EVAL_TREES = {   # name -> synthetic_tree arguments
+    'mixed': dict(seed=31, num_frames=60, big_frames=(7,)),
+    'no_aos_no_cyclist': dict(seed=32, num_frames=30, alpha_invalid=True, never_detected=(2,)),
+}
+
+
+def kitti_eval_goldens():
+    """tests/golden/kitti_eval_<tree>.json: seeded synthetic label / result trees (oracle/kitti_eval.synthetic_tree)
+    and everything the reference's own evaluator writes and prints on them - the binary oracle/kitti_eval_build.py
+    compiles from kitti_native_evaluation/src/evaluate_object_3d_offline.cpp with the Boost stand-in.  The result
+    file names skip index 3, and label file 000003.txt exists without a result file (it must not be evaluated)."""
+    import subprocess
+    from oracle import kitti_eval as ke
+    from oracle import kitti_eval_build
+    binary = kitti_eval_build.build()
+    assert binary, 'needs the reference tree'
+    for name, kw in KITTI_EVAL_TREES.items():
+        gt_texts, det_texts = ke.synthetic_tree(**kw)
+        names = ['%06d.txt' % (i if i < 3 else i + 1) for i in range(len(gt_texts))]
+        tmp = tempfile.mkdtemp()
+        gt_dir, res_dir = os.path.join(tmp, 'label_2'), os.path.join(tmp, 'results')
+        ke.write_tree(gt_dir, res_dir, gt_texts, det_texts, names)
+        with open(os.path.join(gt_dir, '000003.txt'), 'w') as f:
+            f.write('Car 0.00 0 0.1 100 100 200 200 1.5 1.6 3.9 1.0 1.6 10.0 0.1\n')
+        stdout = subprocess.run([binary, gt_dir, res_dir], capture_output=True, text=True, check=True).stdout
+        outputs = {}
+        for d, _, files in os.walk(res_dir):
+            for fname in files:
+                rel = os.path.relpath(os.path.join(d, fname), res_dir)
+                if not rel.startswith('data' + os.sep):
+                    with open(os.path.join(d, fname)) as f:
+                        outputs[rel] = f.read()
+        gts = {n: t for n, t in zip(names, gt_texts)}
+        gts['000003.txt'] = open(os.path.join(gt_dir, '000003.txt')).read()
+        with open(os.path.join(GOLDEN, 'kitti_eval_%s.json' % name), 'w') as f:
+            json.dump({'tree': kw, 'label_2': gts, 'data': dict(zip(names, det_texts)), 'outputs': outputs,
+                       'stdout': stdout}, f, indent=0, sort_keys=True)
+        print('kitti_eval', name, 'frames', len(names), 'outputs', len(outputs))
+        print(stdout)
+
+
 if __name__ == '__main__':
     which = sys.argv[1] if len(sys.argv) > 1 else 'all'
     if which in ('all', 'graph_random'):
@@ -396,3 +437,5 @@ if __name__ == '__main__':
         graph_live_reference_goldens()
     if which in ('all', 'checkpoints'):
         checkpoint_fixtures()
+    if which in ('all', 'kitti_eval'):
+        kitti_eval_goldens()
