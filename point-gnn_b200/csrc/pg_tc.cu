@@ -4,13 +4,15 @@
 //   out = epilogue(A @ W + b), W streamed by a producer warpgroup, A produced on the fly in shared memory by the
 //   two consumer warpgroups that also run the wgmmas.
 //
-//   producers  PROD_ROWS  A = rows of an fp32 matrix (dense layers, the later layers of the pooling MLP)
+//   producers  PROD_ROWS  A = rows of an fp32 matrix (dense layers, a pooling layer wider than one launch)
 //              PROD_GNN   one GNN iteration's edge MLP (/root/reference/models/gnn.py:338-365) after hoisting:
 //                         e0 @ W1 + b1 = (F @ W1[:C] + b1)[src] + (x_src - x_dst') @ W1[C:], so the first edge
 //                         layer is a per-VERTEX table P (a PROD_ROWS GEMM) plus a 3-term per-edge correction;
 //                         A row e = relu(P[src] + (x_src - x_dst') @ W1[C:])
 //              PROD_POOL  PointSetPooling's first layer (gnn.py:264-270) in fp32:
-//                         A row e = relu([feature(src), x_src - x_kp(dst)] @ W0 + b0)
+//                         A row e = relu([feature(src), x_src - x_kp(dst)] @ W0 + b0), then the chain: every
+//                         further pooling layer ahead of the kernel's own runs on the same tile with its input and
+//                         output in the consumer warpgroup's shared-memory region, never in global memory
 //   epilogues  EPI_STORE  act(acc + b) (+ residual) to a row-major matrix
 //              EPI_SEGMAX max over the edges of each destination (edges are grouped by destination):
 //                         relu / bias commute with max, so raw accumulators are reduced across the warp's
@@ -30,9 +32,11 @@
 //
 // Operand layout (no swizzle, K-major): 8-row x 16-byte core matrices, 128 contiguous bytes each;
 // for a 16-k chunk, core(row group g, k half kc) at g * 256 + kc * 128 (LBO = 128, SBO = 256).
+#include <algorithm>
 #include <atomic>
 #include <cstdlib>
 #include <memory>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -61,17 +65,20 @@ constexpr int kTileRows = 128;      // rows per tile (64 per consumer warpgroup)
 constexpr int kMaxRing = 4;
 constexpr int kMaxNT = 304;         // widest padded N one launch covers
 constexpr uint32_t kABytes = 4096;  // one warpgroup's A chunk: hi (2048) + lo (2048), 64 rows x 16 k
+constexpr int kMaxChain = 6;        // on-chip pooling layers ahead of the kernel's own (edge MLPs have <= 8 layers)
 
-// W stages in shared memory for an NT-wide layer: the deepest power of two up to kMaxRing (so the stage of a chunk
-// is a mask) whose ring, A buffers and barriers fit the 227 KB a CTA may use
-constexpr size_t wg_smem_bytes(int nt, int ring) {
-  return size_t(ring) * nt * 64 + 4 * kABytes + 2 * ring * sizeof(uint64_t);
+// shared memory of a CTA: a ring of W stages, one A region per consumer warpgroup (the double buffer of a streamed
+// layer, or a whole on-chip activation), the full / empty barriers
+constexpr size_t wg_smem_bytes(uint32_t stage_bytes, uint32_t region_bytes, int ring) {
+  return size_t(ring) * stage_bytes + 2 * size_t(region_bytes) + 2 * ring * sizeof(uint64_t);
 }
-constexpr int ring_stages(int nt) {
+// the deepest power of two up to kMaxRing (so the stage of a chunk is a mask) that fits the 227 KB a CTA may use
+constexpr int ring_stages(uint32_t stage_bytes, uint32_t region_bytes) {
   int r = kMaxRing;
-  while (r > 1 && wg_smem_bytes(nt, r) > 227 * 1024) r /= 2;
+  while (r > 1 && wg_smem_bytes(stage_bytes, region_bytes, r) > 227 * 1024) r /= 2;
   return r;
 }
+constexpr int log2_ring(int r) { return r >= 4 ? 2 : r >= 2 ? 1 : 0; }
 
 enum { PROD_ROWS = 0, PROD_GNN = 1, PROD_POOL = 2 };
 enum { EPI_STORE = 0, EPI_SEGMAX = 1 };
@@ -79,10 +86,10 @@ enum { EPI_STORE = 0, EPI_SEGMAX = 1 };
 struct WgParams {
   // A producer
   const float* x;           // ROWS: [num_rows, ldx];  GNN: P [num_src, ldx] (ldx = kp, zero padded)
-  int ldx;
+  int ldx;                  // POOL: layer 1's padded K, the row stride of w1x
   int k_real;               // ROWS: true K (multiple of 4)
   const float* feat;        // POOL: [num_src] point features (one channel)
-  const float* w1x;         // GNN: [3, kp] = W1[C:];  POOL: [4, kp] = W0, then [kp] = b0 (zero padded)
+  const float* w1x;         // GNN: [3, kp] = W1[C:];  POOL: [4, ldx] = W0, then [ldx] = b0 (zero padded)
   const float* xyz_src;     // [num_src, 3]
   const float* xyz_dst;     // [*, 3] (already offset)
   const int32_t* dst_index; // optional indirection dst -> row of xyz_dst
@@ -103,6 +110,14 @@ struct WgParams {
   int ldr;
   int* err;
   int64_t num_tiles;
+  // POOL: the on-chip layers ahead of the kernel's own one (layer 1 first), each {16-k chunks, instruction shape
+  // ni * 4 + ns, byte offset of its W image in chain_buf, byte offset of its padded bias}
+  int chain_layers;
+  int4 chain[kMaxChain];
+  const uint8_t* chain_buf;
+  uint32_t stage_bytes;     // POOL: one W ring stage (the widest chunk of any layer of the launch)
+  uint32_t region_bytes;    // POOL: one consumer warpgroup's A region
+  int ring_log2;            // POOL: log2 of the ring depth
 };
 
 __device__ __forceinline__ float4 ldg_nc(const float* ptr) {
@@ -126,17 +141,22 @@ __device__ __forceinline__ void ldg8(const float* ptr, float (&w)[8]) {
 template <int kProd, int kEpi, int NI, int NS>
 __global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
   constexpr int NT = NI * NS;
-  constexpr int kRing = ring_stages(NT);
   constexpr uint32_t kChunkBytes = uint32_t(NT) * 64u;   // hi + lo, 16 k
+  constexpr int kRing = ring_stages(kChunkBytes, 2 * kABytes);
+  // the pooling chain sizes its ring stages and A regions for all of its layers (host side, launch_wg)
+  const uint32_t stage_bytes = kProd == PROD_POOL ? p.stage_bytes : kChunkBytes;
+  const uint32_t region_bytes = kProd == PROD_POOL ? p.region_bytes : 2 * kABytes;
+  const int ring_log2 = kProd == PROD_POOL ? p.ring_log2 : log2_ring(kRing);
+  const uint32_t ring_mask = (1u << ring_log2) - 1;
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t* bring = smem;
-  uint8_t* abuf = smem + kRing * kChunkBytes;            // [consumer warpgroup][buffer][hi | lo]
-  uint64_t* full = reinterpret_cast<uint64_t*>(abuf + 4 * kABytes);
-  uint64_t* empty = full + kRing;
+  uint8_t* abuf = smem + (stage_bytes << ring_log2);     // [consumer warpgroup][region]
+  uint64_t* full = reinterpret_cast<uint64_t*>(abuf + 2 * region_bytes);
+  uint64_t* empty = full + ring_mask + 1;
   const int tid = threadIdx.x;
   const int role = __shfl_sync(0xffffffffu, tid >> 7, 0);   // warpgroup, warp-uniform by construction
   if (tid == 0) {
-    for (int s = 0; s < kRing; ++s) {
+    for (uint32_t s = 0; s <= ring_mask; ++s) {
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], 8);     // lane 0 of each of the 8 consumer warps
     }
@@ -145,32 +165,44 @@ __global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
   __syncthreads();
   const int64_t my_tiles = (p.num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x;
   const int nk = p.nchunks;
+  const int nl = kProd == PROD_POOL ? p.chain_layers : 0;   // on-chip layers ahead of this one
   if (role == 0) {
-    // W producer: one thread streams the CTA's chunks in the order the consumers use them, refilling a stage as
-    // soon as both consumer warpgroups have released it
+    // W producer: one thread streams the CTA's chunks in the order the consumers use them (per tile: the chain's
+    // layers, then the kernel's own), refilling a stage as soon as both consumer warpgroups have released it
     setmaxnreg_dec<kProducerRegs>();
     if (tid != 0) return;
-    const int64_t total = my_tiles * nk;
-    for (int64_t g = 0; g < total; ++g) {
-      const uint32_t stage = uint32_t(g % kRing);
-      if (g >= kRing) mbar_wait(&empty[stage], uint32_t((g / kRing - 1) & 1));
-      mbar_arrive_expect_tx(&full[stage], kChunkBytes);
-      bulk_g2s(bring + stage * kChunkBytes, p.bimg + size_t(g % nk) * kChunkBytes, kChunkBytes, &full[stage]);
-    }
+    int64_t g = 0;
+    for (int64_t j = 0; j < my_tiles; ++j)
+      for (int l = 0; l <= nl; ++l) {
+        int lk = nk;
+        uint32_t bytes = kChunkBytes;
+        const uint8_t* img = p.bimg;
+        if (l < nl) {
+          const int4 c = p.chain[l];
+          lk = c.x;
+          bytes = uint32_t(c.y >> 2) * uint32_t(c.y & 3) * 64u;
+          img = p.chain_buf + c.z;
+        }
+        for (int kc = 0; kc < lk; ++kc, ++g) {
+          const uint32_t stage = uint32_t(g) & ring_mask;
+          if (g > ring_mask) mbar_wait(&empty[stage], uint32_t(((g >> ring_log2) - 1) & 1));
+          mbar_arrive_expect_tx(&full[stage], bytes);
+          bulk_g2s(bring + stage * stage_bytes, img + size_t(kc) * bytes, bytes, &full[stage]);
+        }
+      }
     return;
   }
   setmaxnreg_inc<kConsumerRegs>();
   const int wgi = role - 1, t = tid & 127, warp = t >> 5, lane = tid & 31;
   // chunk g's W stage is free again
   auto release = [&](int64_t g) {
-    if (lane == 0) mbar_arrive(&empty[g % kRing]);
+    if (lane == 0) mbar_arrive(&empty[uint32_t(g) & ring_mask]);
   };
 
   // A geometry: thread t writes 8 consecutive k (half kh) of row pr of its warpgroup's 64
   const int pr = t >> 1, kh = t & 1;
   const uint32_t a_off = uint32_t(pr >> 3) * 256u + uint32_t(kh) * 128u + uint32_t(pr & 7) * 16u;
-  uint8_t* my_a = abuf + wgi * 2 * kABytes;
-  float acc[NS][NI / 2];
+  uint8_t* my_a = abuf + wgi * region_bytes;
   int64_t g = 0;
   for (int64_t j = 0; j < my_tiles; ++j) {
     const int64_t tile = blockIdx.x + j * gridDim.x;
@@ -205,7 +237,8 @@ __global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
     auto put = [&](int buf, const float4 (&q)[2], int kc) {
       const int k0 = kc * 16 + kh * 8;
       float v[8] = {q[0].x, q[0].y, q[0].z, q[0].w, q[1].x, q[1].y, q[1].z, q[1].w};
-      // w1x rows are kp (a multiple of 16) floats long, so this thread's 8 k of every row are 32-byte aligned
+      // w1x rows are kp (GNN) or ldx (POOL) floats long, a multiple of 16, so this thread's 8 k of every row are
+      // 32-byte aligned
       if (kProd == PROD_GNN) {
         float wx[8], wy[8], wz[8];
         ldg8(p.w1x + k0, wx);
@@ -216,10 +249,10 @@ __global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
       } else if (kProd == PROD_POOL) {
         float wf[8], wx[8], wy[8], wz[8], b0[8];
         ldg8(p.w1x + k0, wf);
-        ldg8(p.w1x + p.kp + k0, wx);
-        ldg8(p.w1x + 2 * p.kp + k0, wy);
-        ldg8(p.w1x + 3 * p.kp + k0, wz);
-        ldg8(p.w1x + 4 * p.kp + k0, b0);
+        ldg8(p.w1x + p.ldx + k0, wx);
+        ldg8(p.w1x + 2 * p.ldx + k0, wy);
+        ldg8(p.w1x + 3 * p.ldx + k0, wz);
+        ldg8(p.w1x + 4 * p.ldx + k0, b0);
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
           float a = b0[i];
@@ -239,39 +272,99 @@ __global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
       *reinterpret_cast<uint4*>(dstp) = hi;
       *reinterpret_cast<uint4*>(dstp + kABytes / 2) = lo;
     };
-    float4 q[2] = {make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f)};
-    load(0, q);
-    put(0, q, 0);
-    if (nk > 1) load(1, q);
-    // ---- main loop over 16-k chunks ------------------------------------------------------------------
-    for (int kc = 0; kc < nk; ++kc, ++g) {
-      fence_proxy_async_smem();
-      warpgroup_sync(1 + wgi);
-      mbar_wait(&full[g % kRing], uint32_t((g / kRing) & 1));
-      wgmma_fence();
-      const uint32_t a_base = smem_u32(my_a + (kc & 1) * kABytes);
-      const uint32_t b_base = smem_u32(bring + uint32_t(g % kRing) * kChunkBytes);
-      const uint64_t a_hi = make_smem_desc(a_base, 128, 256), a_lo = make_smem_desc(a_base + kABytes / 2, 128, 256);
-#pragma unroll
-      for (int i = 0; i < NS; ++i) {
-        const uint64_t b_hi = make_smem_desc(b_base + uint32_t(i * NI) * 32u, 128, 256);
-        const uint64_t b_lo = make_smem_desc(b_base + uint32_t(NT) * 32u + uint32_t(i * NI) * 32u, 128, 256);
-        wgmma_bf16<NI>(acc[i], a_hi, b_hi, kc > 0 ? 1 : 0);
-        wgmma_bf16<NI>(acc[i], a_lo, b_hi, 1);
-        wgmma_bf16<NI>(acc[i], a_hi, b_lo, 1);
+    // ---- one layer's loop over 16-k chunks into acc[ns][ni / 2] --------------------------------------
+    // streamed: A chunk kc is produced by load / put into a double buffer at the start of the region while chunk
+    // kc - 1's wgmmas run.  Otherwise the previous on-chip layer left the whole A in the region, chunk kc at
+    // kc * kABytes
+    auto mma_layer = [&](auto& lacc, int lk, bool streamed) {
+      using Acc = std::remove_reference_t<decltype(lacc)>;
+      constexpr int ns = int(std::extent<Acc, 0>::value), ni = 2 * int(std::extent<Acc, 1>::value);
+      float4 q[2] = {make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f)};
+      if (streamed) {
+        load(0, q);
+        put(0, q, 0);
+        if (lk > 1) load(1, q);
       }
-      wgmma_commit();
-      // every iteration leaves exactly chunk kc in flight: a wait on a path of its own (the last chunk's) would make
-      // ptxas drain the wgmmas at the end of every iteration
-      wgmma_wait<1>();                    // chunk kc - 1 complete: its A buffer and W stage are free
-      if (kc > 0) release(g - 1);
-      if (kc + 1 < nk) {
-        put((kc + 1) & 1, q, kc + 1);
-        if (kc + 2 < nk) load(kc + 2, q);
+      for (int kc = 0; kc < lk; ++kc, ++g) {
+        if (streamed || kc == 0) {        // this warpgroup's A writes -> visible to its wgmmas
+          fence_proxy_async_smem();
+          warpgroup_sync(1 + wgi);
+        }
+        mbar_wait(&full[uint32_t(g) & ring_mask], uint32_t((g >> ring_log2) & 1));
+        wgmma_fence();
+        const uint32_t a_base = smem_u32(my_a + uint32_t(streamed ? (kc & 1) : kc) * kABytes);
+        const uint32_t b_base = smem_u32(bring + (uint32_t(g) & ring_mask) * stage_bytes);
+        const uint64_t a_hi = make_smem_desc(a_base, 128, 256), a_lo = make_smem_desc(a_base + kABytes / 2, 128, 256);
+#pragma unroll
+        for (int i = 0; i < ns; ++i) {
+          const uint64_t b_hi = make_smem_desc(b_base + uint32_t(i * ni) * 32u, 128, 256);
+          const uint64_t b_lo = make_smem_desc(b_base + uint32_t(ni * ns) * 32u + uint32_t(i * ni) * 32u, 128, 256);
+          wgmma_bf16<ni>(lacc[i], a_hi, b_hi, kc > 0 ? 1 : 0);
+          wgmma_bf16<ni>(lacc[i], a_lo, b_hi, 1);
+          wgmma_bf16<ni>(lacc[i], a_hi, b_lo, 1);
+        }
+        wgmma_commit();
+        // every iteration leaves exactly chunk kc in flight: a wait on a path of its own (the last chunk's) would
+        // make ptxas drain the wgmmas at the end of every iteration
+        wgmma_wait<1>();                  // chunk kc - 1 complete: its A buffer and W stage are free
+        if (kc > 0) release(g - 1);
+        if (streamed && kc + 1 < lk) {
+          put((kc + 1) & 1, q, kc + 1);
+          if (kc + 2 < lk) load(kc + 2, q);
+        }
+      }
+      wgmma_wait<0>();
+      release(g - 1);
+    };
+    // ---- on-chip pooling layers: relu(acc + b) split into hi / lo over this warpgroup's own (now dead) input in
+    // the region, the first kp_next k of the next layer's A.  A lane's pair (row, cols 8 j + cq, + 1) is one
+    // 4-byte word of a core matrix: a warp writes 128 contiguous bytes per store, free of bank conflicts
+    auto to_region = [&](auto& lacc, const float* bias, int kp_next) {
+      using Acc = std::remove_reference_t<decltype(lacc)>;
+      constexpr int ns = int(std::extent<Acc, 0>::value), ni = 2 * int(std::extent<Acc, 1>::value);
+      const int cq = (lane & 3) * 2;
+#pragma unroll
+      for (int i = 0; i < ns; ++i)
+#pragma unroll
+        for (int jj = 0; jj < ni / 8; ++jj) {
+          const int col = i * ni + jj * 8 + cq;
+          if (i * ni + jj * 8 < kp_next) {
+            const float b0 = __ldg(bias + col), b1 = __ldg(bias + col + 1);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              uint32_t hi, lo;
+              split_bf16x2(fmaxf(lacc[i][4 * jj + 2 * h] + b0, 0.0f), fmaxf(lacc[i][4 * jj + 2 * h + 1] + b1, 0.0f), &hi, &lo);
+              uint8_t* dstp = my_a + uint32_t(col >> 4) * kABytes + uint32_t(warp * 2 + h) * 256u +
+                              uint32_t((col >> 3) & 1) * 128u + uint32_t(lane >> 2) * 16u + uint32_t(cq) * 2u;
+              *reinterpret_cast<uint32_t*>(dstp) = hi;
+              *reinterpret_cast<uint32_t*>(dstp + kABytes / 2) = lo;
+            }
+          }
+        }
+    };
+    if (kProd == PROD_POOL) {
+      for (int l = 0; l < nl; ++l) {
+        const int4 c = p.chain[l];
+        const float* bias = reinterpret_cast<const float*>(p.chain_buf + c.w);
+        const int kp_next = l + 1 < nl ? p.chain[l + 1].x * 16 : p.kp;
+        switch (c.y) {
+          case 64 * 4 + 1: { float a[1][32] = {}; mma_layer(a, c.x, l == 0); to_region(a, bias, kp_next); } break;
+          case 128 * 4 + 1: { float a[1][64] = {}; mma_layer(a, c.x, l == 0); to_region(a, bias, kp_next); } break;
+          case 96 * 4 + 2: { float a[2][48] = {}; mma_layer(a, c.x, l == 0); to_region(a, bias, kp_next); } break;
+          case 128 * 4 + 2: { float a[2][64] = {}; mma_layer(a, c.x, l == 0); to_region(a, bias, kp_next); } break;
+          default: { float a[2][76] = {}; mma_layer(a, c.x, l == 0); to_region(a, bias, kp_next); } break;
+        }
       }
     }
-    wgmma_wait<0>();
-    release(g - 1);
+    // every accumulator is defined before its layer (the wgmmas read it, if only to scale it by 0): otherwise the
+    // values of the previous tile would stay live through the on-chip layers, next to their accumulators
+    float acc[NS][NI / 2];
+    if (kProd == PROD_POOL)
+#pragma unroll
+      for (int i = 0; i < NS; ++i)
+#pragma unroll
+        for (int v = 0; v < NI / 2; ++v) acc[i][v] = 0.0f;
+    mma_layer(acc, nk, nl == 0);
     // ---- epilogue ----------------------------------------------------------------------------------
     const int64_t r0 = tile * kTileRows + wgi * 64 + warp * 16 + (lane >> 2);
     const int cq = (lane & 3) * 2;
@@ -426,7 +519,7 @@ WgShape wg_shape(int k, int n) {
   else if (t.np <= 256) { t.ni = 128; t.ns = 2; }
   else if (t.np <= kMaxNT) { t.ni = 152; t.ns = 2; }
   t.nt = t.ni * t.ns;
-  t.smem = wg_smem_bytes(t.nt, ring_stages(t.nt));
+  t.smem = wg_smem_bytes(uint32_t(t.nt) * 64u, 2 * kABytes, ring_stages(uint32_t(t.nt) * 64u, 2 * kABytes));
   t.ok = t.nt > 0 && k >= 1 && n >= 1;
   return t;
 }
@@ -451,12 +544,55 @@ int prepare_gemm(PreparedGemm& g, const float* w, int ld, const float* bias, int
   return PG_OK;
 }
 
+// POOL: the on-chip layers ahead of a launch's own layer (layer 1 first), their W images and padded biases packed in
+// one buffer once, when the edge layer is prepared
+struct PoolChain {
+  int layers = 0;
+  int4 table[kMaxChain] = {};   // WgParams::chain
+  uint32_t max_chunk = 0;       // widest W chunk (bytes) of these layers
+  int max_kp = 0;               // widest padded input of these layers after the first (held in the A region)
+  Temp buf;
+};
+
+// layers 1 .. own - 1 of the pooling MLP as the chain ahead of layer own
+int prepare_chain(PoolChain& c, const float* const* weights, const float* const* biases, const int32_t* dims, int own,
+                  cudaStream_t s) {
+  c.layers = std::max(0, own - 1);
+  PG_REQUIRE(c.layers <= kMaxChain, "pooling chain of %d layers", c.layers);
+  if (c.layers == 0) return PG_OK;
+  std::vector<WgShape> t(c.layers);
+  size_t bytes = 0;
+  for (int i = 0; i < c.layers; ++i) {
+    t[i] = wg_shape(dims[i + 1], dims[i + 2]);
+    PG_REQUIRE(t[i].ok, "no tensor-core shape for a %d x %d layer", dims[i + 1], dims[i + 2]);
+    c.table[i] = make_int4(t[i].kp / 16, t[i].ni * 4 + t[i].ns, int(bytes), 0);
+    bytes += size_t(t[i].kp) * t[i].nt * 4;
+    c.max_chunk = std::max(c.max_chunk, uint32_t(t[i].nt) * 64u);
+    if (i > 0) c.max_kp = std::max(c.max_kp, t[i].kp);
+  }
+  for (int i = 0; i < c.layers; ++i) {
+    c.table[i].w = int(bytes);
+    bytes += sizeof(float) * t[i].nt;
+  }
+  PG_CUDA_OK(c.buf.alloc(bytes, s));
+  for (int i = 0; i < c.layers; ++i) {
+    uint8_t* buf = c.buf.as<uint8_t>();
+    pack_b_kernel<<<std::min(num_sms(), 64), 256, 0, s>>>(weights[i + 1], dims[i + 1], dims[i + 2], dims[i + 2], t[i].kp,
+                                                          t[i].nt, buf + c.table[i].z);
+    PG_LAUNCH_CHECK();
+    pad_rows_kernel<<<2, 256, 0, s>>>(biases[i + 1], 1, dims[i + 2], t[i].nt, reinterpret_cast<float*>(buf + c.table[i].w));
+    PG_LAUNCH_CHECK();
+  }
+  return PG_OK;
+}
+
 template <int kProd, int kEpi, int NI, int NS>
 int launch_wg_cfg(const WgParams& p, size_t smem, cudaStream_t s) {
   static bool attr_done = false;
   if (!attr_done) {
+    // a pooling chain's footprint depends on its layers, not only on the instance
     PG_CUDA_OK(cudaFuncSetAttribute(wg_gemm_kernel<kProd, kEpi, NI, NS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    int(smem < 48 * 1024 ? 48 * 1024 : 227 * 1024)));
+                                    int(kProd != PROD_POOL && smem < 48 * 1024 ? 48 * 1024 : 227 * 1024)));
     attr_done = true;
   }
   const int grid = int(std::min<int64_t>(p.num_tiles, num_sms()));
@@ -466,8 +602,9 @@ int launch_wg_cfg(const WgParams& p, size_t smem, cudaStream_t s) {
   return PG_OK;
 }
 
+// POOL launches run the chain's layers ahead of g (none without a chain)
 template <int kProd, int kEpi>
-int launch_wg(WgParams p, const PreparedGemm& g, cudaStream_t s) {
+int launch_wg(WgParams p, const PreparedGemm& g, cudaStream_t s, const PoolChain* chain = nullptr) {
   if (p.num_rows == 0) return PG_OK;
   p.kp = g.t.kp;
   p.nchunks = g.t.kp / 16;
@@ -475,13 +612,30 @@ int launch_wg(WgParams p, const PreparedGemm& g, cudaStream_t s) {
   p.bias = g.bias_pad.as<float>();
   p.n = g.n;
   p.num_tiles = ceil_div(p.num_rows, kTileRows);
-  PG_REQUIRE(g.t.smem <= 227 * 1024, "tensor-core kernel needs %zu B of shared memory", g.t.smem);
+  size_t smem = g.t.smem;
+  if (kProd == PROD_POOL) {
+    // ring stages hold the widest chunk of any layer; a warpgroup's A region holds layer 1's double buffer and the
+    // widest activation the chain keeps on chip (the input of every later layer, up to g's own)
+    p.chain_layers = chain ? chain->layers : 0;
+    p.stage_bytes = uint32_t(g.t.nt) * 64u;
+    p.region_bytes = 2 * kABytes;
+    if (p.chain_layers > 0) {
+      std::copy(chain->table, chain->table + kMaxChain, p.chain);
+      p.chain_buf = chain->buf.as<uint8_t>();
+      p.stage_bytes = std::max(p.stage_bytes, chain->max_chunk);
+      p.region_bytes = std::max(p.region_bytes, uint32_t(std::max(chain->max_kp, g.t.kp)) * 256u);
+    }
+    const int ring = ring_stages(p.stage_bytes, p.region_bytes);
+    p.ring_log2 = log2_ring(ring);
+    smem = wg_smem_bytes(p.stage_bytes, p.region_bytes, ring);
+  }
+  PG_REQUIRE(smem <= 227 * 1024, "tensor-core kernel needs %zu B of shared memory", smem);
   switch (g.t.ni * 4 + g.t.ns) {
-    case 64 * 4 + 1: return launch_wg_cfg<kProd, kEpi, 64, 1>(p, g.t.smem, s);
-    case 128 * 4 + 1: return launch_wg_cfg<kProd, kEpi, 128, 1>(p, g.t.smem, s);
-    case 96 * 4 + 2: return launch_wg_cfg<kProd, kEpi, 96, 2>(p, g.t.smem, s);
-    case 128 * 4 + 2: return launch_wg_cfg<kProd, kEpi, 128, 2>(p, g.t.smem, s);
-    case 152 * 4 + 2: return launch_wg_cfg<kProd, kEpi, 152, 2>(p, g.t.smem, s);
+    case 64 * 4 + 1: return launch_wg_cfg<kProd, kEpi, 64, 1>(p, smem, s);
+    case 128 * 4 + 1: return launch_wg_cfg<kProd, kEpi, 128, 1>(p, smem, s);
+    case 96 * 4 + 2: return launch_wg_cfg<kProd, kEpi, 96, 2>(p, smem, s);
+    case 128 * 4 + 2: return launch_wg_cfg<kProd, kEpi, 128, 2>(p, smem, s);
+    case 152 * 4 + 2: return launch_wg_cfg<kProd, kEpi, 152, 2>(p, smem, s);
     default: break;
   }
   PG_REQUIRE(false, "tensor-core kernel: no instance for N = %d", g.t.nt);
@@ -591,10 +745,14 @@ struct PreparedEdge {
   // GNN: W1[C:] as [3, kp];  POOL: W0 [4, kp] + b0 [kp]
   Temp w1x;
   // the per-edge layers: GNN - W2 in column blocks;  POOL - layers 1 .. L-1, the last one in column blocks
-  std::vector<PreparedGemm> mid;      // POOL layers 1 .. L-2 (stored per edge)
   std::vector<PreparedGemm> last;     // the segment-max layer, column blocks
   std::vector<int> last_col0;
-  int mid_width = 0;                  // widest stored per-edge activation (POOL)
+  // POOL: one launch runs layers 1 .. chain_end per edge tile, every activation on chip: layers 1 .. chain_end - 1
+  // as its chain, then layer chain_end.  chain_end = L - 1 (the segment-max launch) unless the last layer is wider
+  // than one launch and L > 2; then chain_end = L - 2, whose output is stored per edge for the column blocks
+  int chain_end = 0;
+  PoolChain chain;
+  PreparedGemm chain_store;           // layer L - 2 when chain_end = L - 2
 };
 
 int prepare_edge(PreparedEdge& e, int mode, int c_in, const float* const* weights, const float* const* biases,
@@ -611,8 +769,8 @@ int prepare_edge(PreparedEdge& e, int mode, int c_in, const float* const* weight
   e.path = EDGE_FP32;
   if (!want_tc || num_layers < 2) return PG_OK;
   if (mode == PG_EDGE_POOL) {
-    // PointSetPooling (one feature channel): layer 0 in fp32 inside the producer of layer 1; layers 1 .. L-2
-    // store their per-edge activations (rows for the next layer); layer L-1 ends in the segment max
+    // PointSetPooling (one feature channel): layer 0 in fp32 inside the producer of layer 1, the following layers
+    // chained on chip (PoolChain), the last one ending in the segment max
     if (c_in != 1) return PG_OK;
     for (int l = 1; l < num_layers; ++l) {
       if (l > 1 && dims[l] % 4 != 0) return PG_OK;
@@ -624,12 +782,13 @@ int prepare_edge(PreparedEdge& e, int mode, int c_in, const float* const* weight
     PG_LAUNCH_CHECK();
     pad_rows_kernel<<<2, 256, 0, s>>>(biases[0], 1, dims[1], e.kp, e.w1x.as<float>() + 4 * e.kp);
     PG_LAUNCH_CHECK();
-    e.mid = std::vector<PreparedGemm>(num_layers - 2);
-    for (int l = 1; l + 1 < num_layers; ++l) {
-      if (int rc = prepare_gemm(e.mid[l - 1], weights[l], dims[l + 1], biases[l], dims[l], dims[l + 1], s)) return rc;
-      e.mid_width = std::max(e.mid_width, int(dims[l + 1]));
-    }
     const int n = dims[num_layers];
+    e.chain_end = (n <= kMaxNT || num_layers == 2) ? num_layers - 1 : num_layers - 2;
+    if (int rc = prepare_chain(e.chain, weights, biases, dims, e.chain_end, s)) return rc;
+    if (e.chain_end < num_layers - 1) {
+      const int l = e.chain_end;
+      if (int rc = prepare_gemm(e.chain_store, weights[l], dims[l + 1], biases[l], dims[l], dims[l + 1], s)) return rc;
+    }
     if (int rc = prepare_column_blocks(e.last, e.last_col0, weights[num_layers - 1], n, biases[num_layers - 1],
                                        dims[num_layers - 1], n, n, s))
       return rc;
@@ -659,7 +818,7 @@ int apply_last(const PreparedEdge& e, WgParams p, int n, float* out, cudaStream_
   for (size_t b = 0; b < e.last.size(); ++b) {
     p.out = out + e.last_col0[b];
     p.ldo = n;
-    if (int rc = launch_wg<kProd, EPI_SEGMAX>(p, e.last[b], s)) return rc;
+    if (int rc = launch_wg<kProd, EPI_SEGMAX>(p, e.last[b], s, &e.chain)) return rc;
   }
   return PG_OK;
 }
@@ -684,46 +843,37 @@ int launch_edge(const PreparedEdge& e, const float* features, const float* xyz_s
   if (e.path == EDGE_POOL) {
     const int L = e.num_layers;
     p.feat = features;
-    if (L == 2) {
-      p.src = src;
-      p.dst = dst;
-      p.num_rows = num_edges;
-      return apply_last<PROD_POOL>(e, p, n, out, s);
-    }
-    // the stored per-edge activations are bounded by slicing the edge list (a destination whose edges straddle
-    // two slices is merged by the atomic max like any tile boundary)
+    p.ldx = e.kp;
+    p.src = src;
+    p.dst = dst;
+    p.num_rows = num_edges;
+    if (e.chain_end == L - 1) return apply_last<PROD_POOL>(e, p, n, out, s);
+    // the last layer is wider than one launch: the chain stores its input once, and its column blocks read it back.
+    // The stored rows are bounded by slicing the edge list (a destination whose edges straddle two slices is merged
+    // by the atomic max like any tile boundary)
+    const int k_last = e.dims[L - 1];
     const int64_t slice = std::min<int64_t>(num_edges, int64_t(1) << 20);
-    Temp h[2];
-    PG_CUDA_OK(h[0].alloc(sizeof(float) * slice * e.mid_width, s));
-    if (L > 3) PG_CUDA_OK(h[1].alloc(sizeof(float) * slice * e.mid_width, s));
+    Temp h;
+    PG_CUDA_OK(h.alloc(sizeof(float) * slice * k_last, s));
     for (int64_t e0 = 0; e0 < num_edges; e0 += slice) {
       const int64_t ne = std::min(slice, num_edges - e0);
       WgParams q = p;
       q.src = src + e0;
       q.dst = dst + e0;
       q.num_rows = ne;
-      q.out = h[0].as<float>();
-      q.ldo = e.dims[2];
+      q.out = h.as<float>();
+      q.ldo = k_last;
       q.act = 1;
-      if (int rc = launch_wg<PROD_POOL, EPI_STORE>(q, e.mid[0], s)) return rc;
-      for (int l = 2; l < L; ++l) {
-        WgParams r{};
-        r.x = h[l & 1].as<float>();
-        r.ldx = e.dims[l];
-        r.k_real = e.dims[l];
-        r.num_rows = ne;
-        r.dst = dst + e0;
-        r.num_dst = num_dst;
-        r.err = err;
-        if (l + 1 < L) {
-          r.out = h[(l + 1) & 1].as<float>();
-          r.ldo = e.dims[l + 1];
-          r.act = 1;
-          if (int rc = launch_wg<PROD_ROWS, EPI_STORE>(r, e.mid[l - 1], s)) return rc;
-        } else if (int rc = apply_last<PROD_ROWS>(e, r, n, out, s)) {
-          return rc;
-        }
-      }
+      if (int rc = launch_wg<PROD_POOL, EPI_STORE>(q, e.chain_store, s, &e.chain)) return rc;
+      WgParams r{};
+      r.x = h.as<float>();
+      r.ldx = k_last;
+      r.k_real = k_last;
+      r.num_rows = ne;
+      r.dst = dst + e0;
+      r.num_dst = num_dst;
+      r.err = err;
+      if (int rc = apply_last<PROD_ROWS>(e, r, n, out, s)) return rc;
     }
     return PG_OK;
   }
