@@ -274,9 +274,36 @@ PG_API int pg_gather_rows(const float* params, int64_t num_rows, int32_t num_cha
                    const int32_t* indices, int64_t num_indices, float* out, void* stream);
 
 /*
+ * Activations: the entries of the reference's activation_fn_dict (gnn.py:24-32).  Every one is monotone
+ * non-decreasing, so the fused segment max applies it once per reduced value.
+ *   PG_ACT_NONE        x (also the is_logits last layer)
+ *   PG_ACT_RELU        max(x, 0)
+ *   PG_ACT_RELU6       min(max(x, 0), 6)
+ *   PG_ACT_LEAKY_RELU  x > 0 ? x : 0.01 x      (alpha 0.01, gnn.py:28)
+ *   PG_ACT_ELU         x > 0 ? x : exp(x) - 1
+ *   PG_ACT_SIGMOID     1 / (1 + exp(-x))
+ *   PG_ACT_TANH        tanh(x)
+ * The prepared layers and pg_edge_mlp_max take the activation in the flag bits of their `precision` word:
+ * PG_PRECISION_ACTIVATION(code) = PG_FLAG_ACTIVATION | code << PG_ACT_SHIFT.  Without PG_FLAG_ACTIVATION the
+ * activation is ReLU; a code outside [0, PG_ACT_COUNT) gives PG_ERR_INVALID_ARGUMENT.
+ */
+#define PG_ACT_NONE 0
+#define PG_ACT_RELU 1
+#define PG_ACT_RELU6 2
+#define PG_ACT_LEAKY_RELU 3
+#define PG_ACT_ELU 4
+#define PG_ACT_SIGMOID 5
+#define PG_ACT_TANH 6
+#define PG_ACT_COUNT 7
+#define PG_FLAG_ACTIVATION 0x200
+#define PG_ACT_SHIFT 16
+#define PG_ACT_MASK 0xff0000
+#define PG_PRECISION_ACTIVATION(code) (PG_FLAG_ACTIVATION | ((code) << PG_ACT_SHIFT))
+
+/*
  * One slim.fully_connected layer (gnn.py:63-80,93-103), normalizer NONE:
  *   out[M,N] = act(x[M,K] @ w[K,N] + bias[N]) (+ residual[M,N] if not NULL)
- * act: 0 = linear (the is_logits last layer), 1 = ReLU.
+ * act: a PG_ACT_* code; 0 = linear (the is_logits last layer), 1 = ReLU.
  * precision: 0 = fp32 FFMA, 1 = wgmma BF16x3 split (fp32-class accuracy).
  */
 PG_API int pg_fully_connected(const float* x, int64_t m, int32_t k, const float* w, const float* bias,
@@ -293,7 +320,7 @@ PG_API int pg_fully_connected(const float* x, int64_t m, int32_t k, const float*
  *   mode PG_EDGE_GNN  : e0 = concat(vertex_features[src], xyz_src[src] - xyz_dst[dst])
  *                       xyz_src = un-offset coords, xyz_dst = coords + auto-offset
  *                       (gnn.py:338-352; SURVEY fact 4)
- *   then num_layers x relu(. @ W_l + b_l)      (is_logits=False, gnn.py:99-103)
+ *   then num_layers x act(. @ W_l + b_l)       (is_logits=False, gnn.py:99-103)
  *   then out[k,:] = max over the edges of destination k   (gnn.py:362-365)
  *
  *   src, dst     [E] int32; dst must be non-decreasing (CSR order, as produced by
@@ -309,6 +336,7 @@ PG_API int pg_fully_connected(const float* x, int64_t m, int32_t k, const float*
  *                pg_radius_graph, or passed pg_check_edges), so the call skips the device->host
  *                read-back of the range-error flag and does not synchronise the stream.  Out-of-range
  *                indices are still clamped on the device (never dereferenced), just not reported.
+ *                act is ReLU unless precision carries PG_PRECISION_ACTIVATION(code).
  */
 #define PG_PRECISION_MASK 0xff
 #define PG_FLAG_TRUSTED_INDICES 0x100
@@ -349,7 +377,9 @@ PG_API int pg_check_edges(const int32_t* src, const int32_t* dst, int64_t num_ed
  *                            reference creates them: cls fc (D->H), cls fc_1 (H->C), then
  *                            for every class c: loc fc (D->H), fc_1 (H->H), fc_2 (H->box_len);
  *                            num_layers = 2 + 3 C.
- *   precision 0 = fp32 FFMA, 1 = wgmma BF16x3 wherever the shapes allow.
+ *   precision 0 = fp32 FFMA, 1 = wgmma BF16x3 wherever the shapes allow; may be OR-ed with
+ *             PG_PRECISION_ACTIVATION(code): the activation of every layer that has one (default ReLU).
+ *             It is fixed here because it selects the kernels the handle launches.
  * ------------------------------------------------------------------------ */
 typedef struct pg_layer pg_layer;
 #define PG_LAYER_MLP 0
@@ -362,7 +392,7 @@ PG_API int pg_layer_create(int32_t kind, const float* const* weights_host, const
 PG_API int pg_layer_destroy(pg_layer* layer);
 
 /* multi_layer_neural_network_fn / multi_layer_fc_fn (gnn.py:34-104) on a prepared chain:
- * ReLU after every layer except - when last_linear != 0 (is_logits=True) - the last;
+ * the layer's activation after every layer except - when last_linear != 0 (is_logits=True) - the last;
  * `residual` [m, dims[last]] (optional) is added to the last layer's output (gnn.py:346, 372). */
 PG_API int pg_layer_mlp(const pg_layer* layer, const float* x, int64_t m, int32_t last_linear,
                  const float* residual, float* out, void* stream);

@@ -96,6 +96,24 @@ SIGNATURES = {
 }
 PG_LAYER_MLP, PG_LAYER_EDGE_POOL, PG_LAYER_EDGE_GNN, PG_LAYER_PREDICTOR = 0, 1, 2, 3
 PG_FLAG_TRUSTED_INDICES = 0x100
+# activations (models/gnn.py's activation_fn_dict maps the reference's names to these)
+PG_ACT_NONE, PG_ACT_RELU, PG_ACT_RELU6, PG_ACT_LEAKY_RELU, PG_ACT_ELU, PG_ACT_SIGMOID, PG_ACT_TANH = range(7)
+PG_ACT_COUNT = 7
+PG_FLAG_ACTIVATION, PG_ACT_SHIFT = 0x200, 16
+PG_ERR_INVALID_ARGUMENT = -1
+
+
+def _act_code(activation):
+    """A PG_ACT_* code, checked here: a code outside [0, PG_ACT_COUNT) would not survive the int32 argument intact."""
+    code = int(activation)
+    if not 0 <= code < PG_ACT_COUNT:
+        raise PointGNNError(PG_ERR_INVALID_ARGUMENT, 'unknown activation code %d' % code)
+    return code
+
+
+def _activation_flags(activation):
+    """The precision-word flag bits that select a PG_ACT_* activation."""
+    return PG_FLAG_ACTIVATION | (_act_code(activation) << PG_ACT_SHIFT)
 
 _lib = None
 
@@ -419,8 +437,11 @@ def _check_fc_shapes(x, k, n, residual):
         raise ValueError('fully_connected: residual shape %s != output shape (%d, %d)' % (tuple(residual.shape), m, n))
 
 
-def fully_connected(x, w, b, relu, residual=None, precision=0):
+def fully_connected(x, w, b, relu, residual=None, precision=0, activation=None):
+    """activation: a PG_ACT_* code; None = ReLU or linear as ``relu`` says."""
     lib = load()
+    if activation is None:
+        activation = PG_ACT_RELU if relu else PG_ACT_NONE
     m, k = x.shape
     n = w.shape[1]
     _check_fc_shapes(x, w.shape[0], n, residual)
@@ -428,7 +449,7 @@ def fully_connected(x, w, b, relu, residual=None, precision=0):
         raise ValueError('fully_connected: bias has %d entries, layer width is %d' % (b.numel(), n))
     out = torch.empty((m, n), dtype=torch.float32, device=x.device)
     _check(lib.pg_fully_connected(_ptr(x, torch.float32, 'x'), m, k, _ptr(w, torch.float32, 'w'),
-                                  _ptr(b, torch.float32, 'b'), n, 1 if relu else 0,
+                                  _ptr(b, torch.float32, 'b'), n, _act_code(activation),
                                   _ptr(residual, torch.float32, 'residual'), _ptr(out, torch.float32, 'out'),
                                   int(precision), _stream()))
     return out
@@ -442,9 +463,10 @@ def check_edges(src, dst, num_src, num_dst):
 
 
 def edge_mlp_max(mode, features, xyz_src, xyz_dst, dst_index, src, dst, num_dst, weights, biases, precision=0,
-                 trusted=False):
+                 trusted=False, activation=PG_ACT_RELU):
     """trusted=True: the caller vouches for the index ranges (graph_gen output / check_edges passed); the call
-    then does not read the range-error flag back and does not synchronise the stream."""
+    then does not read the range-error flag back and does not synchronise the stream.  activation: the PG_ACT_* code
+    applied after every layer."""
     lib = load()
     num_layers = len(weights)
     dims = [weights[0].shape[0]] + [w.shape[1] for w in weights]
@@ -457,7 +479,8 @@ def edge_mlp_max(mode, features, xyz_src, xyz_dst, dst_index, src, dst, num_dst,
                                _ptr(dst_index, torch.int32, 'dst_index'), _ptr(src, torch.int32, 'src'),
                                _ptr(dst, torch.int32, 'dst'), src.numel(), features.shape[0], int(num_dst), wp, bp,
                                dm, num_layers, _ptr(out, torch.float32, 'out'),
-                               int(precision) | (PG_FLAG_TRUSTED_INDICES if trusted else 0), _stream()))
+                               int(precision) | (PG_FLAG_TRUSTED_INDICES if trusted else 0) | _activation_flags(activation),
+                               _stream()))
     return out
 
 
@@ -475,10 +498,12 @@ def softmax_rows(logits):
 class PreparedLayer(object):
     """Owner of one ``pg_layer`` handle.  Keeps the weight tensors alive: the C side stores their pointers."""
 
-    def __init__(self, kind, weights, biases, dims, precision=0):
+    def __init__(self, kind, weights, biases, dims, precision=0, activation=PG_ACT_RELU):
+        """activation: the PG_ACT_* code of every layer that has one (the is_logits last layers stay linear)."""
         lib = load()
         n = len(weights)
         self.kind = int(kind)
+        self.activation = int(activation)
         self.dims = [int(d) for d in dims]
         self._keep = (list(weights), list(biases))
         wp = (ctypes.c_void_p * n)(*[_ptr(w, torch.float32, 'weight').value for w in weights])
@@ -486,7 +511,8 @@ class PreparedLayer(object):
         dm = (c_i32 * len(self.dims))(*self.dims)
         handle = ctypes.c_void_p()
         self._handle = None
-        _check(lib.pg_layer_create(self.kind, wp, bp, dm, n, int(precision), _stream(), ctypes.byref(handle)))
+        _check(lib.pg_layer_create(self.kind, wp, bp, dm, n, int(precision) | _activation_flags(activation), _stream(),
+                                   ctypes.byref(handle)))
         self._handle = handle
 
     def __del__(self):

@@ -99,6 +99,29 @@ __device__ __forceinline__ void atomic_max_float(float* addr, float v) {
     atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(v));
 }
 
+// The PG_ACT_* activations, the one definition every kernel calls.  TF 1.15 semantics as recalled (TF's source is
+// not at hand to check against): leaky_relu with the alpha 0.01 the reference passes; elu is exp(x) - 1 below zero
+// in TF, expm1f here (they differ by < 1e-7).  The accurate CUDA functions, not the __expf intrinsics.  Each one is
+// monotone non-decreasing, which the fused segment max relies on: max_e f(a_e + b) = f(max_e a_e + b).
+__device__ __forceinline__ float activate(int act, float x) {
+  switch (act) {
+    case PG_ACT_RELU: return fmaxf(x, 0.0f);
+    case PG_ACT_RELU6: return fminf(fmaxf(x, 0.0f), 6.0f);
+    case PG_ACT_LEAKY_RELU: return x > 0.0f ? x : 0.01f * x;
+    case PG_ACT_ELU: return x > 0.0f ? x : expm1f(x);
+    case PG_ACT_SIGMOID: return 1.0f / (1.0f + expf(-x));
+    case PG_ACT_TANH: return tanhf(x);
+    default: return x;   // PG_ACT_NONE
+  }
+}
+
+// the activation a precision word's flag bits select (ReLU without PG_FLAG_ACTIVATION); -1 for an unknown code
+inline int activation_of(int32_t precision) {
+  if (!(precision & PG_FLAG_ACTIVATION)) return PG_ACT_RELU;
+  const uint32_t act = uint32_t(precision) >> PG_ACT_SHIFT;   // every bit above the field counts: 256 is not 0
+  return act < PG_ACT_COUNT ? int(act) : -1;
+}
+
 // float <-> order-preserving uint: a < b iff float_to_ordered(a) < float_to_ordered(b), for any non-NaN values
 __device__ inline uint32_t float_to_ordered(float f) {
   uint32_t b = __float_as_uint(f);
@@ -130,12 +153,16 @@ int fill_async(float* p, int64_t n, float v, cudaStream_t s);
 // out [m, ldo] = act(x [m, k] @ w [k, n] + bias) (+ residual [m, n]); columns [n, ldo) are written as zeros
 int fc_fp32_launch(const float* x, int64_t m, int k, const float* w, const float* bias, int n, int act,
                    const float* residual, float* out, int ldo, cudaStream_t s);
-// pg_edge_simt.cu: the fp32 FFMA edge MLP + segment max into out (already filled with -FLT_MAX); sets *err on an
-// out-of-range src / dst
+// out [rows, ldo], columns [0, n): v = act(v + bias) (+ residual [rows, ldr]); bias and residual may be null.
+// skip_empty leaves -FLT_MAX (an empty segment of a segment max) as it is
+int activate_rows(float* out, int64_t rows, int n, int ldo, const float* bias, int act, const float* residual, int ldr,
+                  bool skip_empty, cudaStream_t s);
+// pg_edge_simt.cu: the fp32 FFMA edge MLP (activation act after every layer) + segment max into out (already
+// filled with -FLT_MAX); sets *err on an out-of-range src / dst
 int edge_mlp_max_fp32(int mode, const float* features, int c_in, const float* xyz_src, const float* xyz_dst,
                       const int32_t* dst_index, const int32_t* src, const int32_t* dst, int64_t num_edges,
                       int64_t num_src, int64_t num_dst, const float* const* weights, const float* const* biases,
-                      const int32_t* dims, int num_layers, float* out, int* err, cudaStream_t s);
+                      const int32_t* dims, int num_layers, int act, float* out, int* err, cudaStream_t s);
 
 inline int num_sms() {
   static int sms = 0;

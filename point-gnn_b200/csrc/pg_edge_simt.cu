@@ -3,7 +3,7 @@
 // Replaces, without materialising any [E, *] tensor in HBM:
 //   PointSetPooling.apply_regular   /root/reference/models/gnn.py:256-277
 //   GraphNetAutoCenter.apply_regular /root/reference/models/gnn.py:338-365
-// (gather -> concat(feature, relative xyz) -> L x relu(x@W+b) -> unsorted_segment_max).
+// (gather -> concat(feature, relative xyz) -> L x act(x@W+b) -> unsorted_segment_max).
 //
 // One persistent CTA per SM walks 64-edge tiles.  The tile's activations ping-pong between two
 // shared-memory buffers, each layer is a register-tiled FFMA GEMM against weights streamed
@@ -38,6 +38,7 @@ struct EdgeMlpParams {
   const float* b[kMaxLayers];
   int dims[kMaxLayers + 1];
   int num_layers;
+  int act;               // PG_ACT_* after every layer
   int stride0, stride1;  // row strides (floats) of the two activation buffers
   float* out;
   int* err;
@@ -85,7 +86,7 @@ __global__ void __launch_bounds__(kThreads, 1) edge_mlp_max_fp32_kernel(EdgeMlpP
       }
     }
     __syncthreads();
-    // ---- L x relu(x @ W + b) ------------------------------------------------------------------
+    // ---- L x act(x @ W + b) -------------------------------------------------------------------
     for (int l = 0; l < p.num_layers; ++l) {
       const float* in = (l & 1) ? buf1 : buf0;
       float* outb = (l & 1) ? buf0 : buf1;
@@ -124,7 +125,7 @@ __global__ void __launch_bounds__(kThreads, 1) edge_mlp_max_fp32_kernel(EdgeMlpP
             const float bv = bias[c];
 #pragma unroll
             for (int r = 0; r < 8; ++r)
-              outb[size_t(warp * 8 + r) * out_stride + c] = fmaxf(acc[r][j] + bv, 0.0f);
+              outb[size_t(warp * 8 + r) * out_stride + c] = activate(p.act, acc[r][j] + bv);
           }
         }
       }
@@ -156,7 +157,7 @@ __global__ void __launch_bounds__(kThreads, 1) edge_mlp_max_fp32_kernel(EdgeMlpP
 int edge_mlp_max_fp32(int mode, const float* features, int c_in, const float* xyz_src, const float* xyz_dst,
                       const int32_t* dst_index, const int32_t* src, const int32_t* dst, int64_t num_edges,
                       int64_t num_src, int64_t num_dst, const float* const* weights, const float* const* biases,
-                      const int32_t* dims, int num_layers, float* out, int* err, cudaStream_t s) {
+                      const int32_t* dims, int num_layers, int act, float* out, int* err, cudaStream_t s) {
   PG_REQUIRE(num_layers >= 1 && num_layers <= kMaxLayers, "edge MLP depth %d not in [1,%d]", num_layers, kMaxLayers);
   PG_REQUIRE(dims[0] == c_in + 3, "dims[0]=%d must equal feature channels + 3 = %d", dims[0], c_in + 3);
   EdgeMlpParams p{};
@@ -183,6 +184,7 @@ int edge_mlp_max_fp32(int mode, const float* features, int c_in, const float* xy
     p.b[l] = biases[l];
   }
   p.num_layers = num_layers;
+  p.act = act;
   p.stride0 = w0 + 1;
   p.stride1 = w1 + 1;
   p.out = out;

@@ -3,7 +3,7 @@
 // Replaces the TF ops behind /root/reference/models/gnn.py:
 //   graph_scatter_max_fn  (:106-109, tf.math.unsorted_segment_max)
 //   tf.gather             (:256-262, :338-348)
-//   slim.fully_connected  (:63-80, :93-103)   normalizer NONE, activation ReLU / none
+//   slim.fully_connected  (:63-80, :93-103)   normalizer NONE, any PG_ACT_* activation
 //   tf.nn.softmax         (models.py:165-168)
 #include "pg_common.cuh"
 
@@ -216,10 +216,23 @@ __global__ void __launch_bounds__(256) fc_fp32_kernel(const float* __restrict__ 
       if (gc >= ldo) continue;
       if (gc >= n) { out[gr * ldo + gc] = 0.0f; continue; }   // zero padding columns [n, ldo)
       float v = acc[i][j] + bias[gc];
-      if (act == 1) v = fmaxf(v, 0.0f);
+      v = activate(act, v);
       if (residual != nullptr) v += residual[gr * n + gc];
       out[gr * ldo + gc] = v;
     }
+  }
+}
+
+__global__ void activate_rows_kernel(float* __restrict__ out, int64_t rows, int n, int ldo, const float* __restrict__ bias,
+                                     int act, const float* __restrict__ residual, int ldr, bool skip_empty) {
+  for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < rows * n; i += int64_t(gridDim.x) * blockDim.x) {
+    const int64_t r = i / n;
+    const int c = int(i - r * n);
+    float v = out[r * ldo + c];
+    if (skip_empty && v == -FLT_MAX) continue;
+    v = activate(act, bias ? v + bias[c] : v);
+    if (residual) v += residual[r * ldr + c];
+    out[r * ldo + c] = v;
   }
 }
 
@@ -251,6 +264,15 @@ int fc_fp32_launch(const float* x, int64_t m, int k, const float* w, const float
   PG_REQUIRE(ldo >= n && ldo <= (n + kTN - 1) / kTN * kTN, "fc: bad output stride %d for n=%d", ldo, n);
   dim3 grid(ceil_div(n, kTN), ceil_div(m, kTM));
   fc_fp32_kernel<<<grid, 256, 0, s>>>(x, m, k, w, bias, n, act, residual, out, ldo);
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}
+
+int activate_rows(float* out, int64_t rows, int n, int ldo, const float* bias, int act, const float* residual, int ldr,
+                  bool skip_empty, cudaStream_t s) {
+  if (rows == 0) return PG_OK;
+  const int grid = int(std::min<int64_t>(ceil_div(rows * n, 256), int64_t(num_sms()) * 8));
+  activate_rows_kernel<<<grid, 256, 0, s>>>(out, rows, n, ldo, bias, act, residual, ldr, skip_empty);
   PG_LAUNCH_CHECK();
   return PG_OK;
 }

@@ -8,15 +8,22 @@
 //              PROD_GNN   one GNN iteration's edge MLP (/root/reference/models/gnn.py:338-365) after hoisting:
 //                         e0 @ W1 + b1 = (F @ W1[:C] + b1)[src] + (x_src - x_dst') @ W1[C:], so the first edge
 //                         layer is a per-VERTEX table P (a PROD_ROWS GEMM) plus a 3-term per-edge correction;
-//                         A row e = relu(P[src] + (x_src - x_dst') @ W1[C:])
+//                         A row e = act(P[src] + (x_src - x_dst') @ W1[C:])
 //              PROD_POOL  PointSetPooling's first layer (gnn.py:264-270) in fp32:
 //                         A row e = relu([feature(src), x_src - x_kp(dst)] @ W0 + b0), then the chain: every
 //                         further pooling layer ahead of the kernel's own runs on the same tile with its input and
 //                         output in the consumer warpgroup's shared-memory region, never in global memory
 //   epilogues  EPI_STORE  act(acc + b) (+ residual) to a row-major matrix
 //              EPI_SEGMAX max over the edges of each destination (edges are grouped by destination):
-//                         relu / bias commute with max, so raw accumulators are reduced across the warp's
-//                         16 rows with shuffles and each partial max is flushed with one atomicMax
+//                         bias and every activation are monotone, so they commute with max: raw accumulators
+//                         are reduced across the warp's 16 rows with shuffles and each partial max is flushed
+//                         with one atomic
+//   activation wg_gemm_kernel hard-codes ReLU (linear too in the store epilogue): the kernel of every shipped
+//              config.  wg_gemm_act_kernel, the GNN edge layer with any other activation, is the same body with
+//              activate(p.act, .) in the producer; its segment max flushes the RAW maxima with the sign-aware
+//              atomic_max_float (NONE, LeakyReLU, ELU and Tanh give negative values) and activate_rows applies
+//              act(. + b) once per output element afterwards.  Dense layers with another activation run
+//              wg_gemm_kernel linear, then activate_rows
 //   precision  every fp32 operand is split x = hi + lo (two BF16), and hi*hi' + lo*hi' + hi*lo' is
 //              accumulated in fp32 registers: ~2^-16 relative per product (fp32-class accuracy)
 //   mapping    CTA = 3 warpgroups.  Warpgroup 0 is the W producer (setmaxnreg down to 24 registers): one thread
@@ -105,7 +112,7 @@ struct WgParams {
   // epilogue
   float* out;               // STORE: [num_rows, ldo];  SEGMAX: [num_dst, ldo] pre-filled with -FLT_MAX
   int ldo;
-  int act;                  // STORE: 0 linear, 1 relu
+  int act;                  // STORE: 0 linear, 1 relu;  wg_gemm_act_kernel: the GNN producer's PG_ACT_*
   const float* residual;    // STORE: optional [num_rows, ldr]
   int ldr;
   int* err;
@@ -126,9 +133,22 @@ __device__ __forceinline__ float4 ldg_nc(const float* ptr) {
   return v;
 }
 
+// a layer's activation: ReLU, or with kAnyAct the PG_ACT_* code act
+template <bool kAnyAct>
+__device__ __forceinline__ float layer_act(int act, float x) {
+  return kAnyAct ? activate(act, x) : fmaxf(x, 0.0f);
+}
+
+template <bool kAnyAct>
 __device__ __forceinline__ void seg_flush(const WgParams& p, int d, int col, float m) {
-  // + 0.0f turns a -0.0f into +0.0f, which must win against the -FLT_MAX fill as an integer
-  atomicMax(reinterpret_cast<int*>(p.out + int64_t(d) * p.ldo + col), __float_as_int(fmaxf(m + __ldg(p.bias + col), 0.0f) + 0.0f));
+  float* dst = p.out + int64_t(d) * p.ldo + col;
+  if (kAnyAct) {
+    // the raw maximum, which may be negative: the sign-aware max, still one atomic (bias and activation later)
+    atomic_max_float(dst, m);
+  } else {
+    // + 0.0f turns a -0.0f into +0.0f, which must win against the -FLT_MAX fill as an integer
+    atomicMax(reinterpret_cast<int*>(dst), __float_as_int(fmaxf(m + __ldg(p.bias + col), 0.0f) + 0.0f));
+  }
 }
 
 // w[0 .. 8) = ptr[0 .. 8); ptr is 32-byte aligned
@@ -138,8 +158,8 @@ __device__ __forceinline__ void ldg8(const float* ptr, float (&w)[8]) {
   w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
 }
 
-template <int kProd, int kEpi, int NI, int NS>
-__global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
+template <int kProd, int kEpi, int NI, int NS, bool kAnyAct>
+__device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
   constexpr int NT = NI * NS;
   constexpr uint32_t kChunkBytes = uint32_t(NT) * 64u;   // hi + lo, 16 k
   constexpr int kRing = ring_stages(kChunkBytes, 2 * kABytes);
@@ -245,7 +265,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
         ldg8(p.w1x + p.kp + k0, wy);
         ldg8(p.w1x + 2 * p.kp + k0, wz);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] = fmaxf(fmaf(rz, wz[i], fmaf(ry, wy[i], fmaf(rx, wx[i], v[i]))), 0.0f);
+        for (int i = 0; i < 8; ++i) v[i] = layer_act<kAnyAct>(p.act, fmaf(rz, wz[i], fmaf(ry, wy[i], fmaf(rx, wx[i], v[i]))));
       } else if (kProd == PROD_POOL) {
         float wf[8], wx[8], wy[8], wz[8], b0[8];
         ldg8(p.w1x + k0, wf);
@@ -438,7 +458,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
 #pragma unroll
         for (int k = 0; k < L3; ++k) {
           const int v = v0 + k, col = (v >> 1) * 8 + cq + (v & 1);
-          if (k < nv && col < p.n) seg_flush(p, dw, col, m[k]);
+          if (k < nv && col < p.n) seg_flush<kAnyAct>(p, dw, col, m[k]);
         }
       } else {
         // segmented max down each 8-row half (rows of one destination are contiguous); the first row of
@@ -467,12 +487,24 @@ __global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
                   if (dn[s] == dd) m = fmaxf(m, o);
                 }
                 const int col = i * NI + jj * 8 + cq + c;
-                if (head && col < p.n) seg_flush(p, dd, col, m);
+                if (head && col < p.n) seg_flush<kAnyAct>(p, dd, col, m);
               }
         }
       }
     }
   }
+}
+
+template <int kProd, int kEpi, int NI, int NS>
+__global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
+  wg_gemm_body<kProd, kEpi, NI, NS, false>(p);
+}
+
+// its own name, so that the instance count and the ptxas properties of wg_gemm_kernel stay those of the ReLU build
+template <int kProd, int kEpi, int NI, int NS>
+__global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_act_kernel(WgParams p) {
+  static_assert(kProd == PROD_GNN && kEpi == EPI_SEGMAX, "any-activation instances: the GNN edge layer only");
+  wg_gemm_body<kProd, kEpi, NI, NS, true>(p);
 }
 
 // ---- W [K, N] -> streamed B image ---------------------------------------------------------------
@@ -588,15 +620,22 @@ int prepare_chain(PoolChain& c, const float* const* weights, const float* const*
 
 template <int kProd, int kEpi, int NI, int NS>
 int launch_wg_cfg(const WgParams& p, size_t smem, cudaStream_t s) {
-  static bool attr_done = false;
-  if (!attr_done) {
+  // the GNN edge layer with an activation other than ReLU runs the twin; everything else is ReLU or linear
+  void (*kernel)(WgParams) = wg_gemm_kernel<kProd, kEpi, NI, NS>;
+  bool any_act = false;
+  if constexpr (kProd == PROD_GNN) {
+    any_act = p.act != PG_ACT_RELU;
+    if (any_act) kernel = wg_gemm_act_kernel<kProd, kEpi, NI, NS>;
+  }
+  static bool attr_done[2] = {false, false};
+  if (!attr_done[any_act]) {
     // a pooling chain's footprint depends on its layers, not only on the instance
-    PG_CUDA_OK(cudaFuncSetAttribute(wg_gemm_kernel<kProd, kEpi, NI, NS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    PG_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                     int(kProd != PROD_POOL && smem < 48 * 1024 ? 48 * 1024 : 227 * 1024)));
-    attr_done = true;
+    attr_done[any_act] = true;
   }
   const int grid = int(std::min<int64_t>(p.num_tiles, num_sms()));
-  wg_gemm_kernel<kProd, kEpi, NI, NS><<<grid, kWgThreads, smem, s>>>(p);
+  kernel<<<grid, kWgThreads, smem, s>>>(p);
   PG_LAUNCH_CHECK();
   g_tc_launches[kEpi == EPI_SEGMAX ? 0 : 1].fetch_add(1, std::memory_order_relaxed);
   return PG_OK;
@@ -716,6 +755,11 @@ int apply_fc(const PreparedFc& f, const float* x, int64_t m, int act, const floa
     PG_REQUIRE(f.n == f.n_src || ldo == f.n, "FFMA dense layer: padded width %d needs ldo == n", f.n);
     return fc_fp32_launch(x, m, f.k, f.w, f.bias, f.n_src, act, residual, out, ldo, s);
   }
+  if (act != PG_ACT_NONE && act != PG_ACT_RELU) {
+    // the GEMM linear, then the activation and the residual in one pass over the output
+    if (int rc = apply_fc(f, x, m, PG_ACT_NONE, nullptr, out, ldo, s)) return rc;
+    return activate_rows(out, m, f.n, ldo, nullptr, act, residual, f.n, false, s);
+  }
   for (size_t b = 0; b < f.blocks.size(); ++b) {
     WgParams p{};
     p.x = x;
@@ -737,6 +781,7 @@ enum { EDGE_FP32 = 0, EDGE_GNN = 1, EDGE_POOL = 2 };
 
 struct PreparedEdge {
   int mode = 0, c_in = 0, num_layers = 0, path = EDGE_FP32;
+  int act = PG_ACT_RELU;              // after every layer of the edge MLP
   std::vector<int32_t> dims;
   std::vector<const float*> w, b;     // caller's tensors (must outlive the handle)
   // GNN: hoisted first layer P = F @ W1[:C] + b1 (zero padded to kp columns) and W1[C:]
@@ -756,10 +801,12 @@ struct PreparedEdge {
 };
 
 int prepare_edge(PreparedEdge& e, int mode, int c_in, const float* const* weights, const float* const* biases,
-                 const int32_t* dims, int num_layers, bool want_tc, cudaStream_t s) {
+                 const int32_t* dims, int num_layers, int act, bool want_tc, cudaStream_t s) {
   PG_REQUIRE(num_layers >= 1 && num_layers <= 8, "edge MLP depth %d not in [1, 8]", num_layers);
   PG_REQUIRE(dims[0] == c_in + 3, "dims[0]=%d must equal feature channels + 3 = %d", dims[0], c_in + 3);
+  PG_REQUIRE(act >= 0 && act < PG_ACT_COUNT, "edge MLP: unknown activation");
   e.mode = mode;
+  e.act = act;
   e.c_in = c_in;
   e.num_layers = num_layers;
   e.dims.assign(dims, dims + num_layers + 1);
@@ -769,6 +816,9 @@ int prepare_edge(PreparedEdge& e, int mode, int c_in, const float* const* weight
   e.path = EDGE_FP32;
   if (!want_tc || num_layers < 2) return PG_OK;
   if (mode == PG_EDGE_POOL) {
+    // the on-chip chain is built for ReLU: any-activation instances of it inline the activation at hundreds of
+    // sites and took ptxas minutes each, so other activations run the fp32 edge kernel
+    if (act != PG_ACT_RELU) return PG_OK;
     // PointSetPooling (one feature channel): layer 0 in fp32 inside the producer of layer 1, the following layers
     // chained on chip (PoolChain), the last one ending in the segment max
     if (c_in != 1) return PG_OK;
@@ -831,7 +881,7 @@ int launch_edge(const PreparedEdge& e, const float* features, const float* xyz_s
   const int n = e.dims[e.num_layers];
   if (e.path == EDGE_FP32 || num_edges == 0)
     return edge_mlp_max_fp32(e.mode, features, e.c_in, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst,
-                             e.w.data(), e.b.data(), e.dims.data(), e.num_layers, out, err, s);
+                             e.w.data(), e.b.data(), e.dims.data(), e.num_layers, e.act, out, err, s);
   WgParams p{};
   p.xyz_src = xyz_src;
   p.xyz_dst = xyz_dst;
@@ -887,6 +937,7 @@ int launch_edge(const PreparedEdge& e, const float* features, const float* xyz_s
   p.src = src;
   p.dst = dst;
   p.num_rows = num_edges;
+  p.act = e.act;
   return apply_last<PROD_GNN>(e, p, n, out, s);
 }
 
@@ -901,6 +952,11 @@ int apply_edge(const PreparedEdge& e, const float* features, const float* xyz_sr
   if (int rc = launch_edge(e, features, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst, out,
                            err.ptr(), s))
     return rc;
+  // wg_gemm_act_kernel left the raw maxima: the last layer's bias and activation, once per element
+  if (e.path != EDGE_FP32 && e.act != PG_ACT_RELU && num_edges > 0) {
+    const int n = e.dims[e.num_layers];
+    if (int rc = activate_rows(out, num_dst, n, n, e.b[e.num_layers - 1], e.act, nullptr, 0, true, s)) return rc;
+  }
   int h = 0;
   if (int rc = err.read(&h, trusted, s)) return rc;
   PG_REQUIRE(h == 0, "edge index out of range (src in [0,%lld), dst in [0,%lld))", (long long)num_src,
@@ -909,8 +965,8 @@ int apply_edge(const PreparedEdge& e, const float* features, const float* xyz_sr
 }
 
 // ---- the class-aware predictor heads (gnn.py:133-163) ---------------------------------------------
-// After the concatenated first layers (one GEMM: [D] -> H * (C + 1), ReLU) everything left is tiny per vertex:
-// cls H -> C (linear), and per class H -> H (ReLU) -> box_len (linear).  One SIMT kernel does all of it for a
+// After the concatenated first layers (one GEMM: [D] -> H * (C + 1), act) everything left is tiny per vertex:
+// cls H -> C (linear), and per class H -> H (act) -> box_len (linear).  One SIMT kernel does all of it for a
 // tile of 32 vertices with every head weight resident in shared memory, and writes logits, class
 // probabilities (softmax, models.py:165-168) and the stacked box encodings [K, C, box_len].
 constexpr int kHeadRows = 64;     // vertices per tile
@@ -918,7 +974,7 @@ constexpr int kHeadThreads = 256; // thread = (row = tid / 4, quarter = tid % 4)
 constexpr int kHeadH = 64;        // hidden width the kernel is built for (models.py:60-64 classaware_predictor)
 
 struct HeadsParams {
-  const float* hid;      // [m, htot] = relu(first layers), columns: cls hidden [H] then class c hidden [H] ...
+  const float* hid;      // [m, htot] = act(first layers), columns: cls hidden [H] then class c hidden [H] ...
   int64_t m;
   int htot, C, box;
   const float* wpack;    // [Wcls H*C | bcls C | per class: W2 H*H | b2 H | W3 H*box | b3 box], sections padded to 4 floats
@@ -926,8 +982,10 @@ struct HeadsParams {
   float* logits;         // [m, C]
   float* probs;          // [m, C] or null
   float* boxes;          // [m, C, box]
+  int act;               // PG_ACT_* of the hidden layers (kAnyAct; otherwise ReLU)
 };
 
+template <bool kAnyAct>
 __global__ void __launch_bounds__(kHeadThreads) predictor_heads_kernel(HeadsParams p) {
   constexpr int H = kHeadH, XS = H + 1;
   extern __shared__ __align__(16) float hsm[];
@@ -1002,7 +1060,7 @@ __global__ void __launch_bounds__(kHeadThreads) predictor_heads_kernel(HeadsPara
         }
       }
 #pragma unroll
-      for (int j = 0; j < 16; ++j) h2[r * XS + qd * 16 + j] = fmaxf(acc[j], 0.0f);
+      for (int j = 0; j < 16; ++j) h2[r * XS + qd * 16 + j] = layer_act<kAnyAct>(p.act, acc[j]);
       __syncthreads();
       // third layer (H -> box, linear): outputs qd, qd + 4, ... of row r
       if (r < rows) {
@@ -1027,6 +1085,7 @@ __global__ void copy_block_kernel(const float* __restrict__ src, int64_t rows, i
 
 struct PreparedPredictor {
   int D = 0, H = 0, C = 0, box = 0, htot = 0;
+  int act = PG_ACT_RELU;                   // of the hidden layers; the logits and box layers are linear
   bool fused = false;
   // fused route: the concatenated first layers on the tensor cores, then predictor_heads_kernel
   Temp wcat, bcat, wpack;                  // [D, htot] concatenated first layers, [htot], head weights
@@ -1040,7 +1099,8 @@ struct PreparedPredictor {
 
 // dims = {D, H, C, box_len}; layers = cls fc0, cls fc1, then per class c: fc0, fc1, fc2
 int prepare_predictor(PreparedPredictor& P, const float* const* weights, const float* const* biases,
-                      const int32_t* dims, int num_layers, bool want_tc, cudaStream_t s) {
+                      const int32_t* dims, int num_layers, int act, bool want_tc, cudaStream_t s) {
+  P.act = act;
   P.D = dims[0];
   P.H = dims[1];
   P.C = dims[2];
@@ -1117,7 +1177,7 @@ extern "C" int pg_fully_connected(const float* x, int64_t m, int32_t k, const fl
                                   int32_t act, const float* residual, float* out, int32_t precision, void* stream) {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   PG_REQUIRE(m >= 0 && k >= 1 && n >= 1, "pg_fully_connected: bad sizes m=%lld k=%d n=%d", (long long)m, k, n);
-  PG_REQUIRE(act == 0 || act == 1, "pg_fully_connected: act must be 0 (linear) or 1 (ReLU)");
+  PG_REQUIRE(act >= 0 && act < PG_ACT_COUNT, "pg_fully_connected: unknown activation %d", act);
   if (m == 0) return PG_OK;
   PG_REQUIRE(x && w && bias && out, "pg_fully_connected: null argument");
   PG_REQUIRE(precision == 0 || precision == 1, "pg_fully_connected: unknown precision %d", precision);
@@ -1140,10 +1200,12 @@ extern "C" int pg_edge_mlp_max(int32_t mode, const float* features, int32_t num_
   PG_REQUIRE(mode == PG_EDGE_GNN || dst_index != nullptr || num_edges == 0,
              "pg_edge_mlp_max: POOL mode needs keypoint indices");
   const bool trusted = (precision & PG_FLAG_TRUSTED_INDICES) != 0;
+  const int act = activation_of(precision);
+  PG_REQUIRE(act >= 0, "pg_edge_mlp_max: unknown activation");
   precision &= PG_PRECISION_MASK;
   PG_REQUIRE(precision == 0 || precision == 1, "pg_edge_mlp_max: unknown precision %d", precision);
   PreparedEdge e;
-  if (int rc = prepare_edge(e, mode, num_feature_channels, weights_host, biases_host, dims_host, num_layers,
+  if (int rc = prepare_edge(e, mode, num_feature_channels, weights_host, biases_host, dims_host, num_layers, act,
                             precision == 1 && num_edges > 0 && pg_tc_available(), s))
     return rc;
   return apply_edge(e, features, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst, trusted, out, s);
@@ -1154,6 +1216,7 @@ extern "C" int pg_edge_mlp_max(int32_t mode, const float* features, int32_t num_
 // ---------------------------------------------------------------------------------------------------
 struct pg_layer {
   int kind = 0, num_layers = 0;
+  int act = PG_ACT_RELU;
   std::vector<int32_t> dims;
   std::vector<PreparedFc> fcs;          // PG_LAYER_MLP
   PreparedEdge edge;                    // PG_LAYER_EDGE_POOL / PG_LAYER_EDGE_GNN
@@ -1167,6 +1230,9 @@ extern "C" int pg_layer_create(int32_t kind, const float* const* weights_host, c
   PG_REQUIRE(out_layer != nullptr, "pg_layer_create: out_layer is null");
   *out_layer = nullptr;
   PG_REQUIRE(weights_host && biases_host && dims_host && num_layers >= 1 && num_layers <= 64, "pg_layer_create: bad layer tables");
+  const int act = activation_of(precision);
+  PG_REQUIRE(act >= 0, "pg_layer_create: unknown activation");
+  precision &= ~(PG_FLAG_ACTIVATION | PG_ACT_MASK);
   PG_REQUIRE(precision == 0 || precision == 1, "pg_layer_create: unknown precision %d", precision);
   PG_REQUIRE(kind == PG_LAYER_MLP || kind == PG_LAYER_EDGE_POOL || kind == PG_LAYER_EDGE_GNN || kind == PG_LAYER_PREDICTOR,
              "pg_layer_create: unknown kind %d", kind);
@@ -1174,6 +1240,7 @@ extern "C" int pg_layer_create(int32_t kind, const float* const* weights_host, c
   auto L = std::make_unique<pg_layer>();
   L->kind = kind;
   L->num_layers = num_layers;
+  L->act = act;
   const bool want_tc = precision == 1 && pg_tc_available();
   if (kind == PG_LAYER_MLP) {
     L->dims.assign(dims_host, dims_host + num_layers + 1);
@@ -1185,11 +1252,12 @@ extern "C" int pg_layer_create(int32_t kind, const float* const* weights_host, c
   } else if (kind == PG_LAYER_EDGE_POOL || kind == PG_LAYER_EDGE_GNN) {
     L->dims.assign(dims_host, dims_host + num_layers + 1);
     if (int rc = prepare_edge(L->edge, kind == PG_LAYER_EDGE_POOL ? PG_EDGE_POOL : PG_EDGE_GNN, dims_host[0] - 3,
-                              weights_host, biases_host, dims_host, num_layers, want_tc, s))
+                              weights_host, biases_host, dims_host, num_layers, act, want_tc, s))
       return rc;
   } else {
     L->dims.assign(dims_host, dims_host + 4);
-    if (int rc = prepare_predictor(L->pred, weights_host, biases_host, dims_host, num_layers, want_tc, s)) return rc;
+    if (int rc = prepare_predictor(L->pred, weights_host, biases_host, dims_host, num_layers, act, want_tc, s))
+      return rc;
   }
   *out_layer = L.release();
   return PG_OK;
@@ -1218,7 +1286,7 @@ extern "C" int pg_layer_mlp(const pg_layer* layer, const float* x, int64_t m, in
   for (int l = 0; l < L; ++l) {
     const bool last = l + 1 == L;
     float* dst = last ? out : bufs[l & 1].as<float>();
-    const int act = (last && last_linear) ? 0 : 1;
+    const int act = (last && last_linear) ? PG_ACT_NONE : layer->act;
     if (int rc = apply_fc(layer->fcs[l], cur, m, act, last ? residual : nullptr, dst, layer->dims[l + 1], s)) return rc;
     cur = dst;
   }
@@ -1252,7 +1320,7 @@ extern "C" int pg_layer_predictor(const pg_layer* layer, const float* x, int64_t
     Temp hid;
     PG_CUDA_OK(hid.alloc(sizeof(float) * m * P.htot, s));
     for (size_t g = 0; g < P.first.size(); ++g)
-      if (int rc = apply_fc(P.first[g], x, m, 1, nullptr, hid.as<float>() + P.col0[g], P.htot, s)) return rc;
+      if (int rc = apply_fc(P.first[g], x, m, P.act, nullptr, hid.as<float>() + P.col0[g], P.htot, s)) return rc;
     HeadsParams hp{};
     hp.hid = hid.as<float>();
     hp.m = m;
@@ -1264,13 +1332,16 @@ extern "C" int pg_layer_predictor(const pg_layer* layer, const float* x, int64_t
     hp.logits = logits;
     hp.probs = probs;
     hp.boxes = boxes;
-    static bool attr_done = false;
-    if (!attr_done) {
-      PG_CUDA_OK(cudaFuncSetAttribute(predictor_heads_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-      attr_done = true;
+    hp.act = P.act;
+    const bool any_act = P.act != PG_ACT_RELU;
+    void (*kernel)(HeadsParams) = any_act ? predictor_heads_kernel<true> : predictor_heads_kernel<false>;
+    static bool attr_done[2] = {false, false};
+    if (!attr_done[any_act]) {
+      PG_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+      attr_done[any_act] = true;
     }
     const int blocks = int(std::min<int64_t>(ceil_div(m, kHeadRows), num_sms()));
-    predictor_heads_kernel<<<blocks, kHeadThreads, P.smem, s>>>(hp);
+    kernel<<<blocks, kHeadThreads, P.smem, s>>>(hp);
     PG_LAUNCH_CHECK();
     return PG_OK;
   }
@@ -1279,14 +1350,14 @@ extern "C" int pg_layer_predictor(const pg_layer* layer, const float* x, int64_t
   PG_CUDA_OK(h1.alloc(sizeof(float) * m * P.H, s));
   PG_CUDA_OK(h2.alloc(sizeof(float) * m * P.H, s));
   PG_CUDA_OK(tmp.alloc(sizeof(float) * m * P.box, s));
-  if (int rc = apply_fc(P.layers[0], x, m, 1, nullptr, h1.as<float>(), P.H, s)) return rc;
+  if (int rc = apply_fc(P.layers[0], x, m, P.act, nullptr, h1.as<float>(), P.H, s)) return rc;
   if (int rc = apply_fc(P.layers[1], h1.as<float>(), m, 0, nullptr, logits, P.C, s)) return rc;
   if (probs != nullptr)
     if (int rc = pg_softmax_rows(logits, m, P.C, probs, stream)) return rc;
   for (int c = 0; c < P.C; ++c) {
     const int l = 2 + 3 * c;
-    if (int rc = apply_fc(P.layers[l], x, m, 1, nullptr, h1.as<float>(), P.H, s)) return rc;
-    if (int rc = apply_fc(P.layers[l + 1], h1.as<float>(), m, 1, nullptr, h2.as<float>(), P.H, s)) return rc;
+    if (int rc = apply_fc(P.layers[l], x, m, P.act, nullptr, h1.as<float>(), P.H, s)) return rc;
+    if (int rc = apply_fc(P.layers[l + 1], h1.as<float>(), m, P.act, nullptr, h2.as<float>(), P.H, s)) return rc;
     if (int rc = apply_fc(P.layers[l + 2], h2.as<float>(), m, 0, nullptr, tmp.as<float>(), P.box, s)) return rc;
     copy_block_kernel<<<64, 256, 0, s>>>(tmp.as<float>(), m, P.box, P.C * P.box, boxes + c * P.box);
     PG_LAUNCH_CHECK();

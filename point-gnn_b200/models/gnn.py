@@ -30,7 +30,7 @@ class VariableStore(object):
 
     def __init__(self, variables=None, device=None):
         self.vars = {}
-        self.prepared = {}      # (kind, first variable, depth, precision) -> _lib.PreparedLayer (weights packed once)
+        self.prepared = {}      # (kind, first variable, depth, precision, activation) -> _lib.PreparedLayer
         if variables:
             self.load(variables, device)
 
@@ -107,14 +107,14 @@ def _take_mlp(num_layers):
     return names, ws, bs
 
 
-def _prepared(kind, names, weights, biases, dims):
-    """The prepared (weights packed once) layer for these variables, cached on the bound VariableStore - the
-    stand-in for TF creating / restoring its variables once and only computing at sess.run."""
+def _prepared(kind, names, weights, biases, dims, activation):
+    """The prepared (weights packed once) layer for these variables and this activation, cached on the bound
+    VariableStore - the stand-in for TF creating / restoring its variables once and only computing at sess.run."""
     store = _ctx.store
-    key = (kind, names[0], len(names), get_precision())
+    key = (kind, names[0], len(names), get_precision(), activation)
     layer = store.prepared.get(key)
     if layer is None:
-        layer = _lib.PreparedLayer(kind, weights, biases, dims, get_precision())
+        layer = _lib.PreparedLayer(kind, weights, biases, dims, get_precision(), activation)
         store.prepared[key] = layer
     return layer
 
@@ -127,19 +127,21 @@ def _mlp_dims(ws, bs, widths):
     return dims
 
 
-# the reference's tables (gnn.py:17-32); only the entries its shipped configs use are executable
+# the reference's tables (gnn.py:17-32).  Every activation runs in the fused kernels (the name -> PG_ACT_* code
+# table of the whole package); of the normalizations only 'NONE' is built
 normalization_fn_dict = {'fused_BN_center': 'fused_BN_center', 'BN': 'BN', 'BN_center': 'BN_center',
                          'IN': 'IN', 'NONE': None}
-activation_fn_dict = {'ReLU': 'ReLU', 'ReLU6': 'ReLU6', 'LeakyReLU': 'LeakyReLU', 'ELU': 'ELU',
-                      'NONE': None, 'Sigmoid': 'Sigmoid', 'Tanh': 'Tanh'}
+activation_fn_dict = {'ReLU': _lib.PG_ACT_RELU, 'ReLU6': _lib.PG_ACT_RELU6, 'LeakyReLU': _lib.PG_ACT_LEAKY_RELU,
+                      'ELU': _lib.PG_ACT_ELU, 'NONE': _lib.PG_ACT_NONE, 'Sigmoid': _lib.PG_ACT_SIGMOID,
+                      'Tanh': _lib.PG_ACT_TANH}
 
 
 def _check_types(normalization_type, activation_type):
+    """-> the PG_ACT_* code of activation_type; an unknown name raises KeyError, as the reference's lookup does."""
     if normalization_fn_dict[normalization_type] is not None:
         raise NotImplementedError('normalization %r: every shipped config uses "NONE" '
                                   '(SURVEY fact 3); batch/instance norm are not built' % normalization_type)
-    if activation_fn_dict[activation_type] not in ('ReLU',):
-        raise NotImplementedError('activation %r: every shipped config uses "ReLU"' % activation_type)
+    return activation_fn_dict[activation_type]
 
 
 def multi_layer_fc_fn(sv, mask=None, Ks=(64, 32, 64), num_classes=4, is_logits=False, num_layer=4,
@@ -147,9 +149,9 @@ def multi_layer_fc_fn(sv, mask=None, Ks=(64, 32, 64), num_classes=4, is_logits=F
     """gnn.py:34-84."""
     assert len(sv.shape) == 2
     assert len(Ks) == num_layer - 1
-    _check_types(normalization_type, activation_type)
+    act = _check_types(normalization_type, activation_type)
     names, ws, bs = _take_mlp(num_layer)
-    layer = _prepared(_lib.PG_LAYER_MLP, names, ws, bs, _mlp_dims(ws, bs, list(Ks) + [num_classes]))
+    layer = _prepared(_lib.PG_LAYER_MLP, names, ws, bs, _mlp_dims(ws, bs, list(Ks) + [num_classes]), act)
     features = layer.mlp(sv.contiguous(), last_linear=is_logits)
     if mask is not None:
         features = features * mask
@@ -161,9 +163,9 @@ def multi_layer_neural_network_fn(features, Ks=(64, 32, 64), is_logits=False,
                                   residual=None):
     """gnn.py:86-104.  ``residual`` (extension): added to the last layer's output in-kernel."""
     assert len(features.shape) == 2
-    _check_types(normalization_type, activation_type)
+    act = _check_types(normalization_type, activation_type)
     names, ws, bs = _take_mlp(len(Ks))
-    layer = _prepared(_lib.PG_LAYER_MLP, names, ws, bs, _mlp_dims(ws, bs, Ks))
+    layer = _prepared(_lib.PG_LAYER_MLP, names, ws, bs, _mlp_dims(ws, bs, Ks), act)
     return layer.mlp(features.contiguous(), last_linear=is_logits, residual=residual)
 
 
@@ -219,7 +221,8 @@ class ClassAwarePredictor(object):
     def apply_regular(self, features, num_classes, box_encoding_len,
                       normalization_type='fused_BN_center', activation_type='ReLU'):
         h = self._head_width()
-        if h is not None and normalization_type == 'NONE' and activation_type == 'ReLU':
+        if h is not None and normalization_type == 'NONE':
+            act = _check_types(normalization_type, activation_type)
             # all heads in two launches per column group: the C + 1 first layers as ONE concatenated GEMM, then
             # one kernel for every remaining (tiny) layer, the softmax and the [K, C, box] stacking
             names, ws, bs = [], [], []
@@ -237,7 +240,7 @@ class ClassAwarePredictor(object):
             for class_idx in range(num_classes):
                 w0, w1, w2 = ws[2 + 3 * class_idx:5 + 3 * class_idx]
                 assert tuple(w0.shape) == (d, h) and tuple(w1.shape) == (h, h) and tuple(w2.shape) == (h, box_encoding_len)
-            layer = _prepared(_lib.PG_LAYER_PREDICTOR, names, ws, bs, [d, h, num_classes, box_encoding_len])
+            layer = _prepared(_lib.PG_LAYER_PREDICTOR, names, ws, bs, [d, h, num_classes, box_encoding_len], act)
             logits, box_encodings, probs = layer.predictor(features.contiguous())
             logits._pg_probs = (probs, logits._version)      # models.postprocess returns these (softmax fused)
             return logits, box_encodings
@@ -267,10 +270,10 @@ class PointSetPooling(object):
         self._aggregation_fn = aggregation_fn
         self._output_fn = output_fn
 
-    def _fusable(self, normalization_type, activation_type):
+    def _fusable(self, normalization_type):
         return (self._point_feature_fn is multi_layer_neural_network_fn
                 and self._aggregation_fn is graph_scatter_max_fn
-                and normalization_type == 'NONE' and activation_type == 'ReLU')
+                and normalization_type == 'NONE')
 
     def apply_regular(self, point_features, point_coordinates, keypoint_indices, set_indices,
                       point_MLP_depth_list=None, point_MLP_normalization_type='fused_BN_center',
@@ -279,11 +282,12 @@ class PointSetPooling(object):
         num_keypoints = keypoint_indices.shape[0]
         src, dst = set_indices[:, 0], set_indices[:, 1]
         with variable_scope('extract_vertex_features'):
-            if self._fusable(point_MLP_normalization_type, point_MLP_activation_type):
+            if self._fusable(point_MLP_normalization_type):
+                act = _check_types(point_MLP_normalization_type, point_MLP_activation_type)
                 names, ws, bs = _take_mlp(len(point_MLP_depth_list))
                 dims = [point_features.shape[1] + 3] + [int(k) for k in point_MLP_depth_list]
                 assert _mlp_dims(ws, bs, point_MLP_depth_list) == dims, 'point MLP input width mismatch'
-                layer = _prepared(_lib.PG_LAYER_EDGE_POOL, names, ws, bs, dims)
+                layer = _prepared(_lib.PG_LAYER_EDGE_POOL, names, ws, bs, dims, act)
                 set_features = layer.edge_mlp_max(
                     point_features.contiguous(), point_coordinates.contiguous(), point_coordinates.contiguous(),
                     _i32(keypoint_indices.reshape(-1)), _i32(src), _i32(dst), num_keypoints,
@@ -316,10 +320,10 @@ class GraphNetAutoCenter(object):
         self._update_fn = update_fn
         self._auto_offset_fn = auto_offset_fn
 
-    def _fusable(self, normalization_type, activation_type):
+    def _fusable(self, normalization_type):
         return (self._edge_feature_fn is multi_layer_neural_network_fn
                 and self._aggregation_fn is graph_scatter_max_fn
-                and normalization_type == 'NONE' and activation_type == 'ReLU')
+                and normalization_type == 'NONE')
 
     def apply_regular(self, input_vertex_features, input_vertex_coordinates, NOT_USED, edges,
                       edge_MLP_depth_list=None, edge_MLP_normalization_type='fused_BN_center',
@@ -346,11 +350,12 @@ class GraphNetAutoCenter(object):
                     activation_type=auto_offset_MLP_feature_activation_type)
                 dest_coordinates = (source_coordinates + offset).contiguous()
         with variable_scope('extract_vertex_features'):
-            if self._fusable(edge_MLP_normalization_type, edge_MLP_activation_type):
+            if self._fusable(edge_MLP_normalization_type):
+                act = _check_types(edge_MLP_normalization_type, edge_MLP_activation_type)
                 names, ws, bs = _take_mlp(len(edge_MLP_depth_list))
                 dims = [input_vertex_features.shape[1] + 3] + [int(k) for k in edge_MLP_depth_list]
                 assert _mlp_dims(ws, bs, edge_MLP_depth_list) == dims, 'edge MLP input width mismatch'
-                layer = _prepared(_lib.PG_LAYER_EDGE_GNN, names, ws, bs, dims)
+                layer = _prepared(_lib.PG_LAYER_EDGE_GNN, names, ws, bs, dims, act)
                 aggregated_edge_features = layer.edge_mlp_max(
                     input_vertex_features.contiguous(), source_coordinates, dest_coordinates, None, _i32(src),
                     _i32(dst), num_vertices, trusted=_ctx.trusted_edges)
