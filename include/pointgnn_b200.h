@@ -466,6 +466,28 @@ PG_API int pg_nms_boxes_3d(const int32_t* class_labels, const float* boxes, cons
                     float* out_box, float* out_score, int32_t* out_index, int64_t capacity,
                     int32_t* out_det_frame_ptr, int64_t* out_sizes_host, void* stream);
 
+/* KITTI result rows of the kept boxes (/root/reference/run.py:361-408 with occlusion, run.py:88-100; the box tests of
+ * /root/reference/dataset/kitti_dataset.py:85-162 and the projection of :1036-1052), every frame of a batch at once.
+ * Inputs, as pg_postprocess returns them: boxes [D,7] / labels [D] / scores [D] with det_frame_ptr [num_frames+1];
+ * the last-level vertex coordinates xyz [K,3] with cand_index [B] (flat v * num_classes + c) and cand_frame_ptr
+ * [num_frames+1] (used only with PG_KITTI_ROWS_RESCORE); cam_to_image [num_frames,3,4] float64.
+ * Per box: the 8 corners (nms.py:9-27) projected with the frame's cam_to_image, the min / max of the projections
+ * clipped to the reference's fixed 1242 x 375 (run.py:385-388); the box is dropped when its truncation rate
+ * 1 - clipped area / area exceeds 0.4.  flags PG_KITTI_ROWS_RESCORE: score * (1 + occlusion) over the frame's
+ * candidates strictly inside the box (occlusion = 0 when none is).  Arithmetic: NumPy's dtype chain of that code,
+ * documented in csrc/pg_kitti.cu.
+ * Output: out_rows [D, PG_KITTI_ROW_FIELDS] float64, the surviving rows compacted frame by frame in detection order:
+ *   detection index, frame, label, x, y, z, l, h, w, yaw (the float32 values widened), clipped xmin, ymin, xmax,
+ *   ymax, score, number of candidates inside the box (0 without rescoring);
+ * out_row_frame_ptr [num_frames+1]; out_num_rows_host = number of rows.  PG_ERR_INVALID_ARGUMENT when a surviving
+ * box has l <= 0 (run.py:395's assert).  One host round trip (the row count), none when D = 0. */
+#define PG_KITTI_ROWS_RESCORE 1
+#define PG_KITTI_ROW_FIELDS 16
+PG_API int pg_kitti_rows(const float* boxes, const int32_t* labels, const float* scores, const int32_t* det_frame_ptr,
+                  int32_t num_frames, int64_t num_dets, const float* xyz, const int32_t* cand_index,
+                  const int32_t* cand_frame_ptr, int32_t num_classes, const double* cam_to_image, int32_t flags,
+                  double* out_rows, int32_t* out_row_frame_ptr, int64_t* out_num_rows_host, void* stream);
+
 /* ------------------------------------------------------------------------ *
  * KITTI object evaluation (reference kitti_native_evaluation/src/evaluate_object_3d_offline.cpp)
  * ------------------------------------------------------------------------ */

@@ -80,6 +80,9 @@ SIGNATURES = {
     'pg_nms_boxes_3d': (ctypes.c_int, [c_i32p, c_f32p, c_f32p, c_i32p, c_i32, c_i64, ctypes.c_double,
                                        ctypes.c_double, c_i32, c_i64, c_i32p, c_f32p, c_f32p, c_i32p, c_i64, c_i32p,
                                        ctypes.POINTER(c_i64), ctypes.c_void_p]),
+    'pg_kitti_rows': (ctypes.c_int, [c_f32p, c_i32p, c_f32p, c_i32p, c_i32, c_i64, c_f32p, c_i32p, c_i32p, c_i32,
+                                     ctypes.c_void_p, c_i32, ctypes.c_void_p, c_i32p, ctypes.POINTER(c_i64),
+                                     ctypes.c_void_p]),
     'pg_kitti_eval': (ctypes.c_int, [ctypes.c_void_p, c_i32p, ctypes.c_void_p, c_i32p, ctypes.POINTER(c_i64),
                                      ctypes.POINTER(c_i64), c_i32, c_i32, ctypes.POINTER(ctypes.c_double),
                                      ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double),
@@ -643,6 +646,32 @@ def nms_boxes_3d(class_labels, boxes, scores, frame_ptr, overlapped_thres, merge
                                _stream()))
     d = int(sizes[0])
     return label[:d], box[:d], score[:d], index[:d], det_fp
+
+
+PG_KITTI_ROWS_RESCORE = 1
+KITTI_ROW_FIELDS = 16
+
+
+def kitti_rows(label, box, score, det_frame_ptr, xyz, cand_index, cand_frame_ptr, num_classes, cam_to_image, rescore):
+    """pg_kitti_rows.  The detections and candidates as ``postprocess`` returns them, xyz [K,3] the last-level
+    vertices, cam_to_image [F,3,4] CUDA float64.  -> (rows [R, KITTI_ROW_FIELDS] float64, row_frame_ptr [F+1] int32),
+    the row layout of include/pointgnn_b200.h."""
+    num_frames = det_frame_ptr.numel() - 1
+    d = box.shape[0]
+    dev = box.device
+    if tuple(cam_to_image.shape) != (num_frames, 3, 4):
+        raise ValueError('cam_to_image must be [%d, 3, 4], got %s' % (num_frames, tuple(cam_to_image.shape)))
+    rows = torch.empty((max(d, 1), KITTI_ROW_FIELDS), dtype=torch.float64, device=dev)
+    row_fp = torch.empty(num_frames + 1, dtype=torch.int32, device=dev)
+    n = c_i64(0)
+    _check(load().pg_kitti_rows(
+        _ptr(box, torch.float32, 'box'), _ptr(label, torch.int32, 'label'), _ptr(score, torch.float32, 'score'),
+        _ptr(det_frame_ptr, torch.int32, 'det_frame_ptr'), num_frames, d, _ptr(xyz, torch.float32, 'xyz'),
+        _ptr(cand_index, torch.int32, 'cand_index'), _ptr(cand_frame_ptr, torch.int32, 'cand_frame_ptr'),
+        int(num_classes), _ptr(cam_to_image, torch.float64, 'cam_to_image'),
+        PG_KITTI_ROWS_RESCORE if rescore else 0, _ptr(rows, torch.float64, 'rows'),
+        _ptr(row_fp, torch.int32, 'row_frame_ptr'), ctypes.byref(n), _stream()))
+    return rows[:n.value], row_fp
 
 
 # ---------------------------------------------------------------------------------------------

@@ -5,11 +5,13 @@
   ``get_filename``, ``get_calib`` (kitti_dataset.py:483-522), ``get_image`` (:691-701), ``get_velo_points``
   (:587-609), ``get_cam_points_in_image_with_rgb`` (:666-689) -> GPU (``pg_cam_points_in_image``),
   ``cam_points_to_image`` (:1036-1052), ``box3d_to_normals`` (:923-946), ``sel_xyz_in_box3d`` (:969-988).
-  The last three act on 8 box corners / a few hundred candidate vertices per detection; they stay NumPy as
-  in the reference.  Labels, augmentation, statistics and visualisation are training / tooling code: not built.
+  The last three are the NumPy forms, as in the reference, that ``run.kitti_labels`` uses; ``run.py`` itself
+  runs them for every detection of a batch on the GPU (``models.postprocess.kitti_rows``, ``pg_kitti_rows``).
+  ``get_image_size`` reads an image's size from its PNG header, for input features without colour.
+  Labels, augmentation, statistics and visualisation are training / tooling code: not built.
 * ``Points`` - the reference's namedtuple (kitti_dataset.py:14).
 * ``cam_points_in_image_batch`` - several frames in one GPU call, results staying on the device (what the
-  batched ``run.py`` twin and the end-to-end bench use).
+  batched ``run.py`` and the end-to-end bench use).
 """
 import os
 from collections import namedtuple
@@ -157,6 +159,17 @@ class KittiDataset(object):
     def get_image(self, frame_idx):
         import cv2
         return cv2.imread(join(self._image_dir, self._file_list[frame_idx]) + '.png')
+
+    def get_image_size(self, frame_idx):
+        """(height, width) of the frame's PNG, as ``get_image(frame_idx).shape[:2]``, read from the IHDR chunk that
+        opens every PNG file instead of decoding the image."""
+        path = join(self._image_dir, self._file_list[frame_idx]) + '.png'
+        with open(path, 'rb') as f:
+            head = f.read(24)
+        # 8-byte signature, then the IHDR chunk: length (4), type (4), width (4), height (4), big-endian
+        if len(head) < 24 or head[:8] != b'\x89PNG\r\n\x1a\n' or head[12:16] != b'IHDR':
+            raise ValueError('%s is not a PNG file' % path)
+        return int.from_bytes(head[20:24], 'big'), int.from_bytes(head[16:20], 'big')
 
     def get_velo_data(self, frame_idx):
         """The raw [M, 4] float32 content of the frame's .bin file (x, y, z, reflectance)."""

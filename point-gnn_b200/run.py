@@ -1,7 +1,7 @@
 """Inference pipeline for Point-GNN on KITTI - the eager twin of the reference's ``run.py``.
 
-Same command line, same per-frame flow, same stage timers and the same KITTI-format output files as
-/root/reference/run.py; the TensorFlow-1 pieces are replaced by this package:
+Same command line, same stage timers and the same KITTI-format output files as /root/reference/run.py; the
+TensorFlow-1 pieces are replaced by this package:
 
   reference run.py      here
   :104-150  placeholders + model.predict graph build   -> ``model = get_model(...)(...)``, nothing to build
@@ -10,18 +10,42 @@ Same command line, same per-frame flow, same stage timers and the same KITTI-for
   :219-222  graph_generate_fn(...)                     -> GPU graph build (models.graph_gen, pg_multi_level_graph)
   :252-260  sess.run(fetches, feed_dict)               -> ``model.predict`` / ``model.postprocess`` (CUDA kernels)
   :265-325  box decoding + nms.nms_boxes_3d_*          -> models.postprocess.detect (pg_postprocess), one call
-  :361-433  KITTI label conversion + file writer       -> ``kitti_labels`` / ``write_kitti_file`` below (NumPy, as there)
+  :361-408  KITTI label conversion                     -> models.postprocess.kitti_rows (pg_kitti_rows), one call;
+                                                          ``kitti_labels`` below is the NumPy form, kept as the reference
+  :421-433  file writer                                -> ``write_kitti_file`` below
 
 The visualisation levels (``-l 1|2``, Open3D / OpenCV windows, run.py:151-190, 327-360, 434-473) are not part of
-the detection path and are not built.  Frames keep their data on the GPU from the velodyne bytes to the kept
-boxes; the only host work per frame is file I/O and the per-detection conversion to KITTI text.
+the detection path and are not built.
+
+Batches.  ``--batch_size N`` (default 1) groups consecutive frames of the split; the last batch may be shorter.
+Every stage takes the whole batch in one call (indices are global, frames are independent), so the files do not
+depend on N.  While the GPU runs batch i, a worker thread reads batch i+2's files (velodyne .bin, calibration, and
+the image - only its size, from the PNG header, when the input features use no colour), and the input stage and
+graph build of batch i+1 are issued on the ``utils.prefetch.GraphPrefetcher`` side stream.  Per batch the host then
+waits for the forward pass, runs ``detect`` and ``kitti_rows`` and reads the rows back once; what is left is the text
+formatting and the file writes.
+
+Timers (run.py's names, per-frame means: the sum over batches divided by the number of frames).  Stages of different
+batches overlap, so each timer is the host time spent in its step, and a GPU stage that overlaps another one is
+charged to the step whose wait it ends:
+  fetch input    waiting for the worker thread's files of the batch and issuing its input stage (one size read-back
+                 on the side stream)
+  gen graph      issuing the batch's graph build on the side stream (its one size read-back included)
+  gnn inference  issuing the forward pass and then waiting for it, after the next batch's input and graph have been
+                 issued
+  decode box     ``detect``: box decoding and NMS, ending in its read-back of the number of kept boxes
+  nms            ``kitti_rows``, the one read-back of the rows and their conversion to KITTI tuples (run.py's label
+                 conversion, which its ``nms`` timer covers)
+  total          wall time of the whole loop, file writes included, divided by the number of frames
 
     python -m pointgnn_b200.run CHECKPOINT_PATH [--test] [--no-box-merge] [--no-box-score]
            [--dataset_root_dir DIR] [--dataset_split_file FILE] [--output_dir DIR] [--precision fp32|bf16x3]
+           [--batch_size N]
 """
 import argparse
 import os
 import time
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
@@ -35,6 +59,7 @@ from pointgnn_b200.models.box_encoding import get_box_decoding_fn, get_encoding_
 from pointgnn_b200.models.graph_gen import get_graph_generate_fn
 from pointgnn_b200.models.models import get_model
 from pointgnn_b200.util.config_util import load_config
+from pointgnn_b200.utils.prefetch import GraphPrefetcher
 
 
 def occlusion(label, xyz):
@@ -101,6 +126,24 @@ def kitti_labels(class_labels, detection_boxes_3d, box_probs, candidate_xyz, cal
     return pred_labels
 
 
+def kitti_labels_from_rows(rows, num_frames, label_method):
+    """The rows of ``postprocess.kitti_rows`` (read back as a NumPy [R, 16] float64 array) -> one list per frame of the
+    tuples ``kitti_labels`` returns, with the same field types, so that ``write_kitti_file`` prints the same text:
+    h, w, l, x, y, z, yaw as float32, the clipped box as float64, the score as float64 when rescoring found candidates
+    inside the box and as the float32 NMS score otherwise (run.py:406 multiplies by the Python int 1 then)."""
+    all_class_name = postprocess.CLASS_NAMES[label_method]
+    per_frame = [[] for _ in range(num_frames)]
+    box = rows[:, 3:10].astype(np.float32)          # exact: the kernel widened these float32 values
+    for r in range(rows.shape[0]):
+        row = rows[r]
+        x3d, y3d, z3d, l, h, w, yaw = box[r]
+        clip_xmin, clip_ymin, clip_xmax, clip_ymax = (np.float64(v) for v in row[10:14])
+        score = np.float64(row[14]) if row[15] > 0 else np.float32(row[14])
+        per_frame[int(row[1])].append((all_class_name[int(row[2])], -1, -1, 0, clip_xmin, clip_ymin, clip_xmax,
+                                       clip_ymax, h, w, l, x3d, y3d, z3d, yaw, score))
+    return per_frame
+
+
 def write_kitti_file(filename, pred_labels):
     """run.py:421-429: one line per detection, fields separated (and followed) by a blank, one empty line at the end."""
     os.makedirs(os.path.dirname(filename), exist_ok=True)
@@ -129,7 +172,11 @@ def main(argv=None):
                         help='Path to save the detection results. Default="CHECKPOINT_PATH/eval/"')
     parser.add_argument('--precision', type=str, default=None, choices=['fp32', 'bf16x3'],
                         help='Arithmetic of the dense layers (default: bf16x3 on sm_90, fp32-class accuracy)')
+    parser.add_argument('--batch_size', type=int, default=1,
+                        help='Frames per forward pass (consecutive frames of the split; default 1)')
     args = parser.parse_args(argv)
+    if args.batch_size < 1:
+        parser.error('--batch_size must be >= 1, got %d' % args.batch_size)
     if args.level != 0:
         raise NotImplementedError('visualisation levels 1 / 2 (Open3D windows) are not built')
     IS_TEST = args.test
@@ -179,57 +226,96 @@ def main(argv=None):
     device = torch.device('cuda', torch.cuda.current_device())
     # running network =========================================================
     time_dict = {}
-    for frame_idx in range(0, NUM_TEST_SAMPLE):
+
+    def charge(key, seconds):
+        time_dict[key] = time_dict.get(key, 0) + seconds
+
+    want_rgb = config['input_features'] in ('irgb', '0rgb')
+    pad_attr = not want_rgb and config['input_features'] in ('0000', 'i000')
+    last_layer_graph_level = config['model_kwargs']['layer_configs'][-1]['graph_level']
+    batches = [list(range(first, min(first + args.batch_size, NUM_TEST_SAMPLE)))
+               for first in range(0, NUM_TEST_SAMPLE, args.batch_size)]
+
+    def read_files(frames):
+        """Host file work of one batch (worker thread): velodyne, calibration, image or only its size."""
+        velo, calib, size, image = [], [], [], []
+        for frame_idx in frames:
+            velo.append(dataset.get_velo_data(frame_idx))
+            calib.append(dataset.get_calib(frame_idx))
+            if want_rgb:
+                image.append(dataset.get_image(frame_idx))
+                size.append(image[-1].shape[:2])
+            else:
+                size.append(dataset.get_image_size(frame_idx))
+        return velo, calib, [(w, h) for h, w in size], image if want_rgb else None
+
+    reader = ThreadPoolExecutor(max_workers=1)
+    pending = {}
+
+    def start_reading(b):
+        if b < len(batches):
+            pending[b] = reader.submit(read_files, batches[b])
+
+    prefetcher = GraphPrefetcher(graph_generate_fn, config['runtime_graph_gen_kwargs'], device)
+
+    def issue(b):
+        """Input stage + graph build of batch b on the prefetcher's side stream -> (graph ticket, calibrations)."""
+        t0 = time.time()
+        velo, calib, size, image = pending.pop(b).result()
+        start_reading(b + 1)
+        with torch.cuda.stream(prefetcher.stream):
+            xyz, attr, frame_ptr = kitti_dataset.cam_points_in_image_batch(velo, calib, size, image, device=device)
+            if pad_attr:
+                attr = torch.cat([attr, torch.zeros((attr.shape[0], 3), device=device)], dim=1)
+            t1 = time.time()
+            # submitted from the side stream: the inputs were made there, so the build waits for nothing else
+            ticket = prefetcher.submit(xyz, attr, frame_ptr)
+        charge('fetch input', t1 - t0)
+        charge('gen graph', time.time() - t1)
+        return ticket, calib
+
+    try:
         start_time = time.time()
-        # provide input ======================================================
-        calib = dataset.get_calib(frame_idx)
-        image = dataset.get_image(frame_idx)
-        want_rgb = config['input_features'] in ('irgb', '0rgb')
-        xyz, attr, _ = kitti_dataset.cam_points_in_image_batch(
-            [dataset.get_velo_data(frame_idx)], [calib], [(image.shape[1], image.shape[0])],
-            [image] if want_rgb else None, device=device)
-        if not want_rgb and config['input_features'] in ('0000', 'i000'):
-            attr = torch.cat([attr, torch.zeros((attr.shape[0], 3), device=device)], dim=1)
-        torch.cuda.synchronize()
-        input_time = time.time()
-        time_dict['fetch input'] = time_dict.get('fetch input', 0) + input_time - start_time
-        (vertex_coord_list, keypoint_indices_list, edges_list) = graph_generate_fn(
-            xyz, **config['runtime_graph_gen_kwargs'])
-        torch.cuda.synchronize()
-        graph_time = time.time()
-        time_dict['gen graph'] = time_dict.get('gen graph', 0) + graph_time - input_time
-        input_v = input_features(config, attr)
-        last_layer_graph_level = config['model_kwargs']['layer_configs'][-1]['graph_level']
-        last_layer_points_xyz = vertex_coord_list[last_layer_graph_level + 1]
-        # run forwarding =====================================================
-        logits, pred_box = model.predict(input_v, vertex_coord_list, keypoint_indices_list, edges_list, is_training=True)
-        probs = model.postprocess(logits)
-        torch.cuda.synchronize()
-        gnn_time = time.time()
-        time_dict['gnn inference'] = time_dict.get('gnn inference', 0) + gnn_time - graph_time
-        # box decoding + nms ==================================================
-        det = postprocess.detect(probs, pred_box, last_layer_points_xyz, None, config['label_method'],
-                                 config['nms_overlapped_thres'], use_box_merge=USE_BOX_MERGE,
-                                 use_box_score=USE_BOX_SCORE, want_candidates=True)
-        class_labels = det['label'].cpu().numpy()
-        detection_boxes_3d = det['box'].cpu().numpy()
-        box_probs = det['score'].cpu().numpy()
-        cand_vertices = (det['cand_index'] // NUM_CLASSES).long()
-        candidate_xyz = last_layer_points_xyz[cand_vertices].cpu().numpy()
-        decode_time = time.time()
-        time_dict['decode box'] = time_dict.get('decode box', 0) + decode_time - gnn_time
-        pred_labels = []
-        if len(class_labels) > 0:
-            # convert to KITTI ================================================
-            pred_labels = kitti_labels(class_labels, detection_boxes_3d, box_probs, candidate_xyz, calib,
-                                       config['label_method'], USE_BOX_SCORE)
-        nms_time = time.time()
-        time_dict['nms'] = time_dict.get('nms', 0) + nms_time - decode_time
-        # output ===========================================================
-        filename = OUTPUT_DIR + '/data/' + dataset.get_filename(frame_idx) + '.txt'
-        write_kitti_file(filename, pred_labels)
-        total_time = time.time()
-        time_dict['total'] = time_dict.get('total', 0) + total_time - start_time
+        start_reading(0)
+        upcoming = issue(0) if batches else None
+        for b, frames in enumerate(batches):
+            ticket, calib = upcoming
+            t0 = time.time()
+            attr, vertex_coord_list, keypoint_indices_list, edges_list = prefetcher.collect(ticket)
+            input_v = input_features(config, attr)
+            last_layer_points_xyz = vertex_coord_list[last_layer_graph_level + 1]
+            # run forwarding =================================================
+            logits, pred_box = model.predict(input_v, vertex_coord_list, keypoint_indices_list, edges_list,
+                                             is_training=True)
+            probs = model.postprocess(logits)
+            gnn_issue = time.time() - t0
+            if b + 1 < len(batches):
+                upcoming = issue(b + 1)
+            t1 = time.time()
+            torch.cuda.current_stream().synchronize()
+            t2 = time.time()
+            charge('gnn inference', gnn_issue + t2 - t1)
+            # box decoding + nms =============================================
+            det = postprocess.detect(probs, pred_box, last_layer_points_xyz,
+                                     ticket.frame_ptrs[last_layer_graph_level + 1], config['label_method'],
+                                     config['nms_overlapped_thres'], use_box_merge=USE_BOX_MERGE,
+                                     use_box_score=USE_BOX_SCORE, want_candidates=USE_BOX_SCORE)
+            t3 = time.time()
+            charge('decode box', t3 - t2)
+            # convert to KITTI ===============================================
+            rows, _ = postprocess.kitti_rows(det, last_layer_points_xyz, np.stack([c['cam_to_image'] for c in calib]),
+                                             NUM_CLASSES, USE_BOX_SCORE)
+            pred_labels = kitti_labels_from_rows(rows.cpu().numpy(), len(frames), config['label_method'])
+            charge('nms', time.time() - t3)
+            # output =========================================================
+            for frame_idx, labels in zip(frames, pred_labels):
+                write_kitti_file(OUTPUT_DIR + '/data/' + dataset.get_filename(frame_idx) + '.txt', labels)
+            # the ticket's tensors were made on the side stream; they are released only now that batch b is done
+            del ticket
+        if batches:
+            charge('total', time.time() - start_time)
+    finally:
+        reader.shutdown(wait=True, cancel_futures=True)
     # time statics ============================================================
     for key in time_dict:
         print(key + ' time : ' + str(time_dict[key] / max(NUM_TEST_SAMPLE, 1)))
