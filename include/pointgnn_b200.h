@@ -488,6 +488,30 @@ PG_API int pg_kitti_rows(const float* boxes, const int32_t* labels, const float*
                   const int32_t* cand_frame_ptr, int32_t num_classes, const double* cam_to_image, int32_t flags,
                   double* out_rows, int32_t* out_row_frame_ptr, int64_t* out_num_rows_host, void* stream);
 
+/* LiDAR beam downsampling (the reference's data tool scripts/point_cloud_downsample.py:19-53), every frame of a batch
+ * at once.  velo [num_points, 4] float32 (x, y, z, reflectance: the velodyne .bin rows) with frame_ptr
+ * [num_frames+1].  Per point, cos = double(z) / double(float32 sqrt((x*x + y*y) + z*z)) (:23-25); points whose
+ * cosine is not finite (zero norm) are never kept and take no part in the clustering.
+ * Clustering (skipped when centers_in [num_frames, num_clusters] float64 is given): per frame, the exact optimum of
+ * the 1-D k-means on its finite cosines - the partition of the sorted values into num_clusters contiguous groups
+ * with the least total squared deviation, ties to the smallest split index - where the reference fits an unseeded
+ * scikit-learn KMeans (:26).  centers_out [num_frames, num_clusters] (ascending group means; repeated values when a
+ * frame has fewer distinct cosines than clusters; NaN for a frame without a finite cosine), inertia_out
+ * [num_frames] and group_sizes_out [num_frames, num_clusters] int32 (optional) are written only when clustering
+ * runs; with centers_in, centers_out (optional) receives a copy.
+ * Bands (:27-35): centers = [-1] + centres + [1]; every downsample_rate-th band i keeps the points with
+ * (c[i] + c[i+1]) / 2 < cos < (c[i+1] + c[i+2]) / 2 in float64.
+ * Output: out_velo [num_points, 4] capacity, the kept rows in their original order, bit for bit;
+ * out_frame_ptr [num_frames+1]; out_num_points_host = number of kept rows.
+ * PG_ERR_INVALID_ARGUMENT for num_clusters < 1, downsample_rate < 1, or when clustering a frame that has at least
+ * one but fewer than num_clusters finite cosines (the error message names the first such frame).
+ * Device memory: about 4 * num_clusters + 96 bytes per point when clustering.
+ * One host round trip (the kept count), none when num_points = 0. */
+PG_API int pg_beam_downsample(const float* velo, const int32_t* frame_ptr, int32_t num_frames, int64_t num_points,
+                       int32_t num_clusters, int32_t downsample_rate, const double* centers_in,
+                       double* centers_out, double* inertia_out, int32_t* group_sizes_out, float* out_velo,
+                       int32_t* out_frame_ptr, int64_t* out_num_points_host, void* stream);
+
 /* ------------------------------------------------------------------------ *
  * KITTI object evaluation (reference kitti_native_evaluation/src/evaluate_object_3d_offline.cpp)
  * ------------------------------------------------------------------------ */

@@ -83,6 +83,9 @@ SIGNATURES = {
     'pg_kitti_rows': (ctypes.c_int, [c_f32p, c_i32p, c_f32p, c_i32p, c_i32, c_i64, c_f32p, c_i32p, c_i32p, c_i32,
                                      ctypes.c_void_p, c_i32, ctypes.c_void_p, c_i32p, ctypes.POINTER(c_i64),
                                      ctypes.c_void_p]),
+    'pg_beam_downsample': (ctypes.c_int, [c_f32p, c_i32p, c_i32, c_i64, c_i32, c_i32, ctypes.c_void_p,
+                                          ctypes.c_void_p, ctypes.c_void_p, c_i32p, c_f32p, c_i32p,
+                                          ctypes.POINTER(c_i64), ctypes.c_void_p]),
     'pg_kitti_eval': (ctypes.c_int, [ctypes.c_void_p, c_i32p, ctypes.c_void_p, c_i32p, ctypes.POINTER(c_i64),
                                      ctypes.POINTER(c_i64), c_i32, c_i32, ctypes.POINTER(ctypes.c_double),
                                      ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double),
@@ -706,6 +709,52 @@ def cam_points_in_image(velo, frame_ptr, velo_to_cam, cam_to_image, image_sizes,
         _ptr(out_attr, torch.float32, 'out_attr'), channels, m, _ptr(out_fp, torch.int32, 'out_fp'), ctypes.byref(n),
         _stream()))
     return out_xyz[:n.value], out_attr[:n.value], out_fp
+
+
+# ---------------------------------------------------------------------------------------------
+# LiDAR beam downsampling
+# ---------------------------------------------------------------------------------------------
+class BeamDownsampleError(PointGNNError, ValueError):
+    """pg_beam_downsample rejected its arguments (a frame with fewer finite cosines than clusters, or a bad rate /
+    cluster count), as scikit-learn's KMeans raises ValueError."""
+
+
+def beam_downsample(velo, frame_ptr, num_clusters, downsample_rate, centers_in=None):
+    """pg_beam_downsample.  velo [M,4] CUDA float32, frame_ptr [F+1] CUDA int32; centers_in: None (exact 1-D k-means per
+    frame) or [F, num_clusters] CUDA float64.  -> dict(velo [R,4] float32 kept rows, frame_ptr [F+1] int32,
+    centers [F,K] float64, and without centers_in: inertia [F] float64, group_sizes [F,K] int32)."""
+    num_frames = frame_ptr.numel() - 1
+    k, rate = int(num_clusters), int(downsample_rate)
+    if k < 1 or rate < 1:
+        raise BeamDownsampleError(PG_ERR_INVALID_ARGUMENT, 'num_clusters and downsample_rate must be >= 1, got %d and %d'
+                                  % (k, rate))
+    if velo.dim() != 2 or velo.shape[1] != 4:
+        raise ValueError('velo must be [M, 4], got %s' % (tuple(velo.shape),))
+    m = velo.shape[0]
+    dev = velo.device
+    if centers_in is not None and tuple(centers_in.shape) != (num_frames, k):
+        raise ValueError('centers_in must be [%d, %d], got %s' % (num_frames, k, tuple(centers_in.shape)))
+    if centers_in is not None:   # the script sorts the centres it is given (point_cloud_downsample.py:27)
+        centers_in = torch.sort(centers_in, dim=1).values.contiguous()
+    centers =torch.empty((num_frames, k), dtype=torch.float64, device=dev)
+    inertia = torch.empty(num_frames, dtype=torch.float64, device=dev) if centers_in is None else None
+    sizes = torch.empty((num_frames, k), dtype=torch.int32, device=dev) if centers_in is None else None
+    out = torch.empty((max(m, 1), 4), dtype=torch.float32, device=dev)
+    out_fp = torch.empty(num_frames + 1, dtype=torch.int32, device=dev)
+    n = c_i64(0)
+    lib = load()
+    code = lib.pg_beam_downsample(
+        _ptr(velo, torch.float32, 'velo'), _ptr(frame_ptr, torch.int32, 'frame_ptr'), num_frames, m, k, rate,
+        _ptr(centers_in, torch.float64, 'centers_in'), _ptr(centers, torch.float64, 'centers'),
+        _ptr(inertia, torch.float64, 'inertia'), _ptr(sizes, torch.int32, 'group_sizes'),
+        _ptr(out, torch.float32, 'out'), _ptr(out_fp, torch.int32, 'out_frame_ptr'), ctypes.byref(n), _stream())
+    if code == PG_ERR_INVALID_ARGUMENT:
+        raise BeamDownsampleError(code, lib.pg_last_error().decode())
+    _check(code)
+    res = dict(velo=out[:n.value], frame_ptr=out_fp, centers=centers)
+    if centers_in is None:
+        res.update(inertia=inertia, group_sizes=sizes)
+    return res
 
 
 # ---------------------------------------------------------------------------------------------

@@ -10,6 +10,8 @@
   ``get_image_size`` reads an image's size from its PNG header, for input features without colour.
   Labels, augmentation, statistics and visualisation are training / tooling code: not built.
 * ``Points`` - the reference's namedtuple (kitti_dataset.py:14).
+* ``beam_downsample_batch`` - the beam downsampling of the reference's ``scripts/point_cloud_downsample.py`` on the GPU
+  (``pg_beam_downsample``), with an exact 1-D k-means in place of its scikit-learn ``KMeans``.
 * ``cam_points_in_image_batch`` - several frames in one GPU call, results staying on the device (what the
   batched ``run.py`` and the end-to-end bench use).
 """
@@ -105,6 +107,32 @@ def cam_points_in_image_batch(velo_list, calib_list, image_size_list, image_list
         images = torch.from_numpy(np.concatenate(flat)).to(device)
     return _lib.cam_points_in_image(velo, torch.from_numpy(fp).to(device), vtc, cti, np.asarray(image_size_list, np.int32),
                                     images, offsets)
+
+
+def beam_downsample_batch(velo, frame_ptr=None, downsample_rate=2, num_clusters=64, centers=None):
+    """The beam downsampling of scripts/point_cloud_downsample.py:19-53 on the GPU (``pg_beam_downsample``): keep every
+    ``downsample_rate``-th of ``num_clusters`` beam bands of each frame, the bands cut between the cluster centres
+    of the points' zenith cosines.  The centres come from the exact 1-D k-means of each frame (deterministic; its
+    inertia is never above a KMeans fit's), or from ``centers``.  Points with a zero norm are never kept.
+
+    * ``velo`` a CUDA float32 [M, 4] tensor (x, y, z, reflectance) with ``frame_ptr`` [F+1] CUDA int32, ``centers``
+      None or [F, K] CUDA float64 -> the dict of ``_lib.beam_downsample``: device tensors ``velo`` [R, 4] (kept rows,
+      original order), ``frame_ptr`` [F+1], ``centers`` [F, K], and without ``centers`` also ``inertia`` [F] and
+      ``group_sizes`` [F, K].
+    * ``velo`` one frame's NumPy [M, 4] float32 array (``frame_ptr`` None), ``centers`` None or [K] -> (kept rows
+      [R, 4] float32 array, centres [K] float64 array, inertia float or None).
+    Raises ValueError for a frame with at least one but fewer than ``num_clusters`` clusterable points."""
+    if frame_ptr is not None:
+        return _lib.beam_downsample(velo, frame_ptr, num_clusters, downsample_rate, centers_in=centers)
+    device = torch.device('cuda', torch.cuda.current_device())
+    arr = np.ascontiguousarray(velo, dtype=np.float32).reshape(-1, 4)
+    fp = torch.tensor([0, arr.shape[0]], dtype=torch.int32, device=device)
+    cin = None
+    if centers is not None:
+        cin = torch.from_numpy(np.asarray(centers, dtype=np.float64).reshape(1, -1)).to(device)
+    res = _lib.beam_downsample(torch.from_numpy(arr).to(device), fp, num_clusters, downsample_rate, centers_in=cin)
+    inertia = float(res['inertia'][0]) if 'inertia' in res else None
+    return res['velo'].cpu().numpy(), res['centers'][0].cpu().numpy(), inertia
 
 
 class KittiDataset(object):

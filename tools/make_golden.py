@@ -417,8 +417,101 @@ def kitti_eval_goldens():
         print(stdout)
 
 
+BEAM_SEEDS, BEAM_POINTS = (41, 42, 43), 6000          # small frames: the reference script end to end
+BEAM_FULL_SEEDS, BEAM_FULL_POINTS = (51, 52), 120000    # full-size frames: scikit-learn's inertia only
+
+
+def beam_downsample_goldens():
+    """tests/golden/beam_downsample.npz: the reference's OWN scripts/point_cloud_downsample.py, run unmodified through
+    runpy from a temporary directory laid out as its hard-coded ``../dataset/kitti/...`` paths, on a synthetic
+    training tree (oracle.kitti.write_synthetic_kitti) with a ``3DOP_splits/val.txt`` listing every frame.  Shims,
+    none of which touches the arithmetic the fixture pins:
+      * ``open3d`` is stubbed: the script imports it for its commented-out visualisation only;
+      * ``np.bool = bool``: the alias NumPy 2 removed (the script's mask dtype);
+      * ``sklearn.cluster.KMeans`` is wrapped: ``n_jobs`` (removed in scikit-learn 1.0) is dropped, and the fit
+        uses ``n_init=10`` (the default of the scikit-learn of the reference's era) and ``random_state=0`` so the
+        fixture can be regenerated; each fit's centres and inertia are recorded.
+    Stored: each frame's velodyne rows, scikit-learn's centres (its own order) and inertia, and the bytes the
+    script wrote.  Beside them, for two seeded full-size frames (oracle.beam_downsample.velodyne_frame, 120 000
+    points), the same KMeans fit's inertia on the cosines and the SHA-256 of the frame's bytes."""
+    import hashlib
+    import runpy
+    import shutil
+    import types
+    import sklearn.cluster
+    from oracle import beam_downsample as obd
+    from oracle import kitti as okitti
+    fits = []
+    real_kmeans = sklearn.cluster.KMeans
+
+    class _KMeans(object):
+        def __init__(self, n_clusters=8, n_jobs=None, **kwargs):
+            self._km = real_kmeans(n_clusters=n_clusters, n_init=10, random_state=0, **kwargs)
+
+        def fit(self, x):
+            self._km.fit(x)
+            self.cluster_centers_ = self._km.cluster_centers_
+            self.inertia_ = self._km.inertia_
+            fits.append((np.asarray(self.cluster_centers_, dtype=np.float64).reshape(-1), float(self.inertia_)))
+            return self
+
+    tmp = tempfile.mkdtemp()
+    saved = (os.getcwd(), list(sys.path), sys.modules.get('open3d'), getattr(np, 'bool', None))
+    try:
+        root = os.path.join(tmp, 'dataset', 'kitti')
+        names = okitti.write_synthetic_kitti(root, BEAM_SEEDS, num_points=BEAM_POINTS, test_split=False)
+        os.makedirs(os.path.join(root, '3DOP_splits'))
+        with open(os.path.join(root, '3DOP_splits', 'val.txt'), 'w') as f:
+            f.write(''.join(n + '\n' for n in names))
+        os.makedirs(os.path.join(tmp, 'scripts'))
+        os.chdir(os.path.join(tmp, 'scripts'))
+        sys.path.insert(0, reference_graph.REFERENCE_ROOT)
+        sys.modules['open3d'] = types.ModuleType('open3d')
+        np.bool = bool
+        sklearn.cluster.KMeans = _KMeans
+        runpy.run_path(os.path.join(reference_graph.REFERENCE_ROOT, 'scripts', 'point_cloud_downsample.py'),
+                       run_name='__main__')
+        out = {'names': np.array(names), 'downsample_rate': np.int64(2), 'num_clusters': np.int64(64)}
+        assert len(fits) == len(names)
+        for i, name in enumerate(names):
+            velo = np.fromfile(os.path.join(root, 'velodyne', 'training', 'velodyne', name + '.bin'), dtype=np.float32)
+            written = np.fromfile(os.path.join(root, 'velodyne', 'training_downsampled_2', 'velodyne', name + '.bin'),
+                                  dtype=np.uint8)
+            out['velo_%d' % i] = velo.reshape(-1, 4)
+            out['bin_%d' % i] = written
+            print('beam_downsample', name, 'points', len(velo) // 4, 'kept', len(written) // 16, 'inertia', fits[i][1])
+        out['sk_centers'] = np.stack([c for c, _ in fits])
+        out['sk_inertia'] = np.array([v for _, v in fits])
+        del fits[:]
+        sha, inertia = [], []
+        for seed in BEAM_FULL_SEEDS:
+            velo = obd.velodyne_frame(seed, BEAM_FULL_POINTS)
+            sha.append(hashlib.sha256(velo.tobytes()).hexdigest())
+            _KMeans(n_clusters=64, n_jobs=-1).fit(obd.cosines(velo[:, :3]).reshape(-1, 1))
+            inertia.append(fits[-1][1])
+            print('beam_downsample full-size seed', seed, 'inertia', inertia[-1])
+        out['full_seeds'] = np.array(BEAM_FULL_SEEDS, dtype=np.int64)
+        out['full_num_points'] = np.int64(BEAM_FULL_POINTS)
+        out['full_sha256'] = np.array(sha)
+        out['full_sk_inertia'] = np.array(inertia)
+        np.savez_compressed(os.path.join(GOLDEN, 'beam_downsample.npz'), **out)
+    finally:
+        os.chdir(saved[0])
+        sys.path[:] = saved[1]
+        if saved[2] is None:
+            sys.modules.pop('open3d', None)
+        else:
+            sys.modules['open3d'] = saved[2]
+        if saved[3] is None and hasattr(np, 'bool'):
+            del np.bool
+        sklearn.cluster.KMeans = real_kmeans
+        shutil.rmtree(tmp)
+
+
 if __name__ == '__main__':
     which = sys.argv[1] if len(sys.argv) > 1 else 'all'
+    if which in ('all', 'beam_downsample'):
+        beam_downsample_goldens()
     if which in ('all', 'graph_random'):
         graph_random_goldens()
     if which in ('all', 'graph_multiscale'):
