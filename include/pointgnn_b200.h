@@ -77,6 +77,49 @@ PG_API int pg_cam_points_in_image(const float* velo_points, const int32_t* frame
                            float* out_attr, int32_t attr_channels, int64_t capacity,
                            int32_t* out_frame_ptr, int64_t* out_num_points_host, void* stream);
 
+/*
+ * The two halves of pg_cam_points_in_image, for a caller that changes the camera-frame cloud in between (the voxel
+ * averaging below: get_cam_points, kitti_dataset.py:611-627, averages BEFORE the crop of :674-689).  They run the
+ * device functions of pg_cam_points_in_image, so a point gets the same coordinates and the same verdict either way.
+ *
+ * pg_velo_to_cam: velo_points_to_cam (:998-1006) alone.  out_xyz [M,3] = every point in the camera frame,
+ * out_attr [M,1] = its reflectance; order and frame_ptr unchanged.  Synchronises the stream.
+ *
+ * pg_cam_points_crop: the rest, from cam_xyz [N,3] fp32 camera-frame points with reflectance [N,1] and frame_ptr
+ * [num_frames+1] over them.  The remaining arguments, the outputs and the errors are pg_cam_points_in_image's.
+ */
+PG_API int pg_velo_to_cam(const float* velo_points, const int32_t* frame_ptr, int32_t num_frames, int64_t num_points,
+                          const float* velo_to_cam_host, float* out_xyz, float* out_attr, void* stream);
+PG_API int pg_cam_points_crop(const float* cam_xyz, const float* reflectance, const int32_t* frame_ptr,
+                              int32_t num_frames, int64_t num_points, const double* cam_to_image_host,
+                              const int32_t* image_size_host, const uint8_t* images,
+                              const int64_t* image_offset_host, float* out_xyz, float* out_attr,
+                              int32_t attr_channels, int64_t capacity, int32_t* out_frame_ptr,
+                              int64_t* out_num_points_host, void* stream);
+
+/*
+ * downsample_by_average_voxel (kitti_dataset.py:16-48), the `downsample_by_voxel_size` key of the configs (run.py:210-211),
+ * for a batch of frames: one output point per occupied voxel, its xyz and attributes the means of the voxel's points.
+ *   xyz [M,3] fp32, attr [M,attr_channels] fp32 (attr_channels in [0,4]; attr may be null when 0), frame_ptr
+ *   [num_frames+1] int32 over the M points; voxel_size: the cell edge, as the reference's Python float.
+ * Voxel of a point (:23-28): ((p - frame_min) // float32(voxel_size)).astype(int32) per axis, NumPy float32 floor_divide.
+ * Output order (:29-34): frames in order, and inside a frame ascending ix + iy * dim_x + iz * dim_y * dim_x.
+ *   out_xyz [capacity,3], out_attr [capacity,attr_channels], out_frame_ptr [num_frames+1], *out_num_host = number of
+ *   voxels (one host round trip; the call synchronises the stream).  capacity = M always suffices; PG_ERR_CAPACITY with
+ *   the needed count otherwise.  M = 0 gives no voxel and a zero out_frame_ptr.
+ * Means (:35-42): the reference adds float32 values in an unspecified order (np.argsort is not stable) and returns
+ * float64 means.  Here a voxel's values are added in fp64 in ascending point index, divided in fp64 and rounded once to
+ * float32.  Voxel membership, count and order are the reference's exactly; the means agree within 1e-4.  Frames are
+ * independent: a batch returns the bits of its single-frame calls.
+ * Errors: PG_ERR_INVALID_ARGUMENT for a voxel_size that is not positive and finite, and for a frame (named in the
+ * message) whose dim_x * dim_y * dim_z exceeds 2^31 - 1, where the reference's int32 key wraps; PG_ERR_RANGE when a
+ * frame spans more than 65 536 voxels on one axis.
+ */
+PG_API int pg_voxel_average(const float* xyz, const float* attr, int32_t attr_channels, const int32_t* frame_ptr,
+                            int32_t num_frames, int64_t num_points, double voxel_size, float* out_xyz,
+                            float* out_attr, int64_t capacity, int32_t* out_frame_ptr, int64_t* out_num_host,
+                            void* stream);
+
 /* ------------------------------------------------------------------------ *
  * Graph construction  (reference models/graph_gen.py)
  * ------------------------------------------------------------------------ */

@@ -14,6 +14,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libpointgnn_b200.so')
 
 PG_ERR_CAPACITY = -3
+PG_ERR_RANGE = -4
 
 c_i32p = ctypes.c_void_p
 c_f32p = ctypes.c_void_p
@@ -71,6 +72,13 @@ SIGNATURES = {
                                               ctypes.POINTER(ctypes.c_double), ctypes.POINTER(c_i32), ctypes.c_void_p,
                                               ctypes.POINTER(c_i64), c_f32p, c_f32p, c_i32, c_i64, c_i32p,
                                               ctypes.POINTER(c_i64), ctypes.c_void_p]),
+    'pg_velo_to_cam': (ctypes.c_int, [c_f32p, c_i32p, c_i32, c_i64, ctypes.POINTER(ctypes.c_float), c_f32p, c_f32p,
+                                      ctypes.c_void_p]),
+    'pg_cam_points_crop': (ctypes.c_int, [c_f32p, c_f32p, c_i32p, c_i32, c_i64, ctypes.POINTER(ctypes.c_double),
+                                          ctypes.POINTER(c_i32), ctypes.c_void_p, ctypes.POINTER(c_i64), c_f32p, c_f32p,
+                                          c_i32, c_i64, c_i32p, ctypes.POINTER(c_i64), ctypes.c_void_p]),
+    'pg_voxel_average': (ctypes.c_int, [c_f32p, c_f32p, c_i32, c_i32p, c_i32, c_i64, ctypes.c_double, c_f32p, c_f32p,
+                                        c_i64, c_i32p, ctypes.POINTER(c_i64), ctypes.c_void_p]),
     'pg_decode_boxes': (ctypes.c_int, [c_f32p, c_f32p, c_i64, c_i32, ctypes.POINTER(ctypes.c_float), c_f32p,
                                        ctypes.c_void_p]),
     'pg_postprocess': (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_i32p, c_i32, c_i64, c_i32,
@@ -680,6 +688,23 @@ def kitti_rows(label, box, score, det_frame_ptr, xyz, cand_index, cand_frame_ptr
 # ---------------------------------------------------------------------------------------------
 # input stage
 # ---------------------------------------------------------------------------------------------
+def _crop_host_args(num_frames, cam_to_image, image_sizes, images, image_offsets):
+    """The host arrays both crop entry points take -> (cam_to_image, image_sizes, images, image_offsets) as ctypes
+    arguments, and the arrays themselves, which must stay referenced during the call."""
+    import numpy as np
+    cti = np.ascontiguousarray(cam_to_image, dtype=np.float64).reshape(num_frames, 12)
+    wh = np.ascontiguousarray(image_sizes, dtype=np.int32).reshape(num_frames, 2)
+    offs = None
+    if images is not None:
+        offs = np.ascontiguousarray(image_offsets, dtype=np.int64)
+        if images.dtype != torch.uint8 or not images.is_cuda:
+            raise TypeError('images must be a CUDA uint8 tensor')
+    args = (cti.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), wh.ctypes.data_as(ctypes.POINTER(c_i32)),
+            None if images is None else ctypes.c_void_p(images.data_ptr()),
+            None if offs is None else offs.ctypes.data_as(ctypes.POINTER(c_i64)))
+    return args, (cti, wh, offs)
+
+
 def cam_points_in_image(velo, frame_ptr, velo_to_cam, cam_to_image, image_sizes, images=None, image_offsets=None):
     """pg_cam_points_in_image.  velo [M,4] CUDA fp32, frame_ptr [F+1] CUDA int32, velo_to_cam [F,4,4] / cam_to_image
     [F,3,4] / image_sizes [F,2] host arrays; images: optional CUDA uint8 buffer (+ byte offsets per frame).
@@ -689,26 +714,87 @@ def cam_points_in_image(velo, frame_ptr, velo_to_cam, cam_to_image, image_sizes,
     m = velo.shape[0]
     num_frames = frame_ptr.numel() - 1
     vtc = np.ascontiguousarray(velo_to_cam, dtype=np.float32).reshape(num_frames, 16)
-    cti = np.ascontiguousarray(cam_to_image, dtype=np.float64).reshape(num_frames, 12)
-    wh = np.ascontiguousarray(image_sizes, dtype=np.int32).reshape(num_frames, 2)
+    crop_args, _keep = _crop_host_args(num_frames, cam_to_image, image_sizes, images, image_offsets)
     channels = 4 if images is not None else 1
     out_xyz = torch.empty((m, 3), dtype=torch.float32, device=velo.device)
     out_attr = torch.empty((m, channels), dtype=torch.float32, device=velo.device)
     out_fp = torch.empty(num_frames + 1, dtype=torch.int32, device=velo.device)
     n = c_i64(0)
-    offs = None
-    if images is not None:
-        offs = np.ascontiguousarray(image_offsets, dtype=np.int64)
-        if images.dtype != torch.uint8 or not images.is_cuda:
-            raise TypeError('images must be a CUDA uint8 tensor')
     _check(lib.pg_cam_points_in_image(
         _ptr(velo, torch.float32, 'velo'), _ptr(frame_ptr, torch.int32, 'frame_ptr'), num_frames, m,
-        vtc.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), cti.ctypes.data_as(ctypes.POINTER(ctypes.c_double)),
-        wh.ctypes.data_as(ctypes.POINTER(c_i32)), None if images is None else ctypes.c_void_p(images.data_ptr()),
-        None if offs is None else offs.ctypes.data_as(ctypes.POINTER(c_i64)), _ptr(out_xyz, torch.float32, 'out_xyz'),
+        vtc.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), *crop_args, _ptr(out_xyz, torch.float32, 'out_xyz'),
         _ptr(out_attr, torch.float32, 'out_attr'), channels, m, _ptr(out_fp, torch.int32, 'out_fp'), ctypes.byref(n),
         _stream()))
     return out_xyz[:n.value], out_attr[:n.value], out_fp
+
+
+def velo_to_cam(velo, frame_ptr, velo_to_cam):
+    """pg_velo_to_cam: the transform of ``cam_points_in_image`` alone, same argument forms.
+    -> (xyz [M,3] camera-frame points, attr [M,1] reflectance)."""
+    import numpy as np
+    m = velo.shape[0]
+    num_frames = frame_ptr.numel() - 1
+    vtc = np.ascontiguousarray(velo_to_cam, dtype=np.float32).reshape(num_frames, 16)
+    out_xyz = torch.empty((m, 3), dtype=torch.float32, device=velo.device)
+    out_attr = torch.empty((m, 1), dtype=torch.float32, device=velo.device)
+    _check(load().pg_velo_to_cam(
+        _ptr(velo, torch.float32, 'velo'), _ptr(frame_ptr, torch.int32, 'frame_ptr'), num_frames, m,
+        vtc.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), _ptr(out_xyz, torch.float32, 'out_xyz'),
+        _ptr(out_attr, torch.float32, 'out_attr'), _stream()))
+    return out_xyz, out_attr
+
+
+def cam_points_crop(xyz, reflectance, frame_ptr, cam_to_image, image_sizes, images=None, image_offsets=None):
+    """pg_cam_points_crop: the crop and colour lookup of ``cam_points_in_image`` from camera-frame points xyz [N,3] with
+    reflectance [N,1] (CUDA fp32).  The other arguments and the result are ``cam_points_in_image``'s."""
+    n_in = xyz.shape[0]
+    num_frames = frame_ptr.numel() - 1
+    crop_args, _keep = _crop_host_args(num_frames, cam_to_image, image_sizes, images, image_offsets)
+    channels = 4 if images is not None else 1
+    out_xyz = torch.empty((n_in, 3), dtype=torch.float32, device=xyz.device)
+    out_attr = torch.empty((n_in, channels), dtype=torch.float32, device=xyz.device)
+    out_fp = torch.empty(num_frames + 1, dtype=torch.int32, device=xyz.device)
+    n = c_i64(0)
+    _check(load().pg_cam_points_crop(
+        _ptr(xyz, torch.float32, 'xyz'), _ptr(reflectance, torch.float32, 'reflectance'),
+        _ptr(frame_ptr, torch.int32, 'frame_ptr'), num_frames, n_in, *crop_args, _ptr(out_xyz, torch.float32, 'out_xyz'),
+        _ptr(out_attr, torch.float32, 'out_attr'), channels, n_in, _ptr(out_fp, torch.int32, 'out_fp'), ctypes.byref(n),
+        _stream()))
+    return out_xyz[:n.value], out_attr[:n.value], out_fp
+
+
+class VoxelAverageError(PointGNNError, ValueError):
+    """pg_voxel_average rejected the voxel size, or a frame has more voxels than the reference's int32 voxel key (or
+    the grid's 16 bits per axis) can number."""
+
+
+def voxel_average(xyz, attr, frame_ptr, voxel_size):
+    """pg_voxel_average.  xyz [M,3] CUDA fp32, attr None or [M,C] CUDA fp32 with C <= 4, frame_ptr [F+1] CUDA int32.
+    -> (xyz [V,3], attr [V,C] or None, frame_ptr [F+1]): one point per occupied voxel, see include/pointgnn_b200.h."""
+    import math
+    voxel_size = float(voxel_size)
+    if not (voxel_size > 0.0 and math.isfinite(voxel_size)):
+        raise VoxelAverageError(PG_ERR_INVALID_ARGUMENT, 'voxel_size must be positive and finite, got %r' % voxel_size)
+    if xyz.dim() != 2 or xyz.shape[1] != 3:
+        raise ValueError('xyz must be [M, 3], got %s' % (tuple(xyz.shape),))
+    m = xyz.shape[0]
+    if attr is not None and (attr.dim() != 2 or attr.shape[0] != m):
+        raise ValueError('attr must be [%d, C], got %s' % (m, tuple(attr.shape)))
+    channels = 0 if attr is None else attr.shape[1]
+    num_frames = frame_ptr.numel() - 1
+    out_xyz = torch.empty((m, 3), dtype=torch.float32, device=xyz.device)
+    out_attr = None if attr is None else torch.empty((m, channels), dtype=torch.float32, device=xyz.device)
+    out_fp = torch.empty(num_frames + 1, dtype=torch.int32, device=xyz.device)
+    n = c_i64(0)
+    lib = load()
+    code = lib.pg_voxel_average(
+        _ptr(xyz, torch.float32, 'xyz'), _ptr(attr, torch.float32, 'attr'), channels,
+        _ptr(frame_ptr, torch.int32, 'frame_ptr'), num_frames, m, voxel_size, _ptr(out_xyz, torch.float32, 'out_xyz'),
+        _ptr(out_attr, torch.float32, 'out_attr'), m, _ptr(out_fp, torch.int32, 'out_fp'), ctypes.byref(n), _stream())
+    if code in (PG_ERR_INVALID_ARGUMENT, PG_ERR_RANGE):
+        raise VoxelAverageError(code, lib.pg_last_error().decode())
+    _check(code)
+    return out_xyz[:n.value], None if attr is None else out_attr[:n.value], out_fp
 
 
 # ---------------------------------------------------------------------------------------------

@@ -14,7 +14,7 @@
 // nearest point, radius test) are evaluated in fp64 with explicitly rounded mul/add
 // (no FMA contraction), which is what makes the edge lists bit-exact against the reference's
 // scikit-learn float64 trees.
-#include "pg_common.cuh"
+#include "pg_grid.cuh"
 
 namespace pg {
 namespace {
@@ -61,32 +61,6 @@ __global__ void frame_min_kernel(const float* __restrict__ xyz, const int32_t* _
     atomicMin(&bounds[3 * f + 2], float_to_ordered(mz));
   }
 }
-
-// How a point's cell index follows from its coordinates and the bounding-box minimum of its frame.
-enum class CellRule : int {
-  // open3d.voxel_down_sample (graph_gen.py:41-45): origin = frame_min - cell / 2, floor((p - origin) / cell) in fp64
-  kVoxel,
-  // radius and nearest-vertex search grids: origin = frame_min, floor((p - origin) / cell) in fp64 on the coordinates
-  // divided by `scale` if `scaled`
-  kRadius,
-  // multi_layer_downsampling_random without add_rnd3d (graph_gen.py:124-126): floor_divide(p - frame_min, cell) in
-  // float32
-  kNumpyF32,
-  // add_rnd3d (graph_gen.py:24-31, 127-130): floor_divide((p - frame_min)[float32] + cell * shift[frame], cell) in
-  // float64, shift = the np.random.random((1, 3)) draw of the frame
-  kNumpyF64Shift,
-};
-
-// Grid description shared by key generation and queries.
-struct GridSpec {
-  double cell[3];     // cell edge per axis
-  CellRule rule;
-  // gen_disjointed_rnn_local_graph_v3's `scale` (graph_gen.py:203-206): every coordinate is DIVIDED by scale[axis] in
-  // float64 before anything else (points_xyz / np.array(scale) -> float64).  scaled == 0: coordinates as they are.
-  int scaled;
-  double scale[3];
-  const double* shift;   // kNumpyF64Shift: [num_frames][3] on the device
-};
 
 // coordinate of axis a as the reference sees it: float32 value -> float64, divided by the scale if there is one
 __device__ __forceinline__ double coord(const GridSpec& g, float v, int a) {
@@ -202,13 +176,6 @@ __device__ inline int lower_bound_u64(const uint64_t* __restrict__ a, int n, uin
   return lo;
 }
 
-struct SortedGrid {
-  const uint64_t* cell_key;   // [num_cells]
-  const int32_t* cell_start;  // [num_cells+1]
-  const float4* pts;          // [n] sorted (x,y,z,orig idx)
-  const int32_t* num_cells;   // device scalar (= last element of the head-flag scan): no host round trip
-};
-
 // point range covering cells (f, iz, iy, ix_lo..ix_hi); indices already clamped to [0, kAxisMax]
 __device__ inline void row_range(const SortedGrid& g, uint32_t f, uint32_t iz, uint32_t iy, uint32_t ix_lo,
                                  uint32_t ix_hi, int* begin, int* end) {
@@ -224,21 +191,6 @@ __device__ inline double dist2_rn(double ax, double ay, double az, double bx, do
   const double dy = __dsub_rn(ay, by);
   const double dz = __dsub_rn(az, bz);
   return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
-}
-
-// fp64 centroid of the sorted points [s, e) of one voxel, summed in ascending point order (the sort is stable)
-__device__ inline void voxel_centroid(const SortedGrid& g, int s, int e, double c[3]) {
-  double sx = 0.0, sy = 0.0, sz = 0.0;
-  for (int i = s; i < e; ++i) {
-    const float4 p = g.pts[i];
-    sx = __dadd_rn(sx, double(p.x));
-    sy = __dadd_rn(sy, double(p.y));
-    sz = __dadd_rn(sz, double(p.z));
-  }
-  const double cnt = double(e - s);
-  c[0] = __ddiv_rn(sx, cnt);
-  c[1] = __ddiv_rn(sy, cnt);
-  c[2] = __ddiv_rn(sz, cnt);
 }
 
 // ---- exact nearest point: fp64 squared distance, ties -> lowest original index ----------------------------------
@@ -545,11 +497,6 @@ __global__ void gather_keypoints_kernel(const float* __restrict__ xyz, const int
 }
 
 // ---- host-side building blocks ----------------------------------------------------------------
-struct BuiltGrid {
-  Temp bounds, keys_a, keys_b, vals_a, vals_b, sorted_pts, head, head_scan, cell_key, cell_start, err;
-  SortedGrid view{};
-};
-
 // key bits the frame field needs, including frame `num_frames` (the key of rows beyond n_valid, voxels beyond K)
 int frame_bits(int num_frames) {
   int bits = 1;
@@ -557,8 +504,10 @@ int frame_bits(int num_frames) {
   return bits;
 }
 
+}  // namespace
+
 int build_grid(const float* xyz, const int32_t* frame_ptr, int num_frames, int64_t n, const GridSpec& spec,
-               cudaStream_t s, BuiltGrid* out, const int32_t* n_valid = nullptr) {
+               cudaStream_t s, BuiltGrid* out, const int32_t* n_valid) {
   PG_REQUIRE(num_frames >= 1 && num_frames <= 65534, "num_frames=%d out of range [1,65534]", num_frames);
   PG_REQUIRE(n >= 1 && n < (int64_t(1) << 31), "num_points=%lld out of range", (long long)n);
   PG_CUDA_OK(out->bounds.alloc(sizeof(uint32_t) * 3 * num_frames, s));
@@ -625,6 +574,13 @@ int graph_error(int err) {
   return PG_OK;
 }
 
+int frame_ranges(const uint64_t* keys, const int32_t* num_keys, int num_frames, int frame_shift, int32_t* out_frame_ptr,
+                 cudaStream_t s) {
+  frame_ranges_kernel<<<ceil_div(num_frames + 1, 128), 128, 0, s>>>(keys, num_keys, num_frames, frame_shift, out_frame_ptr);
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}
+
 // ---- keypoint calls: voxel grid spec, and the end every keypoint call shares ----------------------------------
 int voxel_spec(const double* voxel_size_host, CellRule rule, GridSpec* spec) {
   PG_REQUIRE(voxel_size_host[0] > 0 && voxel_size_host[1] > 0 && voxel_size_host[2] > 0, "voxel size must be positive");
@@ -633,6 +589,8 @@ int voxel_spec(const double* voxel_size_host, CellRule rule, GridSpec* spec) {
   spec->rule = rule;
   return PG_OK;
 }
+
+namespace {
 
 // kNumpyF64Shift: the per-frame shifts (host [num_frames][3]) copied to the device
 int upload_shift(const double* shift_host, int num_frames, cudaStream_t s, Temp* shift, GridSpec* spec) {
@@ -648,8 +606,7 @@ int upload_shift(const double* shift_host, int num_frames, cudaStream_t s, Temp*
 int finish_keypoints(const uint64_t* keys, int frame_shift, const int32_t* num_keys, int num_frames, const int* err0,
                      const int* err1, int64_t capacity, const char* what, int32_t* out_frame_ptr, int64_t* out_num_host,
                      cudaStream_t s) {
-  frame_ranges_kernel<<<ceil_div(num_frames + 1, 128), 128, 0, s>>>(keys, num_keys, num_frames, frame_shift, out_frame_ptr);
-  PG_LAUNCH_CHECK();
+  if (int rc = frame_ranges(keys, num_keys, num_frames, frame_shift, out_frame_ptr, s)) return rc;
   int32_t h[3] = {0, 0, 0};
   PG_CUDA_OK(cudaMemcpyAsync(&h[0], num_keys, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
   PG_CUDA_OK(cudaMemcpyAsync(&h[1], err0, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
@@ -1007,9 +964,7 @@ extern "C" int pg_multi_level_graph(const float* xyz, const int32_t* frame_ptr, 
   voxel_keypoint_kernel<<<ceil_div(num_points, 128), 128, 0, s>>>(vgrid.view, vspec, vgrid.bounds.as<uint32_t>(),
                                                                     out_keypoint_idx, kp_capacity);
   PG_LAUNCH_CHECK();
-  frame_ranges_kernel<<<ceil_div(num_frames + 1, 128), 128, 0, s>>>(vgrid.view.cell_key, vgrid.view.num_cells, num_frames,
-                                                                     48, out_kp_frame_ptr);
-  PG_LAUNCH_CHECK();
+  if (int rc = frame_ranges(vgrid.view.cell_key, vgrid.view.num_cells, num_frames, 48, out_kp_frame_ptr, s)) return rc;
   const int32_t* k_dev = vgrid.view.num_cells;      // K = number of occupied voxels, on the device
   gather_keypoints_kernel<<<ceil_div(kp_capacity, 256), 256, 0, s>>>(xyz, out_keypoint_idx, k_dev, kp_capacity, out_kp_xyz);
   PG_LAUNCH_CHECK();

@@ -13,7 +13,9 @@
 * ``beam_downsample_batch`` - the beam downsampling of the reference's ``scripts/point_cloud_downsample.py`` on the GPU
   (``pg_beam_downsample``), with an exact 1-D k-means in place of its scikit-learn ``KMeans``.
 * ``cam_points_in_image_batch`` - several frames in one GPU call, results staying on the device (what the
-  batched ``run.py`` and the end-to-end bench use).
+  batched ``run.py`` and the end-to-end bench use); with ``downsample_voxel_size`` the camera-frame cloud is averaged
+  per voxel ahead of the crop, as ``get_cam_points`` does (kitti_dataset.py:624-626).
+* ``downsample_by_average_voxel`` - kitti_dataset.py:16-48 on the GPU (``pg_voxel_average``) for one frame.
 """
 import os
 from collections import namedtuple
@@ -90,9 +92,28 @@ def parse_calib(calib_file):
     return calib
 
 
-def cam_points_in_image_batch(velo_list, calib_list, image_size_list, image_list=None, device=None):
+def downsample_by_average_voxel(points, voxel_size):
+    """kitti_dataset.py:16-48 on the GPU: one point per occupied voxel of ``points`` (one frame, NumPy ``Points``;
+    ``attr`` may be None), in ascending voxel-key order, xyz and attr the voxel's means.  The means are float32 (fp64
+    sums in point order, rounded once) where the reference returns float64 from float32 sums of unspecified order; they
+    agree within 1e-4.  Raises ValueError for a voxel size that is not positive and finite, or so small that the
+    reference's int32 voxel key would wrap."""
+    device = torch.device('cuda', torch.cuda.current_device())
+    xyz = torch.from_numpy(np.ascontiguousarray(points.xyz, dtype=np.float32).reshape(-1, 3)).to(device)
+    attr = None
+    if points.attr is not None:
+        attr = torch.from_numpy(np.ascontiguousarray(points.attr, dtype=np.float32)).to(device)      # [M, C]
+    fp = torch.tensor([0, xyz.shape[0]], dtype=torch.int32, device=device)
+    out_xyz, out_attr, _ = _lib.voxel_average(xyz, attr, fp, voxel_size)
+    return Points(xyz=out_xyz.cpu().numpy(), attr=None if out_attr is None else out_attr.cpu().numpy())
+
+
+def cam_points_in_image_batch(velo_list, calib_list, image_size_list, image_list=None, device=None,
+                              downsample_voxel_size=None):
     """Several frames in ONE GPU call.  velo_list: [Mi,4] float32 arrays (the .bin contents); calib_list: dicts of
-    ``parse_calib``; image_size_list: (width, height); image_list: optional BGR uint8 images (for rgb attributes).
+    ``parse_calib``; image_size_list: (width, height); image_list: optional BGR uint8 images (for rgb attributes);
+    downsample_voxel_size: None, or the voxel edge of ``downsample_by_average_voxel``, applied to every frame's
+    camera-frame cloud before the crop (three calls then: transform, average, crop).
     -> (xyz [N,3] CUDA, attr [N,1|4] CUDA, frame_ptr [F+1] CUDA int32)."""
     device = device or torch.device('cuda', torch.cuda.current_device())
     sizes = [v.shape[0] for v in velo_list]
@@ -105,8 +126,13 @@ def cam_points_in_image_batch(velo_list, calib_list, image_size_list, image_list
         flat = [np.ascontiguousarray(im, dtype=np.uint8).reshape(-1) for im in image_list]
         offsets = np.concatenate([[0], np.cumsum([f.size for f in flat])[:-1]]).astype(np.int64)
         images = torch.from_numpy(np.concatenate(flat)).to(device)
-    return _lib.cam_points_in_image(velo, torch.from_numpy(fp).to(device), vtc, cti, np.asarray(image_size_list, np.int32),
-                                    images, offsets)
+    fp = torch.from_numpy(fp).to(device)
+    wh = np.asarray(image_size_list, np.int32)
+    if downsample_voxel_size is None:
+        return _lib.cam_points_in_image(velo, fp, vtc, cti, wh, images, offsets)
+    xyz, refl = _lib.velo_to_cam(velo, fp, vtc)
+    xyz, refl, fp = _lib.voxel_average(xyz, refl, fp, downsample_voxel_size)
+    return _lib.cam_points_crop(xyz, refl, fp, cti, wh, images, offsets)
 
 
 def beam_downsample_batch(velo, frame_ptr=None, downsample_rate=2, num_clusters=64, centers=None):
@@ -217,15 +243,14 @@ class KittiDataset(object):
 
     def get_cam_points_in_image_with_rgb(self, frame_idx, downsample_voxel_size=None, calib=None, xyz_range=None):
         """kitti_dataset.py:666-689 on the GPU -> Points(xyz [N,3], attr [N,4] = reflectance, r, g, b) as NumPy."""
-        if downsample_voxel_size is not None:
-            raise NotImplementedError('downsample_by_voxel_size is null in every shipped config (kitti_dataset.py:16-48)')
         if xyz_range is not None:
             raise NotImplementedError('xyz_range is not used by run.py')
         if calib is None:
             calib = self.get_calib(frame_idx)
         image = self.get_image(frame_idx)
         xyz, attr, _ = cam_points_in_image_batch([self.get_velo_data(frame_idx)], [calib],
-                                                 [(image.shape[1], image.shape[0])], [image])
+                                                 [(image.shape[1], image.shape[0])], [image],
+                                                 downsample_voxel_size=downsample_voxel_size)
         return Points(xyz=xyz.cpu().numpy(), attr=attr.cpu().numpy())
 
     def cam_points_to_image(self, points, calib):

@@ -6,7 +6,9 @@ TensorFlow-1 pieces are replaced by this package:
   reference run.py      here
   :104-150  placeholders + model.predict graph build   -> ``model = get_model(...)(...)``, nothing to build
   :192-202  tf.Session, Saver.restore                  -> ``model.load_checkpoint(CHECKPOINT_PATH)`` (no TensorFlow)
-  :210-215  dataset.get_cam_points_in_image_with_rgb   -> GPU input stage (dataset.kitti_dataset, pg_cam_points_in_image)
+  :210-215  dataset.get_cam_points_in_image_with_rgb   -> GPU input stage (dataset.kitti_dataset, pg_cam_points_in_image;
+                                                          with config['downsample_by_voxel_size']: pg_velo_to_cam,
+                                                          pg_voxel_average, pg_cam_points_crop)
   :219-222  graph_generate_fn(...)                     -> GPU graph build (models.graph_gen, pg_multi_level_graph)
   :252-260  sess.run(fetches, feed_dict)               -> ``model.predict`` / ``model.postprocess`` (CUDA kernels)
   :265-325  box decoding + nms.nms_boxes_3d_*          -> models.postprocess.detect (pg_postprocess), one call
@@ -90,6 +92,17 @@ def input_features(config, attr):
     if kind == '0':
         return torch.zeros_like(attr[:, :1])
     raise KeyError(kind)
+
+
+def input_stage(config, velo, calib, size, image, device):
+    """run.py:210-215 for a batch: the frames' camera-frame points inside their images, averaged per voxel first when
+    config['downsample_by_voxel_size'] is set (absent or null: off) -> (xyz, attr, frame_ptr) on the device, attr
+    padded to four columns for the input features that want them without colour."""
+    xyz, attr, frame_ptr = kitti_dataset.cam_points_in_image_batch(
+        velo, calib, size, image, device=device, downsample_voxel_size=config.get('downsample_by_voxel_size'))
+    if image is None and config['input_features'] in ('0000', 'i000'):
+        attr = torch.cat([attr, torch.zeros((attr.shape[0], 3), device=device)], dim=1)
+    return xyz, attr, frame_ptr
 
 
 def kitti_labels(class_labels, detection_boxes_3d, box_probs, candidate_xyz, calib, label_method, use_box_score,
@@ -231,7 +244,6 @@ def main(argv=None):
         time_dict[key] = time_dict.get(key, 0) + seconds
 
     want_rgb = config['input_features'] in ('irgb', '0rgb')
-    pad_attr = not want_rgb and config['input_features'] in ('0000', 'i000')
     last_layer_graph_level = config['model_kwargs']['layer_configs'][-1]['graph_level']
     batches = [list(range(first, min(first + args.batch_size, NUM_TEST_SAMPLE)))
                for first in range(0, NUM_TEST_SAMPLE, args.batch_size)]
@@ -264,9 +276,7 @@ def main(argv=None):
         velo, calib, size, image = pending.pop(b).result()
         start_reading(b + 1)
         with torch.cuda.stream(prefetcher.stream):
-            xyz, attr, frame_ptr = kitti_dataset.cam_points_in_image_batch(velo, calib, size, image, device=device)
-            if pad_attr:
-                attr = torch.cat([attr, torch.zeros((attr.shape[0], 3), device=device)], dim=1)
+            xyz, attr, frame_ptr = input_stage(config, velo, calib, size, image, device)
             t1 = time.time()
             # submitted from the side stream: the inputs were made there, so the build waits for nothing else
             ticket = prefetcher.submit(xyz, attr, frame_ptr)

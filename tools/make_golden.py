@@ -178,6 +178,51 @@ def kitti_goldens():
     print('kitti: points in image', pts.xyz.shape, 'result lines', text.count('\n') - 1)
 
 
+VOXEL_AVG_SIZES = (0.1, 0.4)
+
+
+def kitti_voxel_avg_goldens():
+    """tests/golden/kitti_voxel_avg.npz: the reference's own get_cam_points / get_cam_points_in_image_with_rgb
+    (kitti_dataset.py:611-627, 666-689, with downsample_by_average_voxel :16-48) on the synthetic frame of kitti_io.npz,
+    for two voxel sizes.  Per size <s>: keys_<s> / counts_<s> (the occupied voxels, recomputed from the reference's own
+    index arithmetic), mean_xyz_<s> / mean_attr_<s> (its float64 means), crop_index_<s> (ranks of the voxels that
+    survive its crop), crop_xyz_<s> / crop_attr_<s> (its result), and crop_unsure_<s> / pixel_unsure_<s>: ranks whose
+    crop verdict / colour pixel changes when the mean moves by 1e-4 (oracle.voxel_average.decision_margin)."""
+    import cv2
+    from oracle import kitti as ok
+    from oracle import voxel_average as ova
+    ref = ok.reference_dataset_module()
+    root = tempfile.mkdtemp()
+    ok.write_synthetic_kitti(root, [5], 6000)
+    ds = ref.KittiDataset(os.path.join(root, 'image/testing/image_2'), os.path.join(root, 'velodyne/testing/velodyne/'),
+                          os.path.join(root, 'calib/testing/calib/'), '', num_classes=4, is_training=False)
+    io = np.load(os.path.join(GOLDEN, 'kitti_io.npz'))
+    velo = np.fromfile(os.path.join(root, 'velodyne/testing/velodyne/000000.bin'), dtype=np.float32).reshape(-1, 4)
+    image = cv2.imread(os.path.join(root, 'image/testing/image_2/000000.png'))
+    assert np.array_equal(velo, io['velo']) and np.array_equal(image, io['image']), 'not the frame of kitti_io.npz'
+    calib = ds.get_calib(0)
+    height, width = image.shape[:2]
+    out = {}
+    for vs in VOXEL_AVG_SIZES:
+        tag = ('%g' % vs).replace('.', 'p')
+        full = ds.get_cam_points(0)
+        avg = ds.get_cam_points(0, downsample_voxel_size=vs)
+        crop = ds.get_cam_points_in_image_with_rgb(0, vs)
+        keys, _ = ova.voxel_keys(full.xyz, vs)
+        unique_keys, counts = np.unique(keys, return_counts=True)
+        assert len(unique_keys) == len(avg.xyz) and avg.xyz.dtype == np.float64
+        keep, _ = ova.crop_mask(avg.xyz, calib, width, height)
+        assert np.array_equal(avg.xyz[keep], crop.xyz), 'restated crop != reference crop'
+        crop_unsure, pixel_unsure = ova.decision_margin(avg.xyz, calib, width, height)
+        out.update({'keys_' + tag: unique_keys, 'counts_' + tag: counts, 'mean_xyz_' + tag: avg.xyz,
+                    'mean_attr_' + tag: avg.attr, 'crop_index_' + tag: np.flatnonzero(keep), 'crop_xyz_' + tag: crop.xyz,
+                    'crop_attr_' + tag: crop.attr, 'crop_unsure_' + tag: np.flatnonzero(crop_unsure),
+                    'pixel_unsure_' + tag: np.flatnonzero(pixel_unsure)})
+        print('kitti_voxel_avg', vs, 'points', len(full.xyz), 'voxels', len(unique_keys), 'in image', len(crop.xyz),
+              'crop unsure', int(crop_unsure.sum()), 'pixel unsure', int(pixel_unsure.sum()))
+    np.savez_compressed(os.path.join(GOLDEN, 'kitti_voxel_avg.npz'), **out)
+
+
 def graph_random_goldens():
     """tests/golden/graph_random.npz: the reference's OWN multi_layer_downsampling_random (graph_gen.py:92-153) with its
     two random sources patched to recorded numbers: np.random.random -> `shift`, random.choice(seq) ->
@@ -526,6 +571,8 @@ if __name__ == '__main__':
         post_goldens()
     if which in ('all', 'kitti'):
         kitti_goldens()
+    if which in ('all', 'kitti_voxel_avg'):
+        kitti_voxel_avg_goldens()
     if which in ('all', 'graph_live_reference'):
         graph_live_reference_goldens()
     if which in ('all', 'checkpoints'):
