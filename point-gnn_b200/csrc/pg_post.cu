@@ -213,10 +213,12 @@ __global__ void sorted_geometry_kernel(const int32_t* __restrict__ order, const 
 }
 
 // bit j - (i & ~31)... of row i: candidate j (> i, same frame, same class) overlaps candidate i by more than thres.
-// Rows are `words` 32-bit words wide and indexed by the position INSIDE the frame.
+// Rows are `words` 32-bit words wide and indexed by the position INSIDE the frame.  The two rules differ only for a
+// NaN overlap (0 / 0: both unions zero, e.g. two boxes of height 0): nms.py's merge / rescore variants remove a box iff
+// `overlap > thres` (NaN: kept), bboxes_nms (the int_corners path) keeps it iff `overlap <= thres` (NaN: removed).
 __global__ void adjacency_kernel(const BoxGeom* __restrict__ geom, const int32_t* __restrict__ s_label,
                                  const int32_t* __restrict__ cand_frame_ptr, int num_frames, int words, double thres,
-                                 uint32_t* __restrict__ adj) {
+                                 bool keep_if_le, uint32_t* __restrict__ adj) {
   const int f = blockIdx.z;
   const int begin = cand_frame_ptr[f], count = cand_frame_ptr[f + 1] - begin;
   const int lane = threadIdx.x & 31;
@@ -228,7 +230,10 @@ __global__ void adjacency_kernel(const BoxGeom* __restrict__ geom, const int32_t
          wj += gridDim.x * warps_per_block) {
       const int lj = wj * 32 + lane;
       bool hit = false;
-      if (lj > li && lj < count && s_label[begin + lj] == la) hit = iou_3d(a, geom[begin + lj]) > thres;
+      if (lj > li && lj < count && s_label[begin + lj] == la) {
+        const double ov = iou_3d(a, geom[begin + lj]);
+        hit = keep_if_le ? !(ov <= thres) : ov > thres;
+      }
       const uint32_t m = __ballot_sync(0xffffffffu, hit);
       if (lane == 0) adj[(int64_t(begin) + li) * words + wj] = m;
     }
@@ -475,7 +480,7 @@ static int nms_stage(Candidates& c, const Detections& out, double overlapped_thr
   {
     dim3 grid(std::max(1, std::min(words / 4 + 1, 16)), std::min(h_max, 4096), num_frames);
     adjacency_kernel<<<grid, 128, 0, s>>>(geom.as<BoxGeom>(), slabel.as<int32_t>(), cfp, num_frames, words,
-                                          overlapped_thres, adj.as<uint32_t>());
+                                          overlapped_thres, (flags & PG_NMS_INT_CORNERS) != 0, adj.as<uint32_t>());
     PG_LAUNCH_CHECK();
   }
   sweep_kernel<<<num_frames, 32, 0, s>>>(cfp, words, adj.as<uint32_t>(), valid.as<uint32_t>(), kept.as<int32_t>());
