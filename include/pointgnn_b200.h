@@ -574,18 +574,20 @@ PG_API int pg_beam_downsample(const float* velo, const int32_t* frame_ptr, int32
  *   flags     PG_KITTI_EVAL_AOS: the image metric also computes AOS (no detection has alpha = -10, :152-154);
  *             the other two always compute the heading similarity (AHS) from |gt.ry - det.ry|
  * Outputs (host), segment s = (m * 3 + c) * 3 + d:
- *   out_precision / out_aos / out_ahs [27][41]   the curves eval_class returns (zeros where not computed)
- *   out_num_thresholds [27]                      score thresholds of each segment, at most 41: where the
- *                                                reference would write past its 41-entry arrays (undefined
- *                                                behaviour), the thresholds after the 41st are dropped
- *   out_tp / out_fp / out_fn [27][41]            summed over frames per threshold (zeros past the count)
+ *   out_precision_host / out_aos_host / out_ahs_host [27][41]   the curves eval_class returns (zeros where not
+ *                                                               computed)
+ *   out_num_thresholds_host [27]                score thresholds of each segment, at most 41: where the reference
+ *                                               would write past its 41-entry arrays (undefined behaviour), the
+ *                                               thresholds after the 41st are dropped
+ *   out_tp_host / out_fp_host / out_fn_host [27][41]   summed over frames per threshold (zeros past the count)
  * No limit on boxes per frame.  One host round trip (the final read-back).
  */
 #define PG_KITTI_EVAL_AOS 1
 PG_API int pg_kitti_eval(const double* gt, const int32_t* gt_class, const double* det, const int32_t* det_class,
                   const int64_t* gt_frame_ptr_host, const int64_t* det_frame_ptr_host, int32_t num_frames,
-                  int32_t flags, double* out_precision, double* out_aos, double* out_ahs,
-                  int32_t* out_num_thresholds, int32_t* out_tp, int32_t* out_fp, int32_t* out_fn, void* stream);
+                  int32_t flags, double* out_precision_host, double* out_aos_host, double* out_ahs_host,
+                  int32_t* out_num_thresholds_host, int32_t* out_tp_host, int32_t* out_fp_host, int32_t* out_fn_host,
+                  void* stream);
 
 /* wgmma kernel launches so far (which: 0 = segment-max launches of the edge layers, 1 = store launches:
  * dense layers and the stored per-edge layers of point-set pooling);

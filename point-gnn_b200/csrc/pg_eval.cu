@@ -423,12 +423,12 @@ using namespace pg;
 
 extern "C" int pg_kitti_eval(const double* gt, const int32_t* gt_class, const double* det, const int32_t* det_class,
                              const int64_t* gt_frame_ptr_host, const int64_t* det_frame_ptr_host, int32_t num_frames,
-                             int32_t flags, double* out_precision, double* out_aos, double* out_ahs,
-                             int32_t* out_num_thresholds, int32_t* out_tp, int32_t* out_fp, int32_t* out_fn,
-                             void* stream) {
+                             int32_t flags, double* out_precision_host, double* out_aos_host, double* out_ahs_host,
+                             int32_t* out_num_thresholds_host, int32_t* out_tp_host, int32_t* out_fp_host,
+                             int32_t* out_fn_host, void* stream) {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  PG_REQUIRE(gt_frame_ptr_host && det_frame_ptr_host && out_precision && out_aos && out_ahs && out_num_thresholds &&
-                 out_tp && out_fp && out_fn,
+  PG_REQUIRE(gt_frame_ptr_host && det_frame_ptr_host && out_precision_host && out_aos_host && out_ahs_host &&
+                 out_num_thresholds_host && out_tp_host && out_fp_host && out_fn_host,
              "pg_kitti_eval: null argument");
   PG_REQUIRE(num_frames >= 1, "pg_kitti_eval: num_frames must be >= 1");
   const int64_t num_gt = gt_frame_ptr_host[num_frames], num_det = det_frame_ptr_host[num_frames];
@@ -554,13 +554,14 @@ extern "C" int pg_kitti_eval(const double* gt, const int32_t* gt_class, const do
   PG_LAUNCH_CHECK();
 
   const size_t curve = sizeof(double) * kSegments * kPoints, counts = sizeof(int32_t) * kSegments * kPoints;
-  PG_CUDA_OK(cudaMemcpyAsync(out_precision, prec.ptr, curve, cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaMemcpyAsync(out_aos, aos.ptr, curve, cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaMemcpyAsync(out_ahs, ahs.ptr, curve, cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaMemcpyAsync(out_num_thresholds, num_thr.ptr, sizeof(int32_t) * kSegments, cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaMemcpyAsync(out_tp, tp_sum.ptr, counts, cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaMemcpyAsync(out_fp, fp_sum.ptr, counts, cudaMemcpyDeviceToHost, s));
-  PG_CUDA_OK(cudaMemcpyAsync(out_fn, fn_sum.ptr, counts, cudaMemcpyDeviceToHost, s));
+  PG_CUDA_OK(cudaMemcpyAsync(out_precision_host, prec.ptr, curve, cudaMemcpyDeviceToHost, s));
+  PG_CUDA_OK(cudaMemcpyAsync(out_aos_host, aos.ptr, curve, cudaMemcpyDeviceToHost, s));
+  PG_CUDA_OK(cudaMemcpyAsync(out_ahs_host, ahs.ptr, curve, cudaMemcpyDeviceToHost, s));
+  PG_CUDA_OK(cudaMemcpyAsync(out_num_thresholds_host, num_thr.ptr, sizeof(int32_t) * kSegments, cudaMemcpyDeviceToHost,
+                             s));
+  PG_CUDA_OK(cudaMemcpyAsync(out_tp_host, tp_sum.ptr, counts, cudaMemcpyDeviceToHost, s));
+  PG_CUDA_OK(cudaMemcpyAsync(out_fp_host, fp_sum.ptr, counts, cudaMemcpyDeviceToHost, s));
+  PG_CUDA_OK(cudaMemcpyAsync(out_fn_host, fn_sum.ptr, counts, cudaMemcpyDeviceToHost, s));
   PG_CUDA_OK(cudaStreamSynchronize(s));
   return PG_OK;
 }

@@ -11,23 +11,64 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _header_symbols():
+def _header_text():
     with open(os.path.join(ROOT, 'include', 'pointgnn_b200.h')) as f:
-        text = f.read()
-    return sorted(set(re.findall(r'PG_API\s+[\w\s\*]+?\b(pg_\w+)\s*\(', text)))
+        return f.read()
 
 
-def test_library_exports_every_declared_symbol():
+def _header_symbols():
+    return sorted(set(re.findall(r'PG_API\s+[\w\s\*]+?\b(pg_\w+)\s*\(', _header_text())))
+
+
+def test_library_exports_every_parsed_prototype():
     from pointgnn_b200 import _lib
     lib = _lib.load()
     syms = _header_symbols()
     assert len(syms) >= 12
+    # one parsed prototype per PG_API declaration, and the library exports each with that prototype's arity
+    assert len(re.findall(r'^PG_API\b', _header_text(), re.M)) == len(_lib.PROTOTYPES)
+    assert sorted(_lib.PROTOTYPES) == syms
     for s in syms:
         assert hasattr(lib, s), 'libpointgnn_b200.so does not export %s' % s
-        assert s in _lib.SIGNATURES, 'ctypes binding missing for %s' % s
-    assert sorted(_lib.SIGNATURES) == syms
+        assert len(getattr(lib, s).argtypes) == len(_lib.PROTOTYPES[s][1])
     assert lib.pg_version() == 1
     assert lib.pg_last_error() == b''
+
+
+def test_header_parser():
+    """Integer #defines (negative, hex) become constants, macros do not; a type the binding does not know, or a
+    declaration it cannot read, is an ImportError naming it - never an untyped pointer."""
+    from pointgnn_b200 import _lib
+    prototypes, constants = _lib.parse_header('''
+        #define PG_API __attribute__((visibility("default")))
+        #define PG_A (-4)   /* comment */
+        #define PG_B 0x200
+        #define PG_C 16
+        #define PG_F(code) (PG_B | ((code) << PG_C))
+        PG_API const char* pg_x(void);   /* PG_API int pg_in_comment(void); */
+        PG_API int pg_y(const float* const* w_host, pg_layer **out, void* stream);''')
+    assert constants == {'PG_A': -4, 'PG_B': 0x200, 'PG_C': 16}
+    assert prototypes == {'pg_x': ('const char*', ()),
+                          'pg_y': ('int', (('const float* const*', 'w_host'), ('pg_layer**', 'out'),
+                                           ('void*', 'stream')))}
+    for params in ((('const half*', 'x'),), (('void*', 'x'),), (('int64_t*', 'x'),), (('const uint8_t*', 'x_host'),)):
+        with pytest.raises(ImportError, match=r'pg_z.*x'):
+            _lib._bind('pg_z', 'int', params)
+    with pytest.raises(ImportError, match='pg_q'):
+        _lib.parse_header('PG_API int pg_q(int32_t);')
+
+
+def test_call_binds_arguments_by_name(monkeypatch):
+    """_call rejects a missing, an extra and a misspelt argument name before it converts anything or calls the
+    library."""
+    from pointgnn_b200 import _lib
+    monkeypatch.setattr(_lib, 'load', lambda: pytest.fail('the library was called'))
+    args = dict(src=object(), dst=object(), num_edges=0, num_src=0, num_dst=0)
+    missing = {k: v for k, v in args.items() if k != 'num_dst'}
+    misspelt = {('dest' if k == 'dst' else k): v for k, v in args.items()}
+    for bad in (missing, dict(args, capacity=0), misspelt):
+        with pytest.raises(TypeError, match='pg_check_edges'):
+            _lib._call('pg_check_edges', **bad)
 
 
 def test_no_cpu_fallback():

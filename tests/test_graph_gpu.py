@@ -315,11 +315,10 @@ def test_neighbor_cap_invariants_and_seed(car):
     assert np.array_equal(_np(again), _np(capped))
 
 
-def test_radius_graph_capacity_contract():
+def test_radius_graph_capacity_contract_by_name():
     """pg_radius_graph with an edge buffer that is too small: PG_ERR_CAPACITY, the exact E, and a valid row_ptr."""
     import ctypes
     from pointgnn_b200 import _lib
-    lib = _lib.load()
     xyz, _ = synth.lidar_frame(12, 4000)
     pts = torch.from_numpy(xyz).cuda()
     ctr = pts[::5].contiguous()
@@ -330,11 +329,11 @@ def test_radius_graph_capacity_contract():
     rp = torch.full_like(row_ptr, -1)
     buf = torch.empty((2, 1), dtype=torch.int32, device='cuda')
     e = ctypes.c_int64(0)
-    code = lib.pg_radius_graph(ctypes.c_void_p(pts.data_ptr()), ctypes.c_void_p(fp.data_ptr()),
-                               ctypes.c_void_p(ctr.data_ptr()), ctypes.c_void_p(cfp.data_ptr()), 1, pts.shape[0],
-                               ctr.shape[0], 1.0, ctypes.c_void_p(rp.data_ptr()), ctypes.c_void_p(buf[0].data_ptr()),
-                               ctypes.c_void_p(buf[1].data_ptr()), 1, ctypes.byref(e), _lib._stream())
-    assert code == _lib.PG_ERR_CAPACITY
+    with pytest.raises(_lib.PointGNNError) as err:
+        _lib._call('pg_radius_graph', points=pts, point_frame_ptr=fp, centers=ctr, center_frame_ptr=cfp, num_frames=1,
+                   num_points=pts.shape[0], num_centers=ctr.shape[0], radius=1.0, out_row_ptr=rp, out_src=buf[0],
+                   out_dst=buf[1], capacity=1, out_num_edges_host=ctypes.byref(e))
+    assert err.value.code == _lib.PG_ERR_CAPACITY
     assert e.value == edges.shape[1] > 1
     assert torch.equal(rp, row_ptr)
 
