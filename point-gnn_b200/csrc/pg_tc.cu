@@ -1,8 +1,8 @@
 // Hopper tensor-core kernels (wgmma): the fast path (precision = 1, "BF16x3").
 //
 // wg_gemm_kernel - one persistent, warp-specialised kernel for every tensor-core layer of the network:
-//   out = epilogue(A @ W + b), W streamed by a producer warpgroup, A produced on the fly in shared memory by the
-//   two consumer warpgroups that also run the wgmmas.
+//   out = epilogue(A @ W + b), W streamed by a producer warpgroup, A produced on the fly (in registers, or in shared
+//   memory for the pooling launches) by the two consumer warpgroups that also run the wgmmas.
 //
 //   producers  PROD_ROWS  A = rows of an fp32 matrix (dense layers, a pooling layer wider than one launch)
 //              PROD_GNN   one GNN iteration's edge MLP (/root/reference/models/gnn.py:338-365) after hoisting:
@@ -31,13 +31,17 @@
 //              contiguous block per 16-k chunk) from L2 through a ring of shared-memory stages with
 //              cp.async.bulk, each stage tracked by a "full" (bytes landed) and an "empty" (both consumers done)
 //              mbarrier.  Warpgroups 1 and 2 are the consumers (setmaxnreg up to 240): 128 rows per tile (64 per
-//              warpgroup), the whole padded N (<= 304: two m64nNk16 instructions) in registers.  Each produces
-//              A into a double buffer, issuing the global loads of chunk k + 2 before the wgmmas of chunk k + 1,
-//              and splits and stores chunk k + 1 while chunk k's wgmmas run.  A consumer only arrives on "empty";
-//              it never waits on it or issues a copy: such divergent code in the k-loop makes ptxas serialise
-//              the wgmmas (C7518), and the two consumers would wait for each other on every chunk.
+//              warpgroup), the whole padded N (<= 304: two m64nNk16 instructions) in registers.  A streamed ROWS
+//              or GNN layer takes A from registers (wgmma_bf16_rs): each thread builds its own fragment of a chunk (its
+//              accumulators' two rows, 4 k) from its gathered fp32 values, in one of two alternating register
+//              buffers, issuing the global loads of chunk k + 2 before the wgmmas of chunk k + 1 and building
+//              chunk k + 1 while chunk k's wgmmas run: no shared-memory A, proxy fence or barrier per chunk.  The
+//              pooling launches read A from shared memory: layer 1's fragments are stored to a double buffer
+//              there, the chain's on-chip layers leave theirs in the region.  A consumer only arrives on "empty"; it
+//              never waits on it or issues a copy: such divergent code in the k-loop makes ptxas serialise the
+//              wgmmas (C7518), and the two consumers would wait for each other on every chunk.
 //
-// Operand layout (no swizzle, K-major): 8-row x 16-byte core matrices, 128 contiguous bytes each;
+// Shared-memory operand layout (no swizzle, K-major): 8-row x 16-byte core matrices, 128 contiguous bytes each;
 // for a 16-k chunk, core(row group g, k half kc) at g * 256 + kc * 128 (LBO = 128, SBO = 256).
 #include <algorithm>
 #include <atomic>
@@ -71,11 +75,11 @@ constexpr int kTileRows = 128;      // rows per tile (64 per consumer warpgroup)
 // more L1 for the gathered rows (GNN edge layer at the benchmark shape: 7.7 vs 8.0 ms, H100 SXM at a 400 W limit)
 constexpr int kMaxRing = 4;
 constexpr int kMaxNT = 304;         // widest padded N one launch covers
-constexpr uint32_t kABytes = 4096;  // one warpgroup's A chunk: hi (2048) + lo (2048), 64 rows x 16 k
+constexpr uint32_t kABytes = 4096;  // one warpgroup's shared-memory A chunk: hi (2048) + lo (2048), 64 rows x 16 k
 constexpr int kMaxChain = 6;        // on-chip pooling layers ahead of the kernel's own (edge MLPs have <= 8 layers)
 
-// shared memory of a CTA: a ring of W stages, one A region per consumer warpgroup (the double buffer of a streamed
-// layer, or a whole on-chip activation), the full / empty barriers
+// shared memory of a CTA: a ring of W stages, one A region per consumer warpgroup (POOL only: layer 1's double buffer,
+// or a whole on-chip activation; ROWS and GNN keep A in registers), the full / empty barriers
 constexpr size_t wg_smem_bytes(uint32_t stage_bytes, uint32_t region_bytes, int ring) {
   return size_t(ring) * stage_bytes + 2 * size_t(region_bytes) + 2 * ring * sizeof(uint64_t);
 }
@@ -127,9 +131,9 @@ struct WgParams {
   int ring_log2;            // POOL: log2 of the ring depth
 };
 
-__device__ __forceinline__ float4 ldg_nc(const float* ptr) {
-  float4 v;
-  asm volatile("ld.global.nc.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(ptr));
+__device__ __forceinline__ float2 ldg_nc(const float* ptr) {
+  float2 v;
+  asm volatile("ld.global.nc.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(ptr));
   return v;
 }
 
@@ -151,21 +155,17 @@ __device__ __forceinline__ void seg_flush(const WgParams& p, int d, int col, flo
   }
 }
 
-// w[0 .. 8) = ptr[0 .. 8); ptr is 32-byte aligned
-__device__ __forceinline__ void ldg8(const float* ptr, float (&w)[8]) {
-  const float4 a = __ldg(reinterpret_cast<const float4*>(ptr)), b = __ldg(reinterpret_cast<const float4*>(ptr) + 1);
-  w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w;
-  w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
-}
+// ptr[0 .. 2) through the read-only cache; ptr is 8-byte aligned
+__device__ __forceinline__ float2 ldg2(const float* ptr) { return __ldg(reinterpret_cast<const float2*>(ptr)); }
 
 template <int kProd, int kEpi, int NI, int NS, bool kAnyAct>
 __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
   constexpr int NT = NI * NS;
   constexpr uint32_t kChunkBytes = uint32_t(NT) * 64u;   // hi + lo, 16 k
-  constexpr int kRing = ring_stages(kChunkBytes, 2 * kABytes);
+  constexpr int kRing = ring_stages(kChunkBytes, 0);
   // the pooling chain sizes its ring stages and A regions for all of its layers (host side, launch_wg)
   const uint32_t stage_bytes = kProd == PROD_POOL ? p.stage_bytes : kChunkBytes;
-  const uint32_t region_bytes = kProd == PROD_POOL ? p.region_bytes : 2 * kABytes;
+  const uint32_t region_bytes = kProd == PROD_POOL ? p.region_bytes : 0;
   const int ring_log2 = kProd == PROD_POOL ? p.ring_log2 : log2_ring(kRing);
   const uint32_t ring_mask = (1u << ring_log2) - 1;
   extern __shared__ __align__(128) uint8_t smem[];
@@ -219,118 +219,166 @@ __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
     if (lane == 0) mbar_arrive(&empty[uint32_t(g) & ring_mask]);
   };
 
-  // A geometry: thread t writes 8 consecutive k (half kh) of row pr of its warpgroup's 64
-  const int pr = t >> 1, kh = t & 1;
-  const uint32_t a_off = uint32_t(pr >> 3) * 256u + uint32_t(kh) * 128u + uint32_t(pr & 7) * 16u;
   uint8_t* my_a = abuf + wgi * region_bytes;
   int64_t g = 0;
-  for (int64_t j = 0; j < my_tiles; ++j) {
-    const int64_t tile = blockIdx.x + j * gridDim.x;
-    const int64_t row = tile * kTileRows + wgi * 64 + pr;
-    const bool valid = row < p.num_rows;
-    // ---- row context -----------------------------------------------------------------------------
-    const float* rp = p.x;
-    float rx = 0.f, ry = 0.f, rz = 0.f, f0 = 0.f;
-    if (kProd == PROD_ROWS) {
-      if (valid) rp = p.x + row * int64_t(p.ldx);
-    } else if (valid) {
-      int si = __ldg(p.src + row), di = __ldg(p.dst + row);
-      if (si < 0 || si >= p.num_src || di < 0 || di >= p.num_dst) {
-        *p.err = 1;
-        si = 0;
-        di = 0;
+  for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    // ---- A fragment (wgmma_bf16_rs): thread t holds rows 16 warp + lane / 4 and + 8 of its warpgroup's 64, the rows of
+    // its accumulators, and k = 2 (lane % 4) + {0, 1, 8, 9} of every 16-k chunk.  The tile's streamed layer sets the
+    // rows' context.  ROWS: the rows of p.x;  GNN: the edges' source vertices, their rows of P (32 bits: two registers)
+    const float* rp[2];
+    uint32_t src_row[2];
+    float rx[2], ry[2], rz[2], f0[2];
+    auto row_context = [&]() {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t row = tile * kTileRows + wgi * 64 + warp * 16 + (lane >> 2) + 8 * h;
+        rp[h] = p.x;
+        src_row[h] = 0u;
+        rx[h] = ry[h] = rz[h] = f0[h] = 0.f;
+        if (row >= p.num_rows) continue;
+        if (kProd == PROD_ROWS) {
+          rp[h] = p.x + row * p.ldx;
+          continue;
+        }
+        int si = __ldg(p.src + row), di = __ldg(p.dst + row);
+        if (si < 0 || si >= p.num_src || di < 0 || di >= p.num_dst) {
+          *p.err = 1;
+          si = 0;
+          di = 0;
+        }
+        const int64_t drow = p.dst_index ? int64_t(__ldg(p.dst_index + di)) : int64_t(di);
+        rx[h] = __ldg(p.xyz_src + int64_t(si) * 3 + 0) - __ldg(p.xyz_dst + drow * 3 + 0);
+        ry[h] = __ldg(p.xyz_src + int64_t(si) * 3 + 1) - __ldg(p.xyz_dst + drow * 3 + 1);
+        rz[h] = __ldg(p.xyz_src + int64_t(si) * 3 + 2) - __ldg(p.xyz_dst + drow * 3 + 2);
+        if (kProd == PROD_GNN) src_row[h] = uint32_t(si);
+        else f0[h] = __ldg(p.feat + si);
       }
-      const int64_t drow = p.dst_index ? int64_t(__ldg(p.dst_index + di)) : int64_t(di);
-      rx = __ldg(p.xyz_src + int64_t(si) * 3 + 0) - __ldg(p.xyz_dst + drow * 3 + 0);
-      ry = __ldg(p.xyz_src + int64_t(si) * 3 + 1) - __ldg(p.xyz_dst + drow * 3 + 1);
-      rz = __ldg(p.xyz_src + int64_t(si) * 3 + 2) - __ldg(p.xyz_dst + drow * 3 + 2);
-      if (kProd == PROD_GNN) rp = p.x + int64_t(si) * p.ldx;
-      else f0 = __ldg(p.feat + si);
-    }
-    auto load = [&](int kc, float4 (&q)[2]) {
-      if (kProd == PROD_POOL) return;
-      const int k0 = kc * 16 + kh * 8;
-#pragma unroll
-      for (int i = 0; i < 2; ++i)
-        q[i] = (kProd == PROD_GNN || k0 + 4 * i + 4 <= p.k_real) ? ldg_nc(rp + k0 + 4 * i) : make_float4(0.f, 0.f, 0.f, 0.f);
     };
-    auto put = [&](int buf, const float4 (&q)[2], int kc) {
-      const int k0 = kc * 16 + kh * 8;
-      float v[8] = {q[0].x, q[0].y, q[0].z, q[0].w, q[1].x, q[1].y, q[1].z, q[1].w};
-      // w1x rows are kp (GNN) or ldx (POOL) floats long, a multiple of 16, so this thread's 8 k of every row are
-      // 32-byte aligned
-      if (kProd == PROD_GNN) {
-        float wx[8], wy[8], wz[8];
-        ldg8(p.w1x + k0, wx);
-        ldg8(p.w1x + p.kp + k0, wy);
-        ldg8(p.w1x + 2 * p.kp + k0, wz);
+    // the fp32 inputs of chunk kc's fragment: q[i] for register i, the thread's row i & 1, k kq + 8 (i >> 1) and + 1
+    auto load = [&](int kc, float2 (&q)[4]) {
+      if constexpr (kProd != PROD_POOL) {
 #pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] = layer_act<kAnyAct>(p.act, fmaf(rz, wz[i], fmaf(ry, wy[i], fmaf(rx, wx[i], v[i]))));
-      } else if (kProd == PROD_POOL) {
-        float wf[8], wx[8], wy[8], wz[8], b0[8];
-        ldg8(p.w1x + k0, wf);
-        ldg8(p.w1x + p.ldx + k0, wx);
-        ldg8(p.w1x + 2 * p.ldx + k0, wy);
-        ldg8(p.w1x + 3 * p.ldx + k0, wz);
-        ldg8(p.w1x + 4 * p.ldx + k0, b0);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          float a = b0[i];
-          a = fmaf(f0, wf[i], a);
-          a = fmaf(rx, wx[i], a);
-          a = fmaf(ry, wy[i], a);
-          a = fmaf(rz, wz[i], a);
-          v[i] = fmaxf(a, 0.0f);
+        for (int i = 0; i < 4; ++i) {
+          const int k = kc * 16 + (lane & 3) * 2 + 8 * (i >> 1);
+          q[i] = (kProd == PROD_GNN || k + 2 <= p.k_real)
+                     ? ldg_nc((kProd == PROD_GNN ? p.x + int64_t(src_row[i & 1]) * p.ldx : rp[i & 1]) + k)
+                     : make_float2(0.f, 0.f);
         }
       }
-      uint4 hi, lo;
-      split_bf16x2(v[0], v[1], &hi.x, &lo.x);
-      split_bf16x2(v[2], v[3], &hi.y, &lo.y);
-      split_bf16x2(v[4], v[5], &hi.z, &lo.z);
-      split_bf16x2(v[6], v[7], &hi.w, &lo.w);
-      uint8_t* dstp = my_a + buf * kABytes + a_off;
-      *reinterpret_cast<uint4*>(dstp) = hi;
-      *reinterpret_cast<uint4*>(dstp + kABytes / 2) = lo;
+    };
+    // chunk kc's fragment, split into hi / lo
+    auto make_frag = [&](const float2 (&q)[4], int kc, uint32_t (&hi)[4], uint32_t (&lo)[4]) {
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        const int k = kc * 16 + (lane & 3) * 2 + 8 * c;
+        float2 v[2] = {q[2 * c], q[2 * c + 1]};
+        // w1x rows are kp (GNN) or ldx (POOL) floats long, a multiple of 16, so this thread's pairs are 8-byte aligned
+        if (kProd == PROD_GNN) {
+          const float2 wx = ldg2(p.w1x + k), wy = ldg2(p.w1x + p.kp + k), wz = ldg2(p.w1x + 2 * p.kp + k);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            v[h].x = layer_act<kAnyAct>(p.act, fmaf(rz[h], wz.x, fmaf(ry[h], wy.x, fmaf(rx[h], wx.x, v[h].x))));
+            v[h].y = layer_act<kAnyAct>(p.act, fmaf(rz[h], wz.y, fmaf(ry[h], wy.y, fmaf(rx[h], wx.y, v[h].y))));
+          }
+        } else if (kProd == PROD_POOL) {
+          const float2 wf = ldg2(p.w1x + k), wx = ldg2(p.w1x + p.ldx + k), wy = ldg2(p.w1x + 2 * p.ldx + k),
+                       wz = ldg2(p.w1x + 3 * p.ldx + k), b0 = ldg2(p.w1x + 4 * p.ldx + k);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            v[h].x = fmaxf(fmaf(rz[h], wz.x, fmaf(ry[h], wy.x, fmaf(rx[h], wx.x, fmaf(f0[h], wf.x, b0.x)))), 0.0f);
+            v[h].y = fmaxf(fmaf(rz[h], wz.y, fmaf(ry[h], wy.y, fmaf(rx[h], wx.y, fmaf(f0[h], wf.y, b0.y)))), 0.0f);
+          }
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) split_bf16x2(v[h].x, v[h].y, &hi[2 * c + h], &lo[2 * c + h]);
+      }
     };
     // ---- one layer's loop over 16-k chunks into acc[ns][ni / 2] --------------------------------------
-    // streamed: A chunk kc is produced by load / put into a double buffer at the start of the region while chunk
-    // kc - 1's wgmmas run.  Otherwise the previous on-chip layer left the whole A in the region, chunk kc at
-    // kc * kABytes
+    // streamed: chunk kc + 1's A fragment is built while chunk kc's wgmmas run.  Otherwise the previous on-chip layer
+    // left the whole A in the region, chunk kc at kc * kABytes
     auto mma_layer = [&](auto& lacc, int lk, bool streamed) {
       using Acc = std::remove_reference_t<decltype(lacc)>;
       constexpr int ns = int(std::extent<Acc, 0>::value), ni = 2 * int(std::extent<Acc, 1>::value);
-      float4 q[2] = {make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f)};
-      if (streamed) {
-        load(0, q);
-        put(0, q, 0);
-        if (lk > 1) load(1, q);
-      }
-      for (int kc = 0; kc < lk; ++kc, ++g) {
-        if (streamed || kc == 0) {        // this warpgroup's A writes -> visible to its wgmmas
-          fence_proxy_async_smem();
-          warpgroup_sync(1 + wgi);
-        }
+      // chunk kc's wgmmas on W stage g, A hi / lo from registers (uint32_t[4]) or shared memory (descriptors).  Every
+      // chunk leaves exactly itself in flight: a wait on a path of its own (the last chunk's) would make ptxas drain
+      // the wgmmas at the end of every iteration
+      auto chunk = [&](int kc, const auto& a_hi, const auto& a_lo) {
         mbar_wait(&full[uint32_t(g) & ring_mask], uint32_t((g >> ring_log2) & 1));
         wgmma_fence();
-        const uint32_t a_base = smem_u32(my_a + uint32_t(streamed ? (kc & 1) : kc) * kABytes);
         const uint32_t b_base = smem_u32(bring + (uint32_t(g) & ring_mask) * stage_bytes);
-        const uint64_t a_hi = make_smem_desc(a_base, 128, 256), a_lo = make_smem_desc(a_base + kABytes / 2, 128, 256);
 #pragma unroll
         for (int i = 0; i < ns; ++i) {
           const uint64_t b_hi = make_smem_desc(b_base + uint32_t(i * ni) * 32u, 128, 256);
           const uint64_t b_lo = make_smem_desc(b_base + uint32_t(ni * ns) * 32u + uint32_t(i * ni) * 32u, 128, 256);
-          wgmma_bf16<ni>(lacc[i], a_hi, b_hi, kc > 0 ? 1 : 0);
-          wgmma_bf16<ni>(lacc[i], a_lo, b_hi, 1);
-          wgmma_bf16<ni>(lacc[i], a_hi, b_lo, 1);
+          if constexpr (std::is_same_v<std::decay_t<decltype(a_hi)>, uint64_t>) {
+            wgmma_bf16<ni>(lacc[i], a_hi, b_hi, kc > 0 ? 1 : 0);
+            wgmma_bf16<ni>(lacc[i], a_lo, b_hi, 1);
+            wgmma_bf16<ni>(lacc[i], a_hi, b_lo, 1);
+          } else {
+            wgmma_bf16_rs<ni>(lacc[i], a_hi, b_hi, kc > 0 ? 1 : 0);
+            wgmma_bf16_rs<ni>(lacc[i], a_lo, b_hi, 1);
+            wgmma_bf16_rs<ni>(lacc[i], a_hi, b_lo, 1);
+          }
         }
         wgmma_commit();
-        // every iteration leaves exactly chunk kc in flight: a wait on a path of its own (the last chunk's) would
-        // make ptxas drain the wgmmas at the end of every iteration
-        wgmma_wait<1>();                  // chunk kc - 1 complete: its A buffer and W stage are free
+        wgmma_wait<1>();                  // chunk kc - 1 complete: its A fragment and W stage are free
         if (kc > 0) release(g - 1);
-        if (streamed && kc + 1 < lk) {
-          put((kc + 1) & 1, q, kc + 1);
-          if (kc + 2 < lk) load(kc + 2, q);
+        ++g;
+      };
+      if (streamed && kProd != PROD_POOL) {
+        // a fragment may be written only once the wgmmas reading it are complete: two of them, alternating, and the
+        // loop unrolled by two so that each chunk's fragment registers are fixed at compile time.  The loads of chunk
+        // kc + 2 are issued before chunk kc + 1's wgmmas
+        float2 q[4] = {};
+        uint32_t ahi[2][4], alo[2][4];
+        row_context();
+        load(0, q);
+        make_frag(q, 0, ahi[0], alo[0]);
+        if (lk > 1) load(1, q);
+        auto step = [&](int kc, const uint32_t (&hi)[4], const uint32_t (&lo)[4], uint32_t (&next_hi)[4],
+                        uint32_t (&next_lo)[4]) {
+          chunk(kc, hi, lo);
+          if (kc + 1 < lk) {
+            make_frag(q, kc + 1, next_hi, next_lo);
+            if (kc + 2 < lk) load(kc + 2, q);
+          }
+        };
+        for (int kc = 0; kc < lk; kc += 2) {
+          step(kc, ahi[0], alo[0], ahi[1], alo[1]);
+          if (kc + 1 == lk) break;
+          step(kc + 1, ahi[1], alo[1], ahi[0], alo[0]);
+        }
+      } else if (streamed) {
+        // POOL layer 1: the fragments go through a double buffer at the start of the region, in to_region's layout,
+        // and the wgmmas read A from there.  With A in registers next to the on-chip layers' code, ptxas serialises
+        // the wgmmas of every POOL instance for want of registers (C7512)
+        row_context();
+        auto put = [&](int kc) {
+          float2 q[4] = {};
+          uint32_t hi[4], lo[4];
+          make_frag(q, kc, hi, lo);
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            uint8_t* dstp = my_a + uint32_t(kc & 1) * kABytes + uint32_t(warp * 2 + (i & 1)) * 256u +
+                            uint32_t(i >> 1) * 128u + uint32_t(lane >> 2) * 16u + uint32_t(lane & 3) * 4u;
+            *reinterpret_cast<uint32_t*>(dstp) = hi[i];
+            *reinterpret_cast<uint32_t*>(dstp + kABytes / 2) = lo[i];
+          }
+        };
+        put(0);
+        for (int kc = 0; kc < lk; ++kc) {
+          fence_proxy_async_smem();       // this warpgroup's A writes -> visible to its wgmmas
+          warpgroup_sync(1 + wgi);
+          const uint32_t a_base = smem_u32(my_a + uint32_t(kc & 1) * kABytes);
+          chunk(kc, make_smem_desc(a_base, 128, 256), make_smem_desc(a_base + kABytes / 2, 128, 256));
+          if (kc + 1 < lk) put(kc + 1);
+        }
+      } else {
+        fence_proxy_async_smem();         // this warpgroup's to_region writes -> visible to its wgmmas
+        warpgroup_sync(1 + wgi);
+        for (int kc = 0; kc < lk; ++kc) {
+          const uint32_t a_base = smem_u32(my_a + uint32_t(kc) * kABytes);
+          chunk(kc, make_smem_desc(a_base, 128, 256), make_smem_desc(a_base + kABytes / 2, 128, 256));
         }
       }
       wgmma_wait<0>();
@@ -551,7 +599,7 @@ WgShape wg_shape(int k, int n) {
   else if (t.np <= 256) { t.ni = 128; t.ns = 2; }
   else if (t.np <= kMaxNT) { t.ni = 152; t.ns = 2; }
   t.nt = t.ni * t.ns;
-  t.smem = wg_smem_bytes(uint32_t(t.nt) * 64u, 2 * kABytes, ring_stages(uint32_t(t.nt) * 64u, 2 * kABytes));
+  t.smem = wg_smem_bytes(uint32_t(t.nt) * 64u, 0, ring_stages(uint32_t(t.nt) * 64u, 0));
   t.ok = t.nt > 0 && k >= 1 && n >= 1;
   return t;
 }
