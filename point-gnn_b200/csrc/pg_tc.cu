@@ -1,8 +1,9 @@
 // Hopper tensor-core kernels (wgmma): the fast path (precision = 1, "BF16x3").
 //
-// wg_gemm_kernel - one persistent, warp-specialised kernel for every tensor-core layer of the network:
-//   out = epilogue(A @ W + b), W streamed by a producer warpgroup, A produced on the fly (in registers, or in shared
-//   memory for the pooling launches) by the two consumer warpgroups that also run the wgmmas.
+// wg_gemm_kernel - one persistent kernel for every tensor-core layer of the network: out = epilogue(A @ W + b), A
+//   produced on the fly (in registers, or in shared memory for the pooling launches) by the warpgroups that also run
+//   the wgmmas.  Dense and pooling layers stream W through a producer warpgroup; the GNN edge layer keeps its W
+//   resident in shared memory (mapping, below).
 //
 //   producers  PROD_ROWS  A = rows of an fp32 matrix (dense layers, a pooling layer wider than one launch)
 //              PROD_GNN   one GNN iteration's edge MLP (/root/reference/models/gnn.py:338-365) after hoisting:
@@ -26,13 +27,24 @@
 //              wg_gemm_kernel linear, then activate_rows
 //   precision  every fp32 operand is split x = hi + lo (two BF16), and hi*hi' + lo*hi' + hi*lo' is
 //              accumulated in fp32 registers: ~2^-16 relative per product (fp32-class accuracy)
-//   mapping    CTA = 3 warpgroups.  Warpgroup 0 is the W producer (setmaxnreg down to 24 registers): one thread
+//   mapping    GNN (wg_gnn_body): W resident.  A CTA owns one NI-wide column group c = blockIdx.x % NS of the padded
+//              output.  At kernel start one thread copies that group's hi and lo slices of every 16-k chunk (NI x 32 B
+//              each, straight out of the image layout below) into shared memory with cp.async.bulk on one mbarrier,
+//              which every thread waits on once: kp x NI x 4 B, 185 KB for the car layer (304 x 152).  W then stays
+//              for the whole launch: no ring, no per-chunk barrier, no producer warpgroup.  The three warpgroups
+//              are independent consumers of 64-row tiles (tiles 3 j + wg of CTA slot j = blockIdx.x / NS, stepping by
+//              3 gridDim.x / NS), one m64nNIk16 accumulator each, A in registers as below.  Nothing makes one
+//              warpgroup wait for another, so while one flushes its segment max the other two keep the tensor cores
+//              busy.  Every output column gets the same wgmmas on the same operands in the same order as with the
+//              whole N in one warpgroup, so the results do not depend on the grouping.  Both column groups gather the
+//              same P rows (twice the gather, against a W stream of 370 KB per 128-row tile).
+//              ROWS and POOL: CTA = 3 warpgroups.  Warpgroup 0 is the W producer (setmaxnreg down to 24 registers): one thread
 //              streams W (hi and lo images, pre-packed in the no-swizzle K-major core-matrix layout, one
 //              contiguous block per 16-k chunk) from L2 through a ring of shared-memory stages with
 //              cp.async.bulk, each stage tracked by a "full" (bytes landed) and an "empty" (both consumers done)
 //              mbarrier.  Warpgroups 1 and 2 are the consumers (setmaxnreg up to 240): 128 rows per tile (64 per
 //              warpgroup), the whole padded N (<= 304: two m64nNk16 instructions) in registers.  A streamed ROWS
-//              or GNN layer takes A from registers (wgmma_bf16_rs): each thread builds its own fragment of a chunk (its
+//              layer, like the GNN layer, takes A from registers (wgmma_bf16_rs): each thread builds its own fragment of a chunk (its
 //              accumulators' two rows, 4 k) from its gathered fp32 values, in one of two alternating register
 //              buffers, issuing the global loads of chunk k + 2 before the wgmmas of chunk k + 1 and building
 //              chunk k + 1 while chunk k's wgmmas run: no shared-memory A, proxy fence or barrier per chunk.  The
@@ -67,7 +79,7 @@ namespace pg {
 namespace {
 using namespace wg;
 
-constexpr int kWgThreads = 384;     // warpgroup 0 streams W, warpgroups 1 and 2 compute
+constexpr int kWgThreads = 384;     // dense / pooling: warpgroup 0 streams W, 1 and 2 compute;  GNN: all three compute
 constexpr int kProducerRegs = 24;   // 2 x 128 x 240 + 128 x 24 = 384 x 168, the launch bound's budget
 constexpr int kConsumerRegs = 240;  // 232 spills 8 bytes in the 152 x 2 segment-max instances
 constexpr int kTileRows = 128;      // rows per tile (64 per consumer warpgroup)
@@ -90,6 +102,13 @@ constexpr int ring_stages(uint32_t stage_bytes, uint32_t region_bytes) {
   return r;
 }
 constexpr int log2_ring(int r) { return r >= 4 ? 2 : r >= 2 ? 1 : 0; }
+
+// GNN edge layer (wg_gnn_body): every warpgroup of a CTA computes its own 64-row tiles against the CTA's resident
+// column group of W
+constexpr int kGnnWarpgroups = kWgThreads / 128;
+constexpr int kGnnTileRows = 64;
+// shared memory of a GNN CTA: its column group of W (ni columns, hi + lo, kp k), then the mbarrier
+constexpr size_t gnn_smem_bytes(int kp, int ni) { return size_t(kp) * ni * 4 + sizeof(uint64_t); }
 
 enum { PROD_ROWS = 0, PROD_GNN = 1, PROD_POOL = 2 };
 enum { EPI_STORE = 0, EPI_SEGMAX = 1 };
@@ -158,8 +177,256 @@ __device__ __forceinline__ void seg_flush(const WgParams& p, int d, int col, flo
 // ptr[0 .. 2) through the read-only cache; ptr is 8-byte aligned
 __device__ __forceinline__ float2 ldg2(const float* ptr) { return __ldg(reinterpret_cast<const float2*>(ptr)); }
 
-template <int kProd, int kEpi, int NI, int NS, bool kAnyAct>
+// A rows in registers (wgmma_bf16_rs): thread t of a warpgroup holds rows 16 warp + lane / 4 and + 8 of its 64, the
+// rows of its accumulators, and k = 2 (lane % 4) + {0, 1, 8, 9} of every 16-k chunk.  context() reads what the rows
+// need once per tile.  ROWS: the rows of p.x;  GNN: the edges' source vertices, their rows of P (32 bits: two
+// registers), and x_src - x_dst';  POOL: the same offset and the source's feature
+template <int kProd, bool kAnyAct>
+struct RowA {
+  const float* rp[2];
+  uint32_t src_row[2];
+  float rx[2], ry[2], rz[2], f0[2];
+
+  // rows row0 + 16 warp + lane / 4 (+ 8) of the layer's A
+  __device__ __forceinline__ void context(const WgParams& p, int64_t row0, int warp, int lane) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t row = row0 + warp * 16 + (lane >> 2) + 8 * h;
+      rp[h] = p.x;
+      src_row[h] = 0u;
+      rx[h] = ry[h] = rz[h] = f0[h] = 0.f;
+      if (row >= p.num_rows) continue;
+      if (kProd == PROD_ROWS) {
+        rp[h] = p.x + row * p.ldx;
+        continue;
+      }
+      int si = __ldg(p.src + row), di = __ldg(p.dst + row);
+      if (si < 0 || si >= p.num_src || di < 0 || di >= p.num_dst) {
+        *p.err = 1;
+        si = 0;
+        di = 0;
+      }
+      const int64_t drow = p.dst_index ? int64_t(__ldg(p.dst_index + di)) : int64_t(di);
+      rx[h] = __ldg(p.xyz_src + int64_t(si) * 3 + 0) - __ldg(p.xyz_dst + drow * 3 + 0);
+      ry[h] = __ldg(p.xyz_src + int64_t(si) * 3 + 1) - __ldg(p.xyz_dst + drow * 3 + 1);
+      rz[h] = __ldg(p.xyz_src + int64_t(si) * 3 + 2) - __ldg(p.xyz_dst + drow * 3 + 2);
+      if (kProd == PROD_GNN) src_row[h] = uint32_t(si);
+      else f0[h] = __ldg(p.feat + si);
+    }
+  }
+  // the fp32 inputs of chunk kc's fragment: q[i] for register i, the thread's row i & 1, k kq + 8 (i >> 1) and + 1
+  __device__ __forceinline__ void load(const WgParams& p, int kc, int lane, float2 (&q)[4]) const {
+    if constexpr (kProd != PROD_POOL) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int k = kc * 16 + (lane & 3) * 2 + 8 * (i >> 1);
+        q[i] = (kProd == PROD_GNN || k + 2 <= p.k_real)
+                   ? ldg_nc((kProd == PROD_GNN ? p.x + int64_t(src_row[i & 1]) * p.ldx : rp[i & 1]) + k)
+                   : make_float2(0.f, 0.f);
+      }
+    }
+  }
+  // chunk kc's fragment, split into hi / lo
+  __device__ __forceinline__ void make_frag(const WgParams& p, const float2 (&q)[4], int kc, int lane, uint32_t (&hi)[4],
+                                            uint32_t (&lo)[4]) const {
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+      const int k = kc * 16 + (lane & 3) * 2 + 8 * c;
+      float2 v[2] = {q[2 * c], q[2 * c + 1]};
+      // w1x rows are kp (GNN) or ldx (POOL) floats long, a multiple of 16, so this thread's pairs are 8-byte aligned
+      if (kProd == PROD_GNN) {
+        const float2 wx = ldg2(p.w1x + k), wy = ldg2(p.w1x + p.kp + k), wz = ldg2(p.w1x + 2 * p.kp + k);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          v[h].x = layer_act<kAnyAct>(p.act, fmaf(rz[h], wz.x, fmaf(ry[h], wy.x, fmaf(rx[h], wx.x, v[h].x))));
+          v[h].y = layer_act<kAnyAct>(p.act, fmaf(rz[h], wz.y, fmaf(ry[h], wy.y, fmaf(rx[h], wx.y, v[h].y))));
+        }
+      } else if (kProd == PROD_POOL) {
+        const float2 wf = ldg2(p.w1x + k), wx = ldg2(p.w1x + p.ldx + k), wy = ldg2(p.w1x + 2 * p.ldx + k),
+                     wz = ldg2(p.w1x + 3 * p.ldx + k), b0 = ldg2(p.w1x + 4 * p.ldx + k);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          v[h].x = fmaxf(fmaf(rz[h], wz.x, fmaf(ry[h], wy.x, fmaf(rx[h], wx.x, fmaf(f0[h], wf.x, b0.x)))), 0.0f);
+          v[h].y = fmaxf(fmaf(rz[h], wz.y, fmaf(ry[h], wy.y, fmaf(rx[h], wx.y, fmaf(f0[h], wf.y, b0.y)))), 0.0f);
+        }
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) split_bf16x2(v[h].x, v[h].y, &hi[2 * c + h], &lo[2 * c + h]);
+    }
+  }
+};
+
+// The k-loop of a layer whose A fragments are built in registers: chunk(kc, hi, lo) issues chunk kc's wgmmas and
+// leaves exactly itself in flight.  A fragment may be written only once the wgmmas reading it are complete: two of
+// them, alternating, and the loop unrolled by two so that each chunk's fragment registers are fixed at compile time.
+// Chunk kc + 1's fragment is built while chunk kc's wgmmas run, and the loads of chunk kc + 2 are issued before chunk
+// kc + 1's wgmmas
+template <class A, class Chunk>
+__device__ __forceinline__ void rs_k_loop(const WgParams& p, const A& a, int lk, int lane, Chunk&& chunk) {
+  float2 q[4] = {};
+  uint32_t ahi[2][4], alo[2][4];
+  a.load(p, 0, lane, q);
+  a.make_frag(p, q, 0, lane, ahi[0], alo[0]);
+  if (lk > 1) a.load(p, 1, lane, q);
+  auto step = [&](int kc, const uint32_t (&hi)[4], const uint32_t (&lo)[4], uint32_t (&next_hi)[4],
+                  uint32_t (&next_lo)[4]) {
+    chunk(kc, hi, lo);
+    if (kc + 1 < lk) {
+      a.make_frag(p, q, kc + 1, lane, next_hi, next_lo);
+      if (kc + 2 < lk) a.load(p, kc + 2, lane, q);
+    }
+  };
+  for (int kc = 0; kc < lk; kc += 2) {
+    step(kc, ahi[0], alo[0], ahi[1], alo[1]);
+    if (kc + 1 == lk) break;
+    step(kc + 1, ahi[1], alo[1], ahi[0], alo[0]);
+  }
+}
+
+// Segment max of one warpgroup's 64 x (NI x NS) accumulators: output columns col0 + [0, NI x NS), rows r0 (the
+// thread's first, as in RowA) and r0 + 8
+template <int NI, int NS, bool kAnyAct>
+__device__ __forceinline__ void seg_epilogue(const WgParams& p, const float (&acc)[NS][NI / 2], int64_t r0, int lane,
+                                             int col0) {
+  const int cq = (lane & 3) * 2;
+  int d[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int64_t r = r0 + 8 * h;
+    d[h] = -1;
+    if (r < p.num_rows) {
+      d[h] = __ldg(p.dst + r);
+      if (d[h] < 0 || d[h] >= p.num_dst) {
+        *p.err = 1;
+        d[h] = -1;
+      }
+    }
+  }
+  const int dw = __shfl_sync(0xffffffffu, d[0], 0);
+  if (__all_sync(0xffffffffu, d[0] == dw && d[1] == dw) && dw >= 0) {
+    // the warp's 16 rows are one destination.  Value v of a thread is column (v / 2) * 8 + cq + v % 2; the 8
+    // lanes sharing cq (lane bits 4, 3, 2) reduce-scatter their V values in three halving exchanges, after which
+    // every lane holds the full maxima of V / 8 (rounded up or down) of them and all 32 lanes flush.  V is padded with
+    // -FLT_MAX values to VP, a multiple of 4, so that the first two exchanges halve evenly (V = 38 at NI = 152, NS = 1)
+    constexpr int V = NI * NS / 4, VP = (V + 3) / 4 * 4, L1 = VP / 2, L2 = VP / 4, L3 = (L2 + 1) / 2;
+    float m[VP];
+#pragma unroll
+    for (int i = 0; i < NS; ++i)
+#pragma unroll
+      for (int jj = 0; jj < NI / 8; ++jj)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) m[(i * (NI / 8) + jj) * 2 + c] = fmaxf(acc[i][4 * jj + c], acc[i][4 * jj + 2 + c]);
+#pragma unroll
+    for (int v = V; v < VP; ++v) m[v] = -FLT_MAX;
+    const bool b4 = lane & 16, b3 = lane & 8, b2 = lane & 4;
+    // a lane with the bit set keeps the upper part, its partner the lower; each sends the part it gives up
+#pragma unroll
+    for (int k = 0; k < L1; ++k) {
+      const float keep = b4 ? m[k + L1] : m[k], give = b4 ? m[k] : m[k + L1];
+      m[k] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, give, 16));
+    }
+#pragma unroll
+    for (int k = 0; k < L2; ++k) {
+      const float keep = b3 ? m[k + L2] : m[k], give = b3 ? m[k] : m[k + L2];
+      m[k] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, give, 8));
+    }
+#pragma unroll
+    for (int k = 0; k < L3; ++k) {
+      const float up = k + L3 < L2 ? m[k + L3] : m[k];   // L2 odd: the upper part is one value shorter
+      const float keep = b2 ? up : m[k], give = b2 ? m[k] : up;
+      m[k] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, give, 4));
+    }
+    const int v0 = (b4 ? L1 : 0) + (b3 ? L2 : 0) + (b2 ? L3 : 0), nv = b2 ? L2 - L3 : L3;
+#pragma unroll
+    for (int k = 0; k < L3; ++k) {
+      const int v = v0 + k, col = col0 + (v >> 1) * 8 + cq + (v & 1);
+      if (k < nv && v < V && col < p.n) seg_flush<kAnyAct>(p, dw, col, m[k]);
+    }
+  } else {
+    // segmented max down each 8-row half (rows of one destination are contiguous); the first row of
+    // every run flushes the run's max.  Column by column, both halves: each accumulator dies once used
+    bool head[2];
+    bool same[2][3];   // the row 4 << s lanes down has the same destination
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int up = __shfl_up_sync(0xffffffffu, d[h], 4);
+      head[h] = d[h] >= 0 && (lane < 4 || up != d[h]);
+#pragma unroll
+      for (int s = 0; s < 3; ++s)
+        same[h][s] = __shfl_down_sync(0xffffffffu, d[h], 4 << s) == d[h] && lane + (4 << s) < 32;
+    }
+#pragma unroll
+    for (int i = 0; i < NS; ++i)
+#pragma unroll
+      for (int jj = 0; jj < NI / 8; ++jj)
+#pragma unroll
+        for (int c = 0; c < 2; ++c)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float m = acc[i][4 * jj + 2 * h + c];
+#pragma unroll
+            for (int s = 0; s < 3; ++s) {
+              const float o = __shfl_down_sync(0xffffffffu, m, 4 << s);
+              if (same[h][s]) m = fmaxf(m, o);
+            }
+            const int col = col0 + i * NI + jj * 8 + cq + c;
+            if (head[h] && col < p.n) seg_flush<kAnyAct>(p, d[h], col, m);
+          }
+  }
+}
+
+// ---- GNN edge layer: W resident, three independent consumer warpgroups (header, "mapping") -----------------------
+template <int NI, int NS, bool kAnyAct>
+__device__ __forceinline__ void wg_gnn_body(const WgParams& p) {
+  constexpr int NT = NI * NS;
+  constexpr uint32_t kSlice = uint32_t(NI) * 32u;   // one group's hi (or lo) part of a 16-k chunk
+  extern __shared__ __align__(128) uint8_t smem[];  // [nchunks][hi | lo][NI rows x 16 k], then the mbarrier
+  const int nk = p.nchunks;
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + size_t(nk) * 2 * kSlice);
+  const int tid = threadIdx.x;
+  const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);   // warpgroup, warp-uniform by construction
+  const int group = int(blockIdx.x) % NS;
+  if (tid == 0) {
+    mbar_init(full, 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  if (tid == 0) {
+    mbar_arrive_expect_tx(full, uint32_t(nk) * 2u * kSlice);
+    for (int kc = 0; kc < nk; ++kc)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        bulk_g2s(smem + (size_t(kc) * 2 + h) * kSlice,
+                 p.bimg + size_t(kc) * NT * 64 + size_t(h) * NT * 32 + size_t(group) * kSlice, kSlice, full);
+  }
+  mbar_wait(full, 0);
+  const int warp = (tid & 127) >> 5, lane = tid & 31;
+  const uint32_t w_base = smem_u32(smem);
+  const int num_tiles = int(p.num_tiles), stride = kGnnWarpgroups * int(gridDim.x / NS);
+  for (int tile = kGnnWarpgroups * int(blockIdx.x / NS) + wg; tile < num_tiles; tile += stride) {
+    const int64_t row0 = int64_t(tile) * kGnnTileRows;
+    RowA<PROD_GNN, kAnyAct> a;
+    a.context(p, row0, warp, lane);
+    float acc[1][NI / 2];
+    rs_k_loop(p, a, nk, lane, [&](int kc, const uint32_t (&hi)[4], const uint32_t (&lo)[4]) {
+      wgmma_fence();
+      const uint32_t b = w_base + uint32_t(kc) * 2u * kSlice;
+      const uint64_t b_hi = make_smem_desc(b, 128, 256), b_lo = make_smem_desc(b + kSlice, 128, 256);
+      wgmma_bf16_rs<NI>(acc[0], hi, b_hi, kc > 0 ? 1 : 0);
+      wgmma_bf16_rs<NI>(acc[0], lo, b_hi, 1);
+      wgmma_bf16_rs<NI>(acc[0], hi, b_lo, 1);
+      wgmma_commit();
+      wgmma_wait<1>();                    // chunk kc - 1 complete: its A fragment is free
+    });
+    wgmma_wait<0>();
+    seg_epilogue<NI, 1, kAnyAct>(p, acc, row0 + warp * 16 + (lane >> 2), lane, group * NI);
+  }
+}
+
+// ---- dense and pooling layers: W streamed by a producer warpgroup --------------------------------------------------
+template <int kProd, int kEpi, int NI, int NS>
 __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
+  static_assert(kProd != PROD_GNN, "the GNN edge layer runs wg_gnn_body");
   constexpr int NT = NI * NS;
   constexpr uint32_t kChunkBytes = uint32_t(NT) * 64u;   // hi + lo, 16 k
   constexpr int kRing = ring_stages(kChunkBytes, 0);
@@ -222,77 +489,9 @@ __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
   uint8_t* my_a = abuf + wgi * region_bytes;
   int64_t g = 0;
   for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-    // ---- A fragment (wgmma_bf16_rs): thread t holds rows 16 warp + lane / 4 and + 8 of its warpgroup's 64, the rows of
-    // its accumulators, and k = 2 (lane % 4) + {0, 1, 8, 9} of every 16-k chunk.  The tile's streamed layer sets the
-    // rows' context.  ROWS: the rows of p.x;  GNN: the edges' source vertices, their rows of P (32 bits: two registers)
-    const float* rp[2];
-    uint32_t src_row[2];
-    float rx[2], ry[2], rz[2], f0[2];
-    auto row_context = [&]() {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int64_t row = tile * kTileRows + wgi * 64 + warp * 16 + (lane >> 2) + 8 * h;
-        rp[h] = p.x;
-        src_row[h] = 0u;
-        rx[h] = ry[h] = rz[h] = f0[h] = 0.f;
-        if (row >= p.num_rows) continue;
-        if (kProd == PROD_ROWS) {
-          rp[h] = p.x + row * p.ldx;
-          continue;
-        }
-        int si = __ldg(p.src + row), di = __ldg(p.dst + row);
-        if (si < 0 || si >= p.num_src || di < 0 || di >= p.num_dst) {
-          *p.err = 1;
-          si = 0;
-          di = 0;
-        }
-        const int64_t drow = p.dst_index ? int64_t(__ldg(p.dst_index + di)) : int64_t(di);
-        rx[h] = __ldg(p.xyz_src + int64_t(si) * 3 + 0) - __ldg(p.xyz_dst + drow * 3 + 0);
-        ry[h] = __ldg(p.xyz_src + int64_t(si) * 3 + 1) - __ldg(p.xyz_dst + drow * 3 + 1);
-        rz[h] = __ldg(p.xyz_src + int64_t(si) * 3 + 2) - __ldg(p.xyz_dst + drow * 3 + 2);
-        if (kProd == PROD_GNN) src_row[h] = uint32_t(si);
-        else f0[h] = __ldg(p.feat + si);
-      }
-    };
-    // the fp32 inputs of chunk kc's fragment: q[i] for register i, the thread's row i & 1, k kq + 8 (i >> 1) and + 1
-    auto load = [&](int kc, float2 (&q)[4]) {
-      if constexpr (kProd != PROD_POOL) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int k = kc * 16 + (lane & 3) * 2 + 8 * (i >> 1);
-          q[i] = (kProd == PROD_GNN || k + 2 <= p.k_real)
-                     ? ldg_nc((kProd == PROD_GNN ? p.x + int64_t(src_row[i & 1]) * p.ldx : rp[i & 1]) + k)
-                     : make_float2(0.f, 0.f);
-        }
-      }
-    };
-    // chunk kc's fragment, split into hi / lo
-    auto make_frag = [&](const float2 (&q)[4], int kc, uint32_t (&hi)[4], uint32_t (&lo)[4]) {
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        const int k = kc * 16 + (lane & 3) * 2 + 8 * c;
-        float2 v[2] = {q[2 * c], q[2 * c + 1]};
-        // w1x rows are kp (GNN) or ldx (POOL) floats long, a multiple of 16, so this thread's pairs are 8-byte aligned
-        if (kProd == PROD_GNN) {
-          const float2 wx = ldg2(p.w1x + k), wy = ldg2(p.w1x + p.kp + k), wz = ldg2(p.w1x + 2 * p.kp + k);
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            v[h].x = layer_act<kAnyAct>(p.act, fmaf(rz[h], wz.x, fmaf(ry[h], wy.x, fmaf(rx[h], wx.x, v[h].x))));
-            v[h].y = layer_act<kAnyAct>(p.act, fmaf(rz[h], wz.y, fmaf(ry[h], wy.y, fmaf(rx[h], wx.y, v[h].y))));
-          }
-        } else if (kProd == PROD_POOL) {
-          const float2 wf = ldg2(p.w1x + k), wx = ldg2(p.w1x + p.ldx + k), wy = ldg2(p.w1x + 2 * p.ldx + k),
-                       wz = ldg2(p.w1x + 3 * p.ldx + k), b0 = ldg2(p.w1x + 4 * p.ldx + k);
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            v[h].x = fmaxf(fmaf(rz[h], wz.x, fmaf(ry[h], wy.x, fmaf(rx[h], wx.x, fmaf(f0[h], wf.x, b0.x)))), 0.0f);
-            v[h].y = fmaxf(fmaf(rz[h], wz.y, fmaf(ry[h], wy.y, fmaf(rx[h], wx.y, fmaf(f0[h], wf.y, b0.y)))), 0.0f);
-          }
-        }
-#pragma unroll
-        for (int h = 0; h < 2; ++h) split_bf16x2(v[h].x, v[h].y, &hi[2 * c + h], &lo[2 * c + h]);
-      }
-    };
+    // ---- A: the tile's streamed layer sets the rows' context (RowA)
+    RowA<kProd, false> a;
+    const int64_t row0 = tile * kTileRows + wgi * 64;
     // ---- one layer's loop over 16-k chunks into acc[ns][ni / 2] --------------------------------------
     // streamed: chunk kc + 1's A fragment is built while chunk kc's wgmmas run.  Otherwise the previous on-chip layer
     // left the whole A in the region, chunk kc at kc * kABytes
@@ -326,37 +525,17 @@ __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
         ++g;
       };
       if (streamed && kProd != PROD_POOL) {
-        // a fragment may be written only once the wgmmas reading it are complete: two of them, alternating, and the
-        // loop unrolled by two so that each chunk's fragment registers are fixed at compile time.  The loads of chunk
-        // kc + 2 are issued before chunk kc + 1's wgmmas
-        float2 q[4] = {};
-        uint32_t ahi[2][4], alo[2][4];
-        row_context();
-        load(0, q);
-        make_frag(q, 0, ahi[0], alo[0]);
-        if (lk > 1) load(1, q);
-        auto step = [&](int kc, const uint32_t (&hi)[4], const uint32_t (&lo)[4], uint32_t (&next_hi)[4],
-                        uint32_t (&next_lo)[4]) {
-          chunk(kc, hi, lo);
-          if (kc + 1 < lk) {
-            make_frag(q, kc + 1, next_hi, next_lo);
-            if (kc + 2 < lk) load(kc + 2, q);
-          }
-        };
-        for (int kc = 0; kc < lk; kc += 2) {
-          step(kc, ahi[0], alo[0], ahi[1], alo[1]);
-          if (kc + 1 == lk) break;
-          step(kc + 1, ahi[1], alo[1], ahi[0], alo[0]);
-        }
+        a.context(p, row0, warp, lane);
+        rs_k_loop(p, a, lk, lane, chunk);
       } else if (streamed) {
         // POOL layer 1: the fragments go through a double buffer at the start of the region, in to_region's layout,
         // and the wgmmas read A from there.  With A in registers next to the on-chip layers' code, ptxas serialises
         // the wgmmas of every POOL instance for want of registers (C7512)
-        row_context();
+        a.context(p, row0, warp, lane);
         auto put = [&](int kc) {
           float2 q[4] = {};
           uint32_t hi[4], lo[4];
-          make_frag(q, kc, hi, lo);
+          a.make_frag(p, q, kc, lane, hi, lo);
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
             uint8_t* dstp = my_a + uint32_t(kc & 1) * kABytes + uint32_t(warp * 2 + (i & 1)) * 256u +
@@ -457,102 +636,26 @@ __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
             }
       }
     } else {
-      int d[2];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int64_t r = r0 + 8 * h;
-        d[h] = -1;
-        if (r < p.num_rows) {
-          d[h] = __ldg(p.dst + r);
-          if (d[h] < 0 || d[h] >= p.num_dst) {
-            *p.err = 1;
-            d[h] = -1;
-          }
-        }
-      }
-      const int dw = __shfl_sync(0xffffffffu, d[0], 0);
-      if (__all_sync(0xffffffffu, d[0] == dw && d[1] == dw) && dw >= 0) {
-        // the warp's 16 rows are one destination.  Value v of a thread is column (v / 2) * 8 + cq + v % 2; the 8
-        // lanes sharing cq (lane bits 4, 3, 2) reduce-scatter their V values in three halving exchanges, after which
-        // every lane holds the full maxima of V / 8 (rounded up or down) of them and all 32 lanes flush
-        constexpr int V = NT / 4, L1 = V / 2, L2 = V / 4, L3 = (L2 + 1) / 2;
-        static_assert(V % 4 == 0, "the first two exchanges halve evenly");
-        float m[V];
-#pragma unroll
-        for (int i = 0; i < NS; ++i)
-#pragma unroll
-          for (int jj = 0; jj < NI / 8; ++jj)
-#pragma unroll
-            for (int c = 0; c < 2; ++c) m[(i * (NI / 8) + jj) * 2 + c] = fmaxf(acc[i][4 * jj + c], acc[i][4 * jj + 2 + c]);
-        const bool b4 = lane & 16, b3 = lane & 8, b2 = lane & 4;
-        // a lane with the bit set keeps the upper part, its partner the lower; each sends the part it gives up
-#pragma unroll
-        for (int k = 0; k < L1; ++k) {
-          const float keep = b4 ? m[k + L1] : m[k], give = b4 ? m[k] : m[k + L1];
-          m[k] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, give, 16));
-        }
-#pragma unroll
-        for (int k = 0; k < L2; ++k) {
-          const float keep = b3 ? m[k + L2] : m[k], give = b3 ? m[k] : m[k + L2];
-          m[k] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, give, 8));
-        }
-#pragma unroll
-        for (int k = 0; k < L3; ++k) {
-          const float up = k + L3 < L2 ? m[k + L3] : m[k];   // L2 odd: the upper part is one value shorter
-          const float keep = b2 ? up : m[k], give = b2 ? m[k] : up;
-          m[k] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, give, 4));
-        }
-        const int v0 = (b4 ? L1 : 0) + (b3 ? L2 : 0) + (b2 ? L3 : 0), nv = b2 ? L2 - L3 : L3;
-#pragma unroll
-        for (int k = 0; k < L3; ++k) {
-          const int v = v0 + k, col = (v >> 1) * 8 + cq + (v & 1);
-          if (k < nv && col < p.n) seg_flush<kAnyAct>(p, dw, col, m[k]);
-        }
-      } else {
-        // segmented max down each 8-row half (rows of one destination are contiguous); the first row of
-        // every run flushes the run's max
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int dd = d[h];
-          const int up = __shfl_up_sync(0xffffffffu, dd, 4);
-          const bool head = dd >= 0 && (lane < 4 || up != dd);
-          int dn[3];
-#pragma unroll
-          for (int s = 0; s < 3; ++s) {
-            dn[s] = __shfl_down_sync(0xffffffffu, dd, 4 << s);
-            if (lane + (4 << s) >= 32) dn[s] = -2;
-          }
-#pragma unroll
-          for (int i = 0; i < NS; ++i)
-#pragma unroll
-            for (int jj = 0; jj < NI / 8; ++jj)
-#pragma unroll
-              for (int c = 0; c < 2; ++c) {
-                float m = acc[i][4 * jj + 2 * h + c];
-#pragma unroll
-                for (int s = 0; s < 3; ++s) {
-                  const float o = __shfl_down_sync(0xffffffffu, m, 4 << s);
-                  if (dn[s] == dd) m = fmaxf(m, o);
-                }
-                const int col = i * NI + jj * 8 + cq + c;
-                if (head && col < p.n) seg_flush<kAnyAct>(p, dd, col, m);
-              }
-        }
-      }
+      seg_epilogue<NI, NS, false>(p, acc, r0, lane, 0);
     }
   }
 }
 
 template <int kProd, int kEpi, int NI, int NS>
 __global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
-  wg_gemm_body<kProd, kEpi, NI, NS, false>(p);
+  if constexpr (kProd == PROD_GNN) {
+    static_assert(kEpi == EPI_SEGMAX, "the GNN edge layer ends in the segment max");
+    wg_gnn_body<NI, NS, false>(p);
+  } else {
+    wg_gemm_body<kProd, kEpi, NI, NS>(p);
+  }
 }
 
 // its own name, so that the instance count and the ptxas properties of wg_gemm_kernel stay those of the ReLU build
 template <int kProd, int kEpi, int NI, int NS>
 __global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_act_kernel(WgParams p) {
   static_assert(kProd == PROD_GNN && kEpi == EPI_SEGMAX, "any-activation instances: the GNN edge layer only");
-  wg_gemm_body<kProd, kEpi, NI, NS, true>(p);
+  wg_gnn_body<NI, NS, true>(p);
 }
 
 // ---- W [K, N] -> streamed B image ---------------------------------------------------------------
@@ -677,12 +780,16 @@ int launch_wg_cfg(const WgParams& p, size_t smem, cudaStream_t s) {
   }
   static bool attr_done[2] = {false, false};
   if (!attr_done[any_act]) {
-    // a pooling chain's footprint depends on its layers, not only on the instance
+    // a pooling chain's footprint depends on its layers, a GNN launch's on its K, not only on the instance
     PG_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    int(kProd != PROD_POOL && smem < 48 * 1024 ? 48 * 1024 : 227 * 1024)));
+                                    int(kProd == PROD_ROWS && smem < 48 * 1024 ? 48 * 1024 : 227 * 1024)));
     attr_done[any_act] = true;
   }
-  const int grid = int(std::min<int64_t>(p.num_tiles, num_sms()));
+  int grid = int(std::min<int64_t>(p.num_tiles, num_sms()));
+  // GNN: one CTA per column group and slot, each slot taking kGnnWarpgroups tiles at a time: the largest multiple of
+  // NS up to the SM count, and no more slots than the tiles need
+  if constexpr (kProd == PROD_GNN)
+    grid = int(std::min<int64_t>(num_sms() / NS, ceil_div(p.num_tiles, kGnnWarpgroups))) * NS;
   kernel<<<grid, kWgThreads, smem, s>>>(p);
   PG_LAUNCH_CHECK();
   g_tc_launches[kEpi == EPI_SEGMAX ? 0 : 1].fetch_add(1, std::memory_order_relaxed);
@@ -716,6 +823,10 @@ int launch_wg(WgParams p, const PreparedGemm& g, cudaStream_t s, const PoolChain
     p.ring_log2 = log2_ring(ring);
     smem = wg_smem_bytes(p.stage_bytes, p.region_bytes, ring);
   }
+  if (kProd == PROD_GNN) {
+    p.num_tiles = ceil_div(p.num_rows, kGnnTileRows);
+    smem = gnn_smem_bytes(g.t.kp, g.t.ni);
+  }
   PG_REQUIRE(smem <= 227 * 1024, "tensor-core kernel needs %zu B of shared memory", smem);
   switch (g.t.ni * 4 + g.t.ns) {
     case 64 * 4 + 1: return launch_wg_cfg<kProd, kEpi, 64, 1>(p, smem, s);
@@ -729,10 +840,10 @@ int launch_wg(WgParams p, const PreparedGemm& g, cudaStream_t s, const PoolChain
   return PG_OK;
 }
 
-// column blocks of at most kMaxNT (multiples of 16) covering n
-std::vector<int> column_blocks(int n) {
+// column blocks of at most max_w (multiples of 16) covering n
+std::vector<int> column_blocks(int n, int max_w = kMaxNT) {
   std::vector<int> c0;
-  const int nb = int(ceil_div(n, kMaxNT));
+  const int nb = int(ceil_div(n, max_w));
   const int w = (int(ceil_div(n, nb)) + 15) / 16 * 16;
   for (int c = 0; c < n; c += w) c0.push_back(c);
   return c0;
@@ -747,12 +858,12 @@ std::vector<int> column_blocks(int n) {
 // edge call reads its range-error word back (PG_FLAG_TRUSTED_INDICES) is an argument of apply_edge.
 // =================================================================================================
 
-// W [k, n] with row stride ld as tensor-core GEMMs of at most kMaxNT output features, block b writing the columns
+// W [k, n] with row stride ld as tensor-core GEMMs of at most max_w output features, block b writing the columns
 // from col0[b]; only the first n_src columns of W are read, the pad columns past them get zero weights and bias
 int prepare_column_blocks(std::vector<PreparedGemm>& blocks, std::vector<int>& col0, const float* w, int ld,
-                          const float* bias, int k, int n_src, int n, cudaStream_t s) {
+                          const float* bias, int k, int n_src, int n, cudaStream_t s, int max_w = kMaxNT) {
   PG_REQUIRE(n >= 1, "no tensor-core shape for a %d x %d layer", k, n);
-  col0 = column_blocks(n);
+  col0 = column_blocks(n, max_w);
   blocks = std::vector<PreparedGemm>(col0.size());
   for (size_t b = 0; b < col0.size(); ++b) {
     const int wn = (b + 1 < col0.size() ? col0[b + 1] : n) - col0[b];
@@ -762,6 +873,17 @@ int prepare_column_blocks(std::vector<PreparedGemm>& blocks, std::vector<int>& c
     blocks[b].n = wn;
   }
   return PG_OK;
+}
+
+// whether every column block of at most max_w of an n-wide GNN edge layer keeps its column group of W resident in
+// shared memory at padded K kp
+bool gnn_w_resident(int kp, int n, int max_w) {
+  const std::vector<int> c0 = column_blocks(n, max_w);
+  for (size_t b = 0; b < c0.size(); ++b) {
+    const WgShape t = wg_shape(kp, (b + 1 < c0.size() ? c0[b + 1] : n) - c0[b]);
+    if (gnn_smem_bytes(t.kp, t.ni) > 227 * 1024) return false;
+  }
+  return true;
 }
 
 // narrow / shallow layers (N < 8, K < 64: the 64->3, 64->4, 64->7 heads) stay on the fp32 FFMA kernel
@@ -896,6 +1018,11 @@ int prepare_edge(PreparedEdge& e, int mode, int c_in, const float* const* weight
   if (num_layers != 2) return PG_OK;
   const int d1 = dims[1], n = dims[2];
   e.kp = (d1 + 15) / 16 * 16;
+  // the edge kernel keeps a column group of W2 resident in shared memory: a hidden layer too wide for the groups of
+  // the usual column blocks runs as 64-wide blocks (up to kp = 896), a wider one on the fp32 edge kernel
+  int max_w = kMaxNT;
+  if (!gnn_w_resident(e.kp, n, max_w)) max_w = 64;
+  if (!gnn_w_resident(e.kp, n, max_w)) return PG_OK;
   // hoisted first layer on the tensor cores too: logical N = kp, the pad columns get zero weights and bias
   if (int rc = prepare_fc(e.p_fc, weights[0], d1, biases[0], c_in, d1, e.kp, true, s)) return rc;
   if (!e.p_fc.tc) {   // FFMA fallback writes the zero padding itself (ldo = kp)
@@ -905,7 +1032,7 @@ int prepare_edge(PreparedEdge& e, int mode, int c_in, const float* const* weight
   PG_CUDA_OK(e.w1x.alloc(sizeof(float) * 3 * e.kp, s));
   pad_rows_kernel<<<4, 256, 0, s>>>(weights[0] + int64_t(c_in) * d1, 3, d1, e.kp, e.w1x.as<float>());
   PG_LAUNCH_CHECK();
-  if (int rc = prepare_column_blocks(e.last, e.last_col0, weights[1], n, biases[1], d1, n, n, s)) return rc;
+  if (int rc = prepare_column_blocks(e.last, e.last_col0, weights[1], n, biases[1], d1, n, n, s, max_w)) return rc;
   e.path = EDGE_GNN;
   return PG_OK;
 }
