@@ -33,7 +33,9 @@
 //              which every thread waits on once: kp x NI x 4 B, 185 KB for the car layer (304 x 152).  W then stays
 //              for the whole launch: no ring, no per-chunk barrier, no producer warpgroup.  The three warpgroups
 //              are independent consumers of 64-row tiles (tiles 3 j + wg of CTA slot j = blockIdx.x / NS, stepping by
-//              3 gridDim.x / NS), one m64nNIk16 accumulator each, A in registers as below.  Nothing makes one
+//              3 gridDim.x / NS), one m64nNIk16 accumulator each, A in registers as below.  Their rows of P reach
+//              shared memory kGnnStages chunks ahead of the wgmmas, copied by each thread with cp.async (GnnGather),
+//              and the copies run on into the warpgroup's next tile.  Nothing makes one
 //              warpgroup wait for another, so while one flushes its segment max the other two keep the tensor cores
 //              busy.  Every output column gets the same wgmmas on the same operands in the same order as with the
 //              whole N in one warpgroup, so the results do not depend on the grouping.  Both column groups gather the
@@ -107,8 +109,16 @@ constexpr int log2_ring(int r) { return r >= 4 ? 2 : r >= 2 ? 1 : 0; }
 // column group of W
 constexpr int kGnnWarpgroups = kWgThreads / 128;
 constexpr int kGnnTileRows = 64;
-// shared memory of a GNN CTA: its column group of W (ni columns, hi + lo, kp k), then the mbarrier
-constexpr size_t gnn_smem_bytes(int kp, int ni) { return size_t(kp) * ni * 4 + sizeof(uint64_t); }
+// P chunks a warpgroup has in flight (GnnGather).  One beats two and three on H100 (DESIGN §6): the car layer's
+// 185 KB of W plus one 4 KB stage per warpgroup still fits the 196 KB shared-memory carve-out, deeper stages take the
+// 228 KB one and leave less L1
+constexpr int kGnnStages = 1;
+constexpr uint32_t kGnnStageBytes = 64 * 64;    // one warpgroup's 64 rows of a 16-k chunk of P, fp32
+// shared memory of a GNN CTA: its column group of W (ni columns, hi + lo, kp k), every warpgroup's gather stages,
+// then the mbarrier
+constexpr size_t gnn_smem_bytes(int kp, int ni) {
+  return size_t(kp) * ni * 4 + size_t(kGnnWarpgroups) * kGnnStages * kGnnStageBytes + sizeof(uint64_t);
+}
 
 enum { PROD_ROWS = 0, PROD_GNN = 1, PROD_POOL = 2 };
 enum { EPI_STORE = 0, EPI_SEGMAX = 1 };
@@ -179,12 +189,11 @@ __device__ __forceinline__ float2 ldg2(const float* ptr) { return __ldg(reinterp
 
 // A rows in registers (wgmma_bf16_rs): thread t of a warpgroup holds rows 16 warp + lane / 4 and + 8 of its 64, the
 // rows of its accumulators, and k = 2 (lane % 4) + {0, 1, 8, 9} of every 16-k chunk.  context() reads what the rows
-// need once per tile.  ROWS: the rows of p.x;  GNN: the edges' source vertices, their rows of P (32 bits: two
-// registers), and x_src - x_dst';  POOL: the same offset and the source's feature
+// need once per tile.  ROWS: the rows of p.x;  GNN: x_src - x_dst' (GnnGather copies the rows of P);  POOL: the same
+// offset and the source's feature
 template <int kProd, bool kAnyAct>
 struct RowA {
   const float* rp[2];
-  uint32_t src_row[2];
   float rx[2], ry[2], rz[2], f0[2];
 
   // rows row0 + 16 warp + lane / 4 (+ 8) of the layer's A
@@ -193,7 +202,6 @@ struct RowA {
     for (int h = 0; h < 2; ++h) {
       const int64_t row = row0 + warp * 16 + (lane >> 2) + 8 * h;
       rp[h] = p.x;
-      src_row[h] = 0u;
       rx[h] = ry[h] = rz[h] = f0[h] = 0.f;
       if (row >= p.num_rows) continue;
       if (kProd == PROD_ROWS) {
@@ -210,20 +218,15 @@ struct RowA {
       rx[h] = __ldg(p.xyz_src + int64_t(si) * 3 + 0) - __ldg(p.xyz_dst + drow * 3 + 0);
       ry[h] = __ldg(p.xyz_src + int64_t(si) * 3 + 1) - __ldg(p.xyz_dst + drow * 3 + 1);
       rz[h] = __ldg(p.xyz_src + int64_t(si) * 3 + 2) - __ldg(p.xyz_dst + drow * 3 + 2);
-      if (kProd == PROD_GNN) src_row[h] = uint32_t(si);
-      else f0[h] = __ldg(p.feat + si);
+      if (kProd == PROD_POOL) f0[h] = __ldg(p.feat + si);
     }
   }
-  // the fp32 inputs of chunk kc's fragment: q[i] for register i, the thread's row i & 1, k kq + 8 (i >> 1) and + 1
+  // ROWS: the fp32 inputs of chunk kc's fragment, q[i] for register i: the thread's row i & 1, k kq + 8 (i >> 1), + 1
   __device__ __forceinline__ void load(const WgParams& p, int kc, int lane, float2 (&q)[4]) const {
-    if constexpr (kProd != PROD_POOL) {
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int k = kc * 16 + (lane & 3) * 2 + 8 * (i >> 1);
-        q[i] = (kProd == PROD_GNN || k + 2 <= p.k_real)
-                   ? ldg_nc((kProd == PROD_GNN ? p.x + int64_t(src_row[i & 1]) * p.ldx : rp[i & 1]) + k)
-                   : make_float2(0.f, 0.f);
-      }
+    for (int i = 0; i < 4; ++i) {
+      const int k = kc * 16 + (lane & 3) * 2 + 8 * (i >> 1);
+      q[i] = k + 2 <= p.k_real ? ldg_nc(rp[i & 1] + k) : make_float2(0.f, 0.f);
     }
   }
   // chunk kc's fragment, split into hi / lo
@@ -256,25 +259,19 @@ struct RowA {
   }
 };
 
-// The k-loop of a layer whose A fragments are built in registers: chunk(kc, hi, lo) issues chunk kc's wgmmas and
-// leaves exactly itself in flight.  A fragment may be written only once the wgmmas reading it are complete: two of
-// them, alternating, and the loop unrolled by two so that each chunk's fragment registers are fixed at compile time.
-// Chunk kc + 1's fragment is built while chunk kc's wgmmas run, and the loads of chunk kc + 2 are issued before chunk
-// kc + 1's wgmmas
-template <class A, class Chunk>
-__device__ __forceinline__ void rs_k_loop(const WgParams& p, const A& a, int lk, int lane, Chunk&& chunk) {
-  float2 q[4] = {};
+// The k-loop of a layer whose A fragments are built in registers: frag(kc, hi, lo) builds chunk kc's fragment and
+// issues the loads of what comes next; chunk(kc, hi, lo) issues chunk kc's wgmmas and leaves exactly itself in
+// flight.  A fragment may be written only once the wgmmas reading it are complete: two of them, alternating, and the
+// loop unrolled by two so that each chunk's fragment registers are fixed at compile time.  Chunk kc + 1's fragment is
+// built while chunk kc's wgmmas run
+template <class Frag, class Chunk>
+__device__ __forceinline__ void rs_k_loop(int lk, Frag&& frag, Chunk&& chunk) {
   uint32_t ahi[2][4], alo[2][4];
-  a.load(p, 0, lane, q);
-  a.make_frag(p, q, 0, lane, ahi[0], alo[0]);
-  if (lk > 1) a.load(p, 1, lane, q);
+  frag(0, ahi[0], alo[0]);
   auto step = [&](int kc, const uint32_t (&hi)[4], const uint32_t (&lo)[4], uint32_t (&next_hi)[4],
                   uint32_t (&next_lo)[4]) {
     chunk(kc, hi, lo);
-    if (kc + 1 < lk) {
-      a.make_frag(p, q, kc + 1, lane, next_hi, next_lo);
-      if (kc + 2 < lk) a.load(p, kc + 2, lane, q);
-    }
+    if (kc + 1 < lk) frag(kc + 1, next_hi, next_lo);
   };
   for (int kc = 0; kc < lk; kc += 2) {
     step(kc, ahi[0], alo[0], ahi[1], alo[1]);
@@ -376,23 +373,92 @@ __device__ __forceinline__ void seg_epilogue(const WgParams& p, const float (&ac
 }
 
 // ---- GNN edge layer: W resident, three independent consumer warpgroups (header, "mapping") -----------------------
+// The P gather of one warpgroup, kGnnStages chunks ahead of its wgmmas.  A stage holds the warpgroup's 64 rows of
+// one 16-k chunk of P in fp32, 64 B per row.  Lane q of a quad copies the 16-byte piece q of the quad's two rows (g and
+// g + 8, RowA's) with cp.async.cg, one commit group per chunk; after its wait and a __syncwarp each lane reads its
+// fragment's four 8-byte pairs, written by its own quad.  The 32-byte halves of row r swap places when bit 1 of r is
+// set, so a warp's 8-byte reads (8 rows x 32 B) take the minimal two wavefronts.  No warpgroup barrier and no fence.
+// The copy cursor runs on from a tile's last chunk into the warpgroup's next tile (empty groups past its last), so
+// the next tile's first chunks land while this one finishes and flushes
+struct GnnGather {
+  uint32_t base;      // the warpgroup's stage 0
+  uint32_t wr, rd;    // the thread's piece of row g, and its first pair of row g (k 2 q), within a stage
+  int stage = 0;      // the oldest stage: read next, then refilled
+  int tile, kc = 0;   // the chunk the next copy fetches
+  uint32_t row[2];    // the P rows (source vertices) of the thread's two rows of that tile
+
+  __device__ __forceinline__ void init(uint32_t stages, int warp, int lane) {
+    const uint32_t g = uint32_t(warp * 16 + (lane >> 2)), q = uint32_t(lane & 3), swap = ((g >> 1) & 1u) * 32u;
+    base = stages;
+    wr = g * 64u + (((q >> 1) * 32u) ^ swap) + (q & 1u) * 16u;
+    rd = g * 64u + swap + q * 8u;
+  }
+  __device__ __forceinline__ void rows(const WgParams& p, int warp, int lane) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t r = int64_t(tile) * kGnnTileRows + warp * 16 + (lane >> 2) + 8 * h;
+      const int si = r < p.num_rows ? __ldg(p.src + r) : 0;
+      row[h] = si >= 0 && si < p.num_src ? uint32_t(si) : 0u;   // out of range: RowA::context sets the error word
+    }
+  }
+  __device__ __forceinline__ void copy(const WgParams& p, int num_tiles, int stride, int warp, int lane) {
+    if (tile < num_tiles) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        cp_async_16(base + uint32_t(stage) * kGnnStageBytes + wr + uint32_t(h) * 512u,
+                    p.x + int64_t(row[h]) * p.ldx + kc * 16 + (lane & 3) * 4);
+    }
+    cp_async_commit();
+    stage = stage + 1 == kGnnStages ? 0 : stage + 1;
+    if (++kc == p.nchunks) {
+      kc = 0;
+      tile += stride;
+      rows(p, warp, lane);
+    }
+  }
+  // the fp32 inputs of the oldest chunk in flight, as make_frag takes them (q[i]: row i & 1, k half i >> 1).  The
+  // __syncwarp after the reads keeps the quad's refill of the stage (copy(), next) behind them
+  __device__ __forceinline__ void take(float2 (&q)[4]) const {
+    cp_async_wait<kGnnStages - 1>();
+    __syncwarp();
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+      q[i] = lds_f2(base + uint32_t(stage) * kGnnStageBytes + (rd ^ uint32_t(i >> 1) * 32u) + uint32_t(i & 1) * 512u);
+    __syncwarp();
+  }
+};
+
 template <int NI, int NS, bool kAnyAct>
 __device__ __forceinline__ void wg_gnn_body(const WgParams& p) {
   constexpr int NT = NI * NS;
   constexpr uint32_t kSlice = uint32_t(NI) * 32u;   // one group's hi (or lo) part of a 16-k chunk
-  extern __shared__ __align__(128) uint8_t smem[];  // [nchunks][hi | lo][NI rows x 16 k], then the mbarrier
+  // [nchunks][hi | lo][NI rows x 16 k], then [warpgroup][stage][64 rows x 16 k] fp32 (GnnGather), then the mbarrier
+  extern __shared__ __align__(128) uint8_t smem[];
   const int nk = p.nchunks;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + size_t(nk) * 2 * kSlice);
+  const uint32_t w_bytes = uint32_t(nk) * 2u * kSlice;
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + w_bytes + kGnnWarpgroups * kGnnStages * kGnnStageBytes);
   const int tid = threadIdx.x;
   const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);   // warpgroup, warp-uniform by construction
   const int group = int(blockIdx.x) % NS;
+  const int warp = (tid & 127) >> 5, lane = tid & 31;
+  const int num_tiles = int(p.num_tiles), stride = kGnnWarpgroups * int(gridDim.x / NS);
+  const int first = kGnnWarpgroups * int(blockIdx.x / NS) + wg;
+  // the first chunks of P are on their way while W lands
+  GnnGather gather;
+  gather.init(smem_u32(smem) + w_bytes + uint32_t(wg * kGnnStages) * kGnnStageBytes, warp, lane);
+  gather.tile = first;
+  gather.rows(p, warp, lane);
+#pragma unroll
+  for (int s = 0; s < kGnnStages; ++s) gather.copy(p, num_tiles, stride, warp, lane);
+  RowA<PROD_GNN, kAnyAct> a;
+  a.context(p, int64_t(first) * kGnnTileRows, warp, lane);
   if (tid == 0) {
     mbar_init(full, 1);
     fence_barrier_init();
   }
   __syncthreads();
   if (tid == 0) {
-    mbar_arrive_expect_tx(full, uint32_t(nk) * 2u * kSlice);
+    mbar_arrive_expect_tx(full, w_bytes);
     for (int kc = 0; kc < nk; ++kc)
 #pragma unroll
       for (int h = 0; h < 2; ++h)
@@ -400,15 +466,17 @@ __device__ __forceinline__ void wg_gnn_body(const WgParams& p) {
                  p.bimg + size_t(kc) * NT * 64 + size_t(h) * NT * 32 + size_t(group) * kSlice, kSlice, full);
   }
   mbar_wait(full, 0);
-  const int warp = (tid & 127) >> 5, lane = tid & 31;
   const uint32_t w_base = smem_u32(smem);
-  const int num_tiles = int(p.num_tiles), stride = kGnnWarpgroups * int(gridDim.x / NS);
-  for (int tile = kGnnWarpgroups * int(blockIdx.x / NS) + wg; tile < num_tiles; tile += stride) {
+  for (int tile = first; tile < num_tiles; tile += stride) {
     const int64_t row0 = int64_t(tile) * kGnnTileRows;
-    RowA<PROD_GNN, kAnyAct> a;
-    a.context(p, row0, warp, lane);
     float acc[1][NI / 2];
-    rs_k_loop(p, a, nk, lane, [&](int kc, const uint32_t (&hi)[4], const uint32_t (&lo)[4]) {
+    auto frag = [&](int kc, uint32_t (&hi)[4], uint32_t (&lo)[4]) {
+      float2 q[4];
+      gather.take(q);
+      a.make_frag(p, q, kc, lane, hi, lo);
+      gather.copy(p, num_tiles, stride, warp, lane);
+    };
+    rs_k_loop(nk, frag, [&](int kc, const uint32_t (&hi)[4], const uint32_t (&lo)[4]) {
       wgmma_fence();
       const uint32_t b = w_base + uint32_t(kc) * 2u * kSlice;
       const uint64_t b_hi = make_smem_desc(b, 128, 256), b_lo = make_smem_desc(b + kSlice, 128, 256);
@@ -418,6 +486,8 @@ __device__ __forceinline__ void wg_gnn_body(const WgParams& p) {
       wgmma_commit();
       wgmma_wait<1>();                    // chunk kc - 1 complete: its A fragment is free
     });
+    // the next tile's context while the last wgmmas run; its first chunks of P are already in flight
+    a.context(p, row0 + int64_t(stride) * kGnnTileRows, warp, lane);
     wgmma_wait<0>();
     seg_epilogue<NI, 1, kAnyAct>(p, acc, row0 + warp * 16 + (lane >> 2), lane, group * NI);
   }
@@ -525,8 +595,15 @@ __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
         ++g;
       };
       if (streamed && kProd != PROD_POOL) {
+        // the loads of chunk kc + 1 are issued before chunk kc's wgmmas
         a.context(p, row0, warp, lane);
-        rs_k_loop(p, a, lk, lane, chunk);
+        float2 q[4];
+        a.load(p, 0, lane, q);
+        auto frag = [&](int kc, uint32_t (&hi)[4], uint32_t (&lo)[4]) {
+          a.make_frag(p, q, kc, lane, hi, lo);
+          if (kc + 1 < lk) a.load(p, kc + 1, lane, q);
+        };
+        rs_k_loop(lk, frag, chunk);
       } else if (streamed) {
         // POOL layer 1: the fragments go through a double buffer at the start of the region, in to_region's layout,
         // and the wgmmas read A from there.  With A in registers next to the on-chip layers' code, ptxas serialises
@@ -1019,7 +1096,8 @@ int prepare_edge(PreparedEdge& e, int mode, int c_in, const float* const* weight
   const int d1 = dims[1], n = dims[2];
   e.kp = (d1 + 15) / 16 * 16;
   // the edge kernel keeps a column group of W2 resident in shared memory: a hidden layer too wide for the groups of
-  // the usual column blocks runs as 64-wide blocks (up to kp = 896), a wider one on the fp32 edge kernel
+  // the usual column blocks (kp > 352 at 152 columns) runs as 64-wide blocks (up to kp = 848), a wider one on the fp32
+  // edge kernel
   int max_w = kMaxNT;
   if (!gnn_w_resident(e.kp, n, max_w)) max_w = 64;
   if (!gnn_w_resident(e.kp, n, max_w)) return PG_OK;

@@ -56,6 +56,23 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
                : "memory");
 }
 
+// ---- cp.async: one thread's copies global -> shared, completion per commit group of that thread ---------------
+// 16 bytes, through L2 only (bypassing L1); both addresses 16-byte aligned
+__device__ __forceinline__ void cp_async_16(uint32_t smem_dst, const void* gmem_src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_dst), "l"(gmem_src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+// every group of this thread but the N most recent has landed
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
+__device__ __forceinline__ float2 lds_f2(uint32_t smem_src) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(smem_src) : "memory");
+  return v;
+}
+
 // ---- named barrier over one warpgroup ------------------------------------------------------------
 __device__ __forceinline__ void warpgroup_sync(int id) {
   asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory");
