@@ -48,7 +48,7 @@ PG_API int pg_version(void);
 PG_API const char* pg_last_error(void);
 /* 1 if the visible device is sm_90 (H100); the wgmma kernels require it. */
 PG_API int pg_device_is_sm90(void);
-/* 1 if the wgmma (precision = 1) kernels are built in AND the device can run them. */
+/* 1 if the wgmma (precision = 1 and 2) kernels are built in AND the device can run them. */
 PG_API int pg_tc_available(void);
 
 /* ------------------------------------------------------------------------ *
@@ -347,7 +347,10 @@ PG_API int pg_gather_rows(const float* params, int64_t num_rows, int32_t num_cha
  * One slim.fully_connected layer (gnn.py:63-80,93-103), normalizer NONE:
  *   out[M,N] = act(x[M,K] @ w[K,N] + bias[N]) (+ residual[M,N] if not NULL)
  * act: a PG_ACT_* code; 0 = linear (the is_logits last layer), 1 = ReLU.
- * precision: 0 = fp32 FFMA, 1 = wgmma BF16x3 split (fp32-class accuracy).
+ * precision: 0 = fp32 FFMA, 1 = wgmma BF16x3 split (fp32-class accuracy), 2 = wgmma FP16: every tensor-core
+ * operand rounded once to FP16 (nearest, saturating at +-65504), fp32 accumulation, one product per 16-k chunk
+ * (~1e-2 on the shipped models' logits).  Without the wgmma kernels, 1 and 2 both run the fp32 FFMA kernels.
+ * Any other code gives PG_ERR_INVALID_ARGUMENT.
  */
 PG_API int pg_fully_connected(const float* x, int64_t m, int32_t k, const float* w, const float* bias,
                        int32_t n, int32_t act, const float* residual, float* out,
@@ -374,7 +377,8 @@ PG_API int pg_fully_connected(const float* x, int64_t m, int32_t k, const float*
  *                W_l is [dims[l], dims[l+1]] row-major, dims[0] = C_in + 3.
  *   dims_host    (host) [num_layers+1]
  *   out          [num_dst, dims[num_layers]]; empty segments get -FLT_MAX.
- *   precision    0 = fp32 FFMA, 1 = wgmma BF16x3 for the wide layers; may be OR-ed with
+ *   precision    0 = fp32 FFMA, 1 = wgmma BF16x3, 2 = wgmma FP16 (as pg_fully_connected) for the wide
+ *                layers; may be OR-ed with
  *                PG_FLAG_TRUSTED_INDICES: the caller guarantees src / dst are in range (they come from
  *                pg_radius_graph, or passed pg_check_edges), so the call skips the device->host
  *                read-back of the range-error flag and does not synchronise the stream.  Out-of-range
@@ -404,7 +408,7 @@ PG_API int pg_check_edges(const int32_t* src, const int32_t* dst, int64_t num_ed
  * slim.fully_connected at graph-build time, gnn.py:63-80, models.py:113-163) and
  * restores them once (run.py:192-202); every sess.run then only computes.  The
  * equivalent here: pg_layer_create packs everything that depends on the weights
- * only (BF16 hi / lo tensor-core operand images, padded biases, the hoisted first
+ * only (BF16 hi / lo or FP16 tensor-core operand images, padded biases, the hoisted first
  * edge layer, the concatenated predictor heads) into an opaque handle; the
  * pg_layer_* calls below launch compute kernels only.  The handle keeps the
  * caller's weight pointers (the fp32 FFMA paths read them directly): they must
@@ -420,7 +424,8 @@ PG_API int pg_check_edges(const int32_t* src, const int32_t* dst, int64_t num_ed
  *                            reference creates them: cls fc (D->H), cls fc_1 (H->C), then
  *                            for every class c: loc fc (D->H), fc_1 (H->H), fc_2 (H->box_len);
  *                            num_layers = 2 + 3 C.
- *   precision 0 = fp32 FFMA, 1 = wgmma BF16x3 wherever the shapes allow; may be OR-ed with
+ *   precision 0 = fp32 FFMA, 1 = wgmma BF16x3, 2 = wgmma FP16 (as pg_fully_connected) wherever the shapes
+ *             allow; may be OR-ed with
  *             PG_PRECISION_ACTIVATION(code): the activation of every layer that has one (default ReLU).
  *             It is fixed here because it selects the kernels the handle launches.
  * ------------------------------------------------------------------------ */

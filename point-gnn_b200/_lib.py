@@ -238,7 +238,7 @@ def tc_launch_count(which=0):
 
 
 def tc_available():
-    """True when the wgmma (precision=1) kernels are compiled in and the device is sm_90."""
+    """True when the wgmma (precision=1 and 2) kernels are compiled in and the device is sm_90."""
     return bool(_call('pg_tc_available'))
 
 

@@ -1,4 +1,4 @@
-// Hopper tensor-core kernels (wgmma): the fast path (precision = 1, "BF16x3").
+// Hopper tensor-core kernels (wgmma): the fast paths (precision = 1, "BF16x3", and precision = 2, "FP16").
 //
 // wg_gemm_kernel - one persistent kernel for every tensor-core layer of the network: out = epilogue(A @ W + b), A
 //   produced on the fly (in registers, or in shared memory for the pooling launches) by the warpgroups that also run
@@ -25,8 +25,12 @@
 //              atomic_max_float (NONE, LeakyReLU, ELU and Tanh give negative values) and activate_rows applies
 //              act(. + b) once per output element afterwards.  Dense layers with another activation run
 //              wg_gemm_kernel linear, then activate_rows
-//   precision  every fp32 operand is split x = hi + lo (two BF16), and hi*hi' + lo*hi' + hi*lo' is
-//              accumulated in fp32 registers: ~2^-16 relative per product (fp32-class accuracy)
+//   precision  BF16x3 (kArith = ARITH_BF16X3): every fp32 operand is split x = hi + lo (two BF16), and
+//              hi*hi' + lo*hi' + hi*lo' is accumulated in fp32 registers: ~2^-16 relative per product (fp32-class
+//              accuracy).  FP16 (ARITH_F16, the *_f16_kernel instances): every operand is rounded once to FP16
+//              (nearest, saturating at +-65504), one wgmma per 16-k chunk, fp32 accumulation: ~2^-11 relative per
+//              operand, a third of the wgmmas and half the W bytes.  Everything that is not a tensor-core operand
+//              (the GNN layer's per-edge correction, pooling layer 0, bias, activation, segment max) stays fp32 in both
 //   mapping    GNN (wg_gnn_body): W resident.  A CTA owns one NI-wide column group c = blockIdx.x % NS of the padded
 //              output.  At kernel start one thread copies that group's hi and lo slices of every 16-k chunk (NI x 32 B
 //              each, straight out of the image layout below) into shared memory with cp.async.bulk on one mbarrier,
@@ -89,8 +93,16 @@ constexpr int kTileRows = 128;      // rows per tile (64 per consumer warpgroup)
 // more L1 for the gathered rows (GNN edge layer at the benchmark shape: 7.7 vs 8.0 ms, H100 SXM at a 400 W limit)
 constexpr int kMaxRing = 4;
 constexpr int kMaxNT = 304;         // widest padded N one launch covers
-constexpr uint32_t kABytes = 4096;  // one warpgroup's shared-memory A chunk: hi (2048) + lo (2048), 64 rows x 16 k
 constexpr int kMaxChain = 6;        // on-chip pooling layers ahead of the kernel's own (edge MLPs have <= 8 layers)
+
+// The arithmetic of a tensor-core layer (header, "precision"): BF16x3 keeps two operand planes (hi, lo) per 16-k
+// chunk and issues three wgmmas; FP16 keeps one plane and issues one
+enum { ARITH_BF16X3 = 0, ARITH_F16 = 1 };
+constexpr int arith_planes(int arith) { return arith == ARITH_F16 ? 1 : 2; }
+// bytes of one W row (output feature) of a 16-k chunk: 32 per plane
+constexpr uint32_t w_row_bytes(int arith) { return 32u * uint32_t(arith_planes(arith)); }
+// one warpgroup's shared-memory A chunk, 64 rows x 16 k: 2048 bytes per plane
+constexpr uint32_t a_chunk_bytes(int arith) { return 2048u * uint32_t(arith_planes(arith)); }
 
 // shared memory of a CTA: a ring of W stages, one A region per consumer warpgroup (POOL only: layer 1's double buffer,
 // or a whole on-chip activation; ROWS and GNN keep A in registers), the full / empty barriers
@@ -114,10 +126,11 @@ constexpr int kGnnTileRows = 64;
 // 228 KB one and leave less L1
 constexpr int kGnnStages = 1;
 constexpr uint32_t kGnnStageBytes = 64 * 64;    // one warpgroup's 64 rows of a 16-k chunk of P, fp32
-// shared memory of a GNN CTA: its column group of W (ni columns, hi + lo, kp k), every warpgroup's gather stages,
-// then the mbarrier
-constexpr size_t gnn_smem_bytes(int kp, int ni) {
-  return size_t(kp) * ni * 4 + size_t(kGnnWarpgroups) * kGnnStages * kGnnStageBytes + sizeof(uint64_t);
+// shared memory of a GNN CTA: its column group of W (ni columns, every plane of the arithmetic, kp k), every
+// warpgroup's gather stages, then the mbarrier
+constexpr size_t gnn_smem_bytes(int kp, int ni, int arith) {
+  return size_t(kp / 16) * ni * w_row_bytes(arith) + size_t(kGnnWarpgroups) * kGnnStages * kGnnStageBytes +
+         sizeof(uint64_t);
 }
 
 enum { PROD_ROWS = 0, PROD_GNN = 1, PROD_POOL = 2 };
@@ -229,7 +242,8 @@ struct RowA {
       q[i] = k + 2 <= p.k_real ? ldg_nc(rp[i & 1] + k) : make_float2(0.f, 0.f);
     }
   }
-  // chunk kc's fragment, split into hi / lo
+  // chunk kc's fragment: BF16x3 splits it into hi / lo, FP16 rounds it once into hi (lo is not written)
+  template <int kArith>
   __device__ __forceinline__ void make_frag(const WgParams& p, const float2 (&q)[4], int kc, int lane, uint32_t (&hi)[4],
                                             uint32_t (&lo)[4]) const {
 #pragma unroll
@@ -254,10 +268,41 @@ struct RowA {
         }
       }
 #pragma unroll
-      for (int h = 0; h < 2; ++h) split_bf16x2(v[h].x, v[h].y, &hi[2 * c + h], &lo[2 * c + h]);
+      for (int h = 0; h < 2; ++h) {
+        if constexpr (kArith == ARITH_F16)
+          hi[2 * c + h] = pack_f16x2(v[h].x, v[h].y);
+        else
+          split_bf16x2(v[h].x, v[h].y, &hi[2 * c + h], &lo[2 * c + h]);
+      }
     }
   }
 };
+
+// chunk kc's wgmmas of one m64nNk16 accumulator, A from registers: BF16x3 hi*hi' + lo*hi' + hi*lo' (b_lo the lo plane
+// of B), FP16 one product
+template <int kArith, int N>
+__device__ __forceinline__ void mma_rs(float (&d)[N / 2], const uint32_t (&hi)[4], const uint32_t (&lo)[4], uint64_t b_hi,
+                                       uint64_t b_lo, int scale_d) {
+  if constexpr (kArith == ARITH_F16) {
+    wgmma_f16_rs<N>(d, hi, b_hi, scale_d);
+  } else {
+    wgmma_bf16_rs<N>(d, hi, b_hi, scale_d);
+    wgmma_bf16_rs<N>(d, lo, b_hi, 1);
+    wgmma_bf16_rs<N>(d, hi, b_lo, 1);
+  }
+}
+// the same with A from shared memory (descriptors of its planes)
+template <int kArith, int N>
+__device__ __forceinline__ void mma_ss(float (&d)[N / 2], uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo,
+                                       int scale_d) {
+  if constexpr (kArith == ARITH_F16) {
+    wgmma_f16<N>(d, a_hi, b_hi, scale_d);
+  } else {
+    wgmma_bf16<N>(d, a_hi, b_hi, scale_d);
+    wgmma_bf16<N>(d, a_lo, b_hi, 1);
+    wgmma_bf16<N>(d, a_hi, b_lo, 1);
+  }
+}
 
 // The k-loop of a layer whose A fragments are built in registers: frag(kc, hi, lo) builds chunk kc's fragment and
 // issues the loads of what comes next; chunk(kc, hi, lo) issues chunk kc's wgmmas and leaves exactly itself in
@@ -428,14 +473,15 @@ struct GnnGather {
   }
 };
 
-template <int NI, int NS, bool kAnyAct>
+template <int NI, int NS, bool kAnyAct, int kArith>
 __device__ __forceinline__ void wg_gnn_body(const WgParams& p) {
   constexpr int NT = NI * NS;
-  constexpr uint32_t kSlice = uint32_t(NI) * 32u;   // one group's hi (or lo) part of a 16-k chunk
-  // [nchunks][hi | lo][NI rows x 16 k], then [warpgroup][stage][64 rows x 16 k] fp32 (GnnGather), then the mbarrier
+  constexpr uint32_t kSlice = uint32_t(NI) * 32u;   // one group's part of one plane (hi, lo or FP16) of a 16-k chunk
+  constexpr int kPlanes = arith_planes(kArith);
+  // [nchunks][planes][NI rows x 16 k], then [warpgroup][stage][64 rows x 16 k] fp32 (GnnGather), then the mbarrier
   extern __shared__ __align__(128) uint8_t smem[];
   const int nk = p.nchunks;
-  const uint32_t w_bytes = uint32_t(nk) * 2u * kSlice;
+  const uint32_t w_bytes = uint32_t(nk) * kPlanes * kSlice;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + w_bytes + kGnnWarpgroups * kGnnStages * kGnnStageBytes);
   const int tid = threadIdx.x;
   const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);   // warpgroup, warp-uniform by construction
@@ -461,9 +507,10 @@ __device__ __forceinline__ void wg_gnn_body(const WgParams& p) {
     mbar_arrive_expect_tx(full, w_bytes);
     for (int kc = 0; kc < nk; ++kc)
 #pragma unroll
-      for (int h = 0; h < 2; ++h)
-        bulk_g2s(smem + (size_t(kc) * 2 + h) * kSlice,
-                 p.bimg + size_t(kc) * NT * 64 + size_t(h) * NT * 32 + size_t(group) * kSlice, kSlice, full);
+      for (int h = 0; h < kPlanes; ++h)
+        bulk_g2s(smem + (size_t(kc) * kPlanes + h) * kSlice,
+                 p.bimg + size_t(kc) * NT * w_row_bytes(kArith) + size_t(h) * NT * 32 + size_t(group) * kSlice, kSlice,
+                 full);
   }
   mbar_wait(full, 0);
   const uint32_t w_base = smem_u32(smem);
@@ -473,16 +520,14 @@ __device__ __forceinline__ void wg_gnn_body(const WgParams& p) {
     auto frag = [&](int kc, uint32_t (&hi)[4], uint32_t (&lo)[4]) {
       float2 q[4];
       gather.take(q);
-      a.make_frag(p, q, kc, lane, hi, lo);
+      a.template make_frag<kArith>(p, q, kc, lane, hi, lo);
       gather.copy(p, num_tiles, stride, warp, lane);
     };
     rs_k_loop(nk, frag, [&](int kc, const uint32_t (&hi)[4], const uint32_t (&lo)[4]) {
       wgmma_fence();
-      const uint32_t b = w_base + uint32_t(kc) * 2u * kSlice;
+      const uint32_t b = w_base + uint32_t(kc) * kPlanes * kSlice;
       const uint64_t b_hi = make_smem_desc(b, 128, 256), b_lo = make_smem_desc(b + kSlice, 128, 256);
-      wgmma_bf16_rs<NI>(acc[0], hi, b_hi, kc > 0 ? 1 : 0);
-      wgmma_bf16_rs<NI>(acc[0], lo, b_hi, 1);
-      wgmma_bf16_rs<NI>(acc[0], hi, b_lo, 1);
+      mma_rs<kArith, NI>(acc[0], hi, lo, b_hi, b_lo, kc > 0 ? 1 : 0);
       wgmma_commit();
       wgmma_wait<1>();                    // chunk kc - 1 complete: its A fragment is free
     });
@@ -494,11 +539,12 @@ __device__ __forceinline__ void wg_gnn_body(const WgParams& p) {
 }
 
 // ---- dense and pooling layers: W streamed by a producer warpgroup --------------------------------------------------
-template <int kProd, int kEpi, int NI, int NS>
+template <int kProd, int kEpi, int NI, int NS, int kArith>
 __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
   static_assert(kProd != PROD_GNN, "the GNN edge layer runs wg_gnn_body");
   constexpr int NT = NI * NS;
-  constexpr uint32_t kChunkBytes = uint32_t(NT) * 64u;   // hi + lo, 16 k
+  constexpr uint32_t kChunkBytes = uint32_t(NT) * w_row_bytes(kArith);   // every plane, 16 k
+  constexpr uint32_t kABytes = a_chunk_bytes(kArith);
   constexpr int kRing = ring_stages(kChunkBytes, 0);
   // the pooling chain sizes its ring stages and A regions for all of its layers (host side, launch_wg)
   const uint32_t stage_bytes = kProd == PROD_POOL ? p.stage_bytes : kChunkBytes;
@@ -537,7 +583,7 @@ __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
         if (l < nl) {
           const int4 c = p.chain[l];
           lk = c.x;
-          bytes = uint32_t(c.y >> 2) * uint32_t(c.y & 3) * 64u;
+          bytes = uint32_t(c.y >> 2) * uint32_t(c.y & 3) * w_row_bytes(kArith);
           img = p.chain_buf + c.z;
         }
         for (int kc = 0; kc < lk; ++kc, ++g) {
@@ -568,9 +614,9 @@ __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
     auto mma_layer = [&](auto& lacc, int lk, bool streamed) {
       using Acc = std::remove_reference_t<decltype(lacc)>;
       constexpr int ns = int(std::extent<Acc, 0>::value), ni = 2 * int(std::extent<Acc, 1>::value);
-      // chunk kc's wgmmas on W stage g, A hi / lo from registers (uint32_t[4]) or shared memory (descriptors).  Every
-      // chunk leaves exactly itself in flight: a wait on a path of its own (the last chunk's) would make ptxas drain
-      // the wgmmas at the end of every iteration
+      // chunk kc's wgmmas on W stage g, A hi / lo (FP16: hi only) from registers (uint32_t[4]) or shared memory
+      // (descriptors).  Every chunk leaves exactly itself in flight: a wait on a path of its own (the last chunk's)
+      // would make ptxas drain the wgmmas at the end of every iteration
       auto chunk = [&](int kc, const auto& a_hi, const auto& a_lo) {
         mbar_wait(&full[uint32_t(g) & ring_mask], uint32_t((g >> ring_log2) & 1));
         wgmma_fence();
@@ -579,15 +625,10 @@ __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
         for (int i = 0; i < ns; ++i) {
           const uint64_t b_hi = make_smem_desc(b_base + uint32_t(i * ni) * 32u, 128, 256);
           const uint64_t b_lo = make_smem_desc(b_base + uint32_t(ni * ns) * 32u + uint32_t(i * ni) * 32u, 128, 256);
-          if constexpr (std::is_same_v<std::decay_t<decltype(a_hi)>, uint64_t>) {
-            wgmma_bf16<ni>(lacc[i], a_hi, b_hi, kc > 0 ? 1 : 0);
-            wgmma_bf16<ni>(lacc[i], a_lo, b_hi, 1);
-            wgmma_bf16<ni>(lacc[i], a_hi, b_lo, 1);
-          } else {
-            wgmma_bf16_rs<ni>(lacc[i], a_hi, b_hi, kc > 0 ? 1 : 0);
-            wgmma_bf16_rs<ni>(lacc[i], a_lo, b_hi, 1);
-            wgmma_bf16_rs<ni>(lacc[i], a_hi, b_lo, 1);
-          }
+          if constexpr (std::is_same_v<std::decay_t<decltype(a_hi)>, uint64_t>)
+            mma_ss<kArith, ni>(lacc[i], a_hi, a_lo, b_hi, b_lo, kc > 0 ? 1 : 0);
+          else
+            mma_rs<kArith, ni>(lacc[i], a_hi, a_lo, b_hi, b_lo, kc > 0 ? 1 : 0);
         }
         wgmma_commit();
         wgmma_wait<1>();                  // chunk kc - 1 complete: its A fragment and W stage are free
@@ -600,7 +641,7 @@ __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
         float2 q[4];
         a.load(p, 0, lane, q);
         auto frag = [&](int kc, uint32_t (&hi)[4], uint32_t (&lo)[4]) {
-          a.make_frag(p, q, kc, lane, hi, lo);
+          a.template make_frag<kArith>(p, q, kc, lane, hi, lo);
           if (kc + 1 < lk) a.load(p, kc + 1, lane, q);
         };
         rs_k_loop(lk, frag, chunk);
@@ -612,13 +653,13 @@ __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
         auto put = [&](int kc) {
           float2 q[4] = {};
           uint32_t hi[4], lo[4];
-          a.make_frag(p, q, kc, lane, hi, lo);
+          a.template make_frag<kArith>(p, q, kc, lane, hi, lo);
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
             uint8_t* dstp = my_a + uint32_t(kc & 1) * kABytes + uint32_t(warp * 2 + (i & 1)) * 256u +
                             uint32_t(i >> 1) * 128u + uint32_t(lane >> 2) * 16u + uint32_t(lane & 3) * 4u;
             *reinterpret_cast<uint32_t*>(dstp) = hi[i];
-            *reinterpret_cast<uint32_t*>(dstp + kABytes / 2) = lo[i];
+            if constexpr (kArith != ARITH_F16) *reinterpret_cast<uint32_t*>(dstp + kABytes / 2) = lo[i];
           }
         };
         put(0);
@@ -640,9 +681,10 @@ __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
       wgmma_wait<0>();
       release(g - 1);
     };
-    // ---- on-chip pooling layers: relu(acc + b) split into hi / lo over this warpgroup's own (now dead) input in
-    // the region, the first kp_next k of the next layer's A.  A lane's pair (row, cols 8 j + cq, + 1) is one
-    // 4-byte word of a core matrix: a warp writes 128 contiguous bytes per store, free of bank conflicts
+    // ---- on-chip pooling layers: relu(acc + b) split into hi / lo (FP16: rounded once into one plane) over this
+    // warpgroup's own (now dead) input in the region, the first kp_next k of the next layer's A.  A lane's pair (row,
+    // cols 8 j + cq, + 1) is one 4-byte word of a core matrix: a warp writes 128 contiguous bytes per store, free of
+    // bank conflicts
     auto to_region = [&](auto& lacc, const float* bias, int kp_next) {
       using Acc = std::remove_reference_t<decltype(lacc)>;
       constexpr int ns = int(std::extent<Acc, 0>::value), ni = 2 * int(std::extent<Acc, 1>::value);
@@ -656,12 +698,17 @@ __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
             const float b0 = __ldg(bias + col), b1 = __ldg(bias + col + 1);
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-              uint32_t hi, lo;
-              split_bf16x2(fmaxf(lacc[i][4 * jj + 2 * h] + b0, 0.0f), fmaxf(lacc[i][4 * jj + 2 * h + 1] + b1, 0.0f), &hi, &lo);
+              const float v0 = fmaxf(lacc[i][4 * jj + 2 * h] + b0, 0.0f), v1 = fmaxf(lacc[i][4 * jj + 2 * h + 1] + b1, 0.0f);
               uint8_t* dstp = my_a + uint32_t(col >> 4) * kABytes + uint32_t(warp * 2 + h) * 256u +
                               uint32_t((col >> 3) & 1) * 128u + uint32_t(lane >> 2) * 16u + uint32_t(cq) * 2u;
-              *reinterpret_cast<uint32_t*>(dstp) = hi;
-              *reinterpret_cast<uint32_t*>(dstp + kABytes / 2) = lo;
+              if constexpr (kArith == ARITH_F16) {
+                *reinterpret_cast<uint32_t*>(dstp) = pack_f16x2(v0, v1);
+              } else {
+                uint32_t hi, lo;
+                split_bf16x2(v0, v1, &hi, &lo);
+                *reinterpret_cast<uint32_t*>(dstp) = hi;
+                *reinterpret_cast<uint32_t*>(dstp + kABytes / 2) = lo;
+              }
             }
           }
         }
@@ -718,37 +765,60 @@ __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
   }
 }
 
-template <int kProd, int kEpi, int NI, int NS>
-__global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
+template <int kProd, int kEpi, int NI, int NS, int kArith>
+__device__ __forceinline__ void wg_kernel_body(const WgParams& p) {
   if constexpr (kProd == PROD_GNN) {
     static_assert(kEpi == EPI_SEGMAX, "the GNN edge layer ends in the segment max");
-    wg_gnn_body<NI, NS, false>(p);
+    wg_gnn_body<NI, NS, false, kArith>(p);
   } else {
-    wg_gemm_body<kProd, kEpi, NI, NS>(p);
+    wg_gemm_body<kProd, kEpi, NI, NS, kArith>(p);
   }
+}
+
+template <int kProd, int kEpi, int NI, int NS>
+__global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
+  wg_kernel_body<kProd, kEpi, NI, NS, ARITH_BF16X3>(p);
 }
 
 // its own name, so that the instance count and the ptxas properties of wg_gemm_kernel stay those of the ReLU build
 template <int kProd, int kEpi, int NI, int NS>
 __global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_act_kernel(WgParams p) {
   static_assert(kProd == PROD_GNN && kEpi == EPI_SEGMAX, "any-activation instances: the GNN edge layer only");
-  wg_gnn_body<NI, NS, true>(p);
+  wg_gnn_body<NI, NS, true, ARITH_BF16X3>(p);
+}
+
+// the FP16 instances of the two kernels above (precision = 2): the same bodies, one operand plane and one wgmma per
+// 16-k chunk.  Names of their own, for the same reason
+template <int kProd, int kEpi, int NI, int NS>
+__global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_f16_kernel(WgParams p) {
+  wg_kernel_body<kProd, kEpi, NI, NS, ARITH_F16>(p);
+}
+
+template <int kProd, int kEpi, int NI, int NS>
+__global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_act_f16_kernel(WgParams p) {
+  static_assert(kProd == PROD_GNN && kEpi == EPI_SEGMAX, "any-activation instances: the GNN edge layer only");
+  wg_gnn_body<NI, NS, true, ARITH_F16>(p);
 }
 
 // ---- W [K, N] -> streamed B image ---------------------------------------------------------------
-// B operand rows are OUTPUT features (N), K-major, one block per 16-k chunk: [hi | lo], each NT / 8 row
-// groups of two core matrices: element (k, col) at chunk (k / 16), (col / 8) * 256 + ((k % 16) / 8) * 128 +
-// (col % 8) * 16 + (k % 8) * 2.  Columns >= n_src and rows >= k are zero.
-__global__ void pack_b_kernel(const float* __restrict__ w, int k, int n_src, int ld, int kp, int nt,
+// B operand rows are OUTPUT features (N), K-major, one block per 16-k chunk: its planes ([hi | lo] for BF16x3, one
+// FP16 plane), each NT / 8 row groups of two core matrices: element (k, col) at chunk (k / 16), (col / 8) * 256 +
+// ((k % 16) / 8) * 128 + (col % 8) * 16 + (k % 8) * 2.  Columns >= n_src and rows >= k are zero.
+__global__ void pack_b_kernel(const float* __restrict__ w, int k, int n_src, int ld, int kp, int nt, int arith,
                               uint8_t* __restrict__ img) {
   const int total = kp * nt;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
     const int kk = i / nt, col = i - kk * nt;
     const float v = (col < n_src && kk < k) ? w[int64_t(kk) * ld + col] : 0.0f;
+    const size_t off = size_t(kk / 16) * (size_t(nt) * w_row_bytes(arith)) + size_t(col / 8) * 256 +
+                       size_t((kk % 16) / 8) * 128 + size_t(col % 8) * 16 + size_t(kk % 8) * 2;
+    if (arith == ARITH_F16) {
+      // the A operands' rounding: nearest, saturating at +-65504
+      *reinterpret_cast<uint16_t*>(img + off) = uint16_t(pack_f16x2(v, 0.0f) & 0xffffu);
+      continue;
+    }
     const __nv_bfloat16 hi = __float2bfloat16_rn(v);
     const __nv_bfloat16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-    const size_t off = size_t(kk / 16) * (size_t(nt) * 64) + size_t(col / 8) * 256 + size_t((kk % 16) / 8) * 128 +
-                       size_t(col % 8) * 16 + size_t(kk % 8) * 2;
     *reinterpret_cast<__nv_bfloat16*>(img + off) = hi;
     *reinterpret_cast<__nv_bfloat16*>(img + off + size_t(nt) * 32) = lo;
   }
@@ -764,12 +834,12 @@ __global__ void pad_rows_kernel(const float* __restrict__ in, int rows, int cols
 
 struct WgShape {
   int kp, np, ni, ns, nt;
-  size_t smem;
+  size_t smem;   // a streamed (ROWS) launch's, for the arithmetic wg_shape was given
   bool ok;
 };
 
 // N is padded to one of the instruction shapes the kernel is built for (zero weight columns)
-WgShape wg_shape(int k, int n) {
+WgShape wg_shape(int k, int n, int arith) {
   WgShape t{};
   t.kp = (k + 15) / 16 * 16;
   t.np = (n + 15) / 16 * 16;
@@ -779,27 +849,30 @@ WgShape wg_shape(int k, int n) {
   else if (t.np <= 256) { t.ni = 128; t.ns = 2; }
   else if (t.np <= kMaxNT) { t.ni = 152; t.ns = 2; }
   t.nt = t.ni * t.ns;
-  t.smem = wg_smem_bytes(uint32_t(t.nt) * 64u, 0, ring_stages(uint32_t(t.nt) * 64u, 0));
+  const uint32_t chunk = uint32_t(t.nt) * w_row_bytes(arith);
+  t.smem = wg_smem_bytes(chunk, 0, ring_stages(chunk, 0));
   t.ok = t.nt > 0 && k >= 1 && n >= 1;
   return t;
 }
 
-// one weight matrix in the streamed image layout + its padded bias
+// one weight matrix in the streamed image layout of its arithmetic + its padded bias
 struct PreparedGemm {
   WgShape t{};
   int n = 0;
+  int arith = ARITH_BF16X3;
   Temp img, bias_pad;
 };
 
-int prepare_gemm(PreparedGemm& g, const float* w, int ld, const float* bias, int k, int n, cudaStream_t s) {
-  g.t = wg_shape(k, n);
+int prepare_gemm(PreparedGemm& g, const float* w, int ld, const float* bias, int k, int n, int arith, cudaStream_t s) {
+  g.t = wg_shape(k, n, arith);
   g.n = n;
+  g.arith = arith;
   PG_REQUIRE(g.t.ok, "no tensor-core shape for a %d x %d layer", k, n);
   PG_CUDA_OK(g.bias_pad.alloc(sizeof(float) * g.t.nt, s));
   pad_rows_kernel<<<2, 256, 0, s>>>(bias, 1, n, g.t.nt, g.bias_pad.as<float>());
   PG_LAUNCH_CHECK();
-  PG_CUDA_OK(g.img.alloc(size_t(g.t.kp) * g.t.nt * 4, s));
-  pack_b_kernel<<<std::min(num_sms(), 64), 256, 0, s>>>(w, k, n, ld, g.t.kp, g.t.nt, g.img.as<uint8_t>());
+  PG_CUDA_OK(g.img.alloc(size_t(g.t.kp / 16) * g.t.nt * w_row_bytes(arith), s));
+  pack_b_kernel<<<std::min(num_sms(), 64), 256, 0, s>>>(w, k, n, ld, g.t.kp, g.t.nt, arith, g.img.as<uint8_t>());
   PG_LAUNCH_CHECK();
   return PG_OK;
 }
@@ -816,18 +889,18 @@ struct PoolChain {
 
 // layers 1 .. own - 1 of the pooling MLP as the chain ahead of layer own
 int prepare_chain(PoolChain& c, const float* const* weights, const float* const* biases, const int32_t* dims, int own,
-                  cudaStream_t s) {
+                  int arith, cudaStream_t s) {
   c.layers = std::max(0, own - 1);
   PG_REQUIRE(c.layers <= kMaxChain, "pooling chain of %d layers", c.layers);
   if (c.layers == 0) return PG_OK;
   std::vector<WgShape> t(c.layers);
   size_t bytes = 0;
   for (int i = 0; i < c.layers; ++i) {
-    t[i] = wg_shape(dims[i + 1], dims[i + 2]);
+    t[i] = wg_shape(dims[i + 1], dims[i + 2], arith);
     PG_REQUIRE(t[i].ok, "no tensor-core shape for a %d x %d layer", dims[i + 1], dims[i + 2]);
     c.table[i] = make_int4(t[i].kp / 16, t[i].ni * 4 + t[i].ns, int(bytes), 0);
-    bytes += size_t(t[i].kp) * t[i].nt * 4;
-    c.max_chunk = std::max(c.max_chunk, uint32_t(t[i].nt) * 64u);
+    bytes += size_t(t[i].kp / 16) * t[i].nt * w_row_bytes(arith);
+    c.max_chunk = std::max(c.max_chunk, uint32_t(t[i].nt) * w_row_bytes(arith));
     if (i > 0) c.max_kp = std::max(c.max_kp, t[i].kp);
   }
   for (int i = 0; i < c.layers; ++i) {
@@ -838,7 +911,7 @@ int prepare_chain(PoolChain& c, const float* const* weights, const float* const*
   for (int i = 0; i < c.layers; ++i) {
     uint8_t* buf = c.buf.as<uint8_t>();
     pack_b_kernel<<<std::min(num_sms(), 64), 256, 0, s>>>(weights[i + 1], dims[i + 1], dims[i + 2], dims[i + 2], t[i].kp,
-                                                          t[i].nt, buf + c.table[i].z);
+                                                          t[i].nt, arith, buf + c.table[i].z);
     PG_LAUNCH_CHECK();
     pad_rows_kernel<<<2, 256, 0, s>>>(biases[i + 1], 1, dims[i + 2], t[i].nt, reinterpret_cast<float*>(buf + c.table[i].w));
     PG_LAUNCH_CHECK();
@@ -846,14 +919,15 @@ int prepare_chain(PoolChain& c, const float* const* weights, const float* const*
   return PG_OK;
 }
 
-template <int kProd, int kEpi, int NI, int NS>
+template <int kProd, int kEpi, int NI, int NS, int kArith>
 int launch_wg_cfg(const WgParams& p, size_t smem, cudaStream_t s) {
   // the GNN edge layer with an activation other than ReLU runs the twin; everything else is ReLU or linear
-  void (*kernel)(WgParams) = wg_gemm_kernel<kProd, kEpi, NI, NS>;
+  constexpr bool kF16 = kArith == ARITH_F16;
+  void (*kernel)(WgParams) = kF16 ? wg_gemm_f16_kernel<kProd, kEpi, NI, NS> : wg_gemm_kernel<kProd, kEpi, NI, NS>;
   bool any_act = false;
   if constexpr (kProd == PROD_GNN) {
     any_act = p.act != PG_ACT_RELU;
-    if (any_act) kernel = wg_gemm_act_kernel<kProd, kEpi, NI, NS>;
+    if (any_act) kernel = kF16 ? wg_gemm_act_f16_kernel<kProd, kEpi, NI, NS> : wg_gemm_act_kernel<kProd, kEpi, NI, NS>;
   }
   static bool attr_done[2] = {false, false};
   if (!attr_done[any_act]) {
@@ -873,6 +947,21 @@ int launch_wg_cfg(const WgParams& p, size_t smem, cudaStream_t s) {
   return PG_OK;
 }
 
+// the instance of g's instruction shape
+template <int kProd, int kEpi, int kArith>
+int launch_wg_shape(const WgParams& p, const PreparedGemm& g, size_t smem, cudaStream_t s) {
+  switch (g.t.ni * 4 + g.t.ns) {
+    case 64 * 4 + 1: return launch_wg_cfg<kProd, kEpi, 64, 1, kArith>(p, smem, s);
+    case 128 * 4 + 1: return launch_wg_cfg<kProd, kEpi, 128, 1, kArith>(p, smem, s);
+    case 96 * 4 + 2: return launch_wg_cfg<kProd, kEpi, 96, 2, kArith>(p, smem, s);
+    case 128 * 4 + 2: return launch_wg_cfg<kProd, kEpi, 128, 2, kArith>(p, smem, s);
+    case 152 * 4 + 2: return launch_wg_cfg<kProd, kEpi, 152, 2, kArith>(p, smem, s);
+    default: break;
+  }
+  PG_REQUIRE(false, "tensor-core kernel: no instance for N = %d", g.t.nt);
+  return PG_OK;
+}
+
 // POOL launches run the chain's layers ahead of g (none without a chain)
 template <int kProd, int kEpi>
 int launch_wg(WgParams p, const PreparedGemm& g, cudaStream_t s, const PoolChain* chain = nullptr) {
@@ -887,14 +976,15 @@ int launch_wg(WgParams p, const PreparedGemm& g, cudaStream_t s, const PoolChain
   if (kProd == PROD_POOL) {
     // ring stages hold the widest chunk of any layer; a warpgroup's A region holds layer 1's double buffer and the
     // widest activation the chain keeps on chip (the input of every later layer, up to g's own)
+    const uint32_t a_bytes = a_chunk_bytes(g.arith);
     p.chain_layers = chain ? chain->layers : 0;
-    p.stage_bytes = uint32_t(g.t.nt) * 64u;
-    p.region_bytes = 2 * kABytes;
+    p.stage_bytes = uint32_t(g.t.nt) * w_row_bytes(g.arith);
+    p.region_bytes = 2 * a_bytes;
     if (p.chain_layers > 0) {
       std::copy(chain->table, chain->table + kMaxChain, p.chain);
       p.chain_buf = chain->buf.as<uint8_t>();
       p.stage_bytes = std::max(p.stage_bytes, chain->max_chunk);
-      p.region_bytes = std::max(p.region_bytes, uint32_t(std::max(chain->max_kp, g.t.kp)) * 256u);
+      p.region_bytes = std::max(p.region_bytes, uint32_t(std::max(chain->max_kp, g.t.kp) / 16) * a_bytes);
     }
     const int ring = ring_stages(p.stage_bytes, p.region_bytes);
     p.ring_log2 = log2_ring(ring);
@@ -902,19 +992,11 @@ int launch_wg(WgParams p, const PreparedGemm& g, cudaStream_t s, const PoolChain
   }
   if (kProd == PROD_GNN) {
     p.num_tiles = ceil_div(p.num_rows, kGnnTileRows);
-    smem = gnn_smem_bytes(g.t.kp, g.t.ni);
+    smem = gnn_smem_bytes(g.t.kp, g.t.ni, g.arith);
   }
   PG_REQUIRE(smem <= 227 * 1024, "tensor-core kernel needs %zu B of shared memory", smem);
-  switch (g.t.ni * 4 + g.t.ns) {
-    case 64 * 4 + 1: return launch_wg_cfg<kProd, kEpi, 64, 1>(p, smem, s);
-    case 128 * 4 + 1: return launch_wg_cfg<kProd, kEpi, 128, 1>(p, smem, s);
-    case 96 * 4 + 2: return launch_wg_cfg<kProd, kEpi, 96, 2>(p, smem, s);
-    case 128 * 4 + 2: return launch_wg_cfg<kProd, kEpi, 128, 2>(p, smem, s);
-    case 152 * 4 + 2: return launch_wg_cfg<kProd, kEpi, 152, 2>(p, smem, s);
-    default: break;
-  }
-  PG_REQUIRE(false, "tensor-core kernel: no instance for N = %d", g.t.nt);
-  return PG_OK;
+  if (g.arith == ARITH_F16) return launch_wg_shape<kProd, kEpi, ARITH_F16>(p, g, smem, s);
+  return launch_wg_shape<kProd, kEpi, ARITH_BF16X3>(p, g, smem, s);
 }
 
 // column blocks of at most max_w (multiples of 16) covering n
@@ -938,7 +1020,7 @@ std::vector<int> column_blocks(int n, int max_w = kMaxNT) {
 // W [k, n] with row stride ld as tensor-core GEMMs of at most max_w output features, block b writing the columns
 // from col0[b]; only the first n_src columns of W are read, the pad columns past them get zero weights and bias
 int prepare_column_blocks(std::vector<PreparedGemm>& blocks, std::vector<int>& col0, const float* w, int ld,
-                          const float* bias, int k, int n_src, int n, cudaStream_t s, int max_w = kMaxNT) {
+                          const float* bias, int k, int n_src, int n, int arith, cudaStream_t s, int max_w = kMaxNT) {
   PG_REQUIRE(n >= 1, "no tensor-core shape for a %d x %d layer", k, n);
   col0 = column_blocks(n, max_w);
   blocks = std::vector<PreparedGemm>(col0.size());
@@ -946,19 +1028,19 @@ int prepare_column_blocks(std::vector<PreparedGemm>& blocks, std::vector<int>& c
     const int wn = (b + 1 < col0.size() ? col0[b + 1] : n) - col0[b];
     const int src_cols = std::max(0, std::min(wn, n_src - col0[b]));
     PG_REQUIRE(src_cols > 0, "dense layer: column block beyond the weight matrix");
-    if (int rc = prepare_gemm(blocks[b], w + col0[b], ld, bias + col0[b], k, src_cols, s)) return rc;
+    if (int rc = prepare_gemm(blocks[b], w + col0[b], ld, bias + col0[b], k, src_cols, arith, s)) return rc;
     blocks[b].n = wn;
   }
   return PG_OK;
 }
 
 // whether every column block of at most max_w of an n-wide GNN edge layer keeps its column group of W resident in
-// shared memory at padded K kp
-bool gnn_w_resident(int kp, int n, int max_w) {
+// shared memory at padded K kp in the arithmetic arith
+bool gnn_w_resident(int kp, int n, int max_w, int arith) {
   const std::vector<int> c0 = column_blocks(n, max_w);
   for (size_t b = 0; b < c0.size(); ++b) {
-    const WgShape t = wg_shape(kp, (b + 1 < c0.size() ? c0[b + 1] : n) - c0[b]);
-    if (gnn_smem_bytes(t.kp, t.ni) > 227 * 1024) return false;
+    const WgShape t = wg_shape(kp, (b + 1 < c0.size() ? c0[b + 1] : n) - c0[b], arith);
+    if (gnn_smem_bytes(t.kp, t.ni, arith) > 227 * 1024) return false;
   }
   return true;
 }
@@ -979,7 +1061,7 @@ struct PreparedFc {
 };
 
 int prepare_fc(PreparedFc& f, const float* w, int ld_src, const float* bias, int k, int n_src, int n, bool want_tc,
-               cudaStream_t s) {
+               int arith, cudaStream_t s) {
   f.k = k;
   f.n = n;
   f.n_src = n_src;
@@ -990,7 +1072,7 @@ int prepare_fc(PreparedFc& f, const float* w, int ld_src, const float* bias, int
   f.col0.clear();
   f.tc = want_tc && fc_uses_tc(k, n);
   if (!f.tc) return PG_OK;
-  return prepare_column_blocks(f.blocks, f.col0, w, ld_src, bias, k, n_src, n, s);
+  return prepare_column_blocks(f.blocks, f.col0, w, ld_src, bias, k, n_src, n, arith, s);
 }
 
 // out [m, ldo]: columns [0, n) = act(x @ W + b) (+ residual [m, n]); ldo >= n
@@ -1048,7 +1130,7 @@ struct PreparedEdge {
 };
 
 int prepare_edge(PreparedEdge& e, int mode, int c_in, const float* const* weights, const float* const* biases,
-                 const int32_t* dims, int num_layers, int act, bool want_tc, cudaStream_t s) {
+                 const int32_t* dims, int num_layers, int act, bool want_tc, int arith, cudaStream_t s) {
   PG_REQUIRE(num_layers >= 1 && num_layers <= 8, "edge MLP depth %d not in [1, 8]", num_layers);
   PG_REQUIRE(dims[0] == c_in + 3, "dims[0]=%d must equal feature channels + 3 = %d", dims[0], c_in + 3);
   PG_REQUIRE(act >= 0 && act < PG_ACT_COUNT, "edge MLP: unknown activation");
@@ -1081,13 +1163,14 @@ int prepare_edge(PreparedEdge& e, int mode, int c_in, const float* const* weight
     PG_LAUNCH_CHECK();
     const int n = dims[num_layers];
     e.chain_end = (n <= kMaxNT || num_layers == 2) ? num_layers - 1 : num_layers - 2;
-    if (int rc = prepare_chain(e.chain, weights, biases, dims, e.chain_end, s)) return rc;
+    if (int rc = prepare_chain(e.chain, weights, biases, dims, e.chain_end, arith, s)) return rc;
     if (e.chain_end < num_layers - 1) {
       const int l = e.chain_end;
-      if (int rc = prepare_gemm(e.chain_store, weights[l], dims[l + 1], biases[l], dims[l], dims[l + 1], s)) return rc;
+      if (int rc = prepare_gemm(e.chain_store, weights[l], dims[l + 1], biases[l], dims[l], dims[l + 1], arith, s))
+        return rc;
     }
     if (int rc = prepare_column_blocks(e.last, e.last_col0, weights[num_layers - 1], n, biases[num_layers - 1],
-                                       dims[num_layers - 1], n, n, s))
+                                       dims[num_layers - 1], n, n, arith, s))
       return rc;
     e.path = EDGE_POOL;
     return PG_OK;
@@ -1099,10 +1182,10 @@ int prepare_edge(PreparedEdge& e, int mode, int c_in, const float* const* weight
   // the usual column blocks (kp > 352 at 152 columns) runs as 64-wide blocks (up to kp = 848), a wider one on the fp32
   // edge kernel
   int max_w = kMaxNT;
-  if (!gnn_w_resident(e.kp, n, max_w)) max_w = 64;
-  if (!gnn_w_resident(e.kp, n, max_w)) return PG_OK;
+  if (!gnn_w_resident(e.kp, n, max_w, arith)) max_w = 64;
+  if (!gnn_w_resident(e.kp, n, max_w, arith)) return PG_OK;
   // hoisted first layer on the tensor cores too: logical N = kp, the pad columns get zero weights and bias
-  if (int rc = prepare_fc(e.p_fc, weights[0], d1, biases[0], c_in, d1, e.kp, true, s)) return rc;
+  if (int rc = prepare_fc(e.p_fc, weights[0], d1, biases[0], c_in, d1, e.kp, true, arith, s)) return rc;
   if (!e.p_fc.tc) {   // FFMA fallback writes the zero padding itself (ldo = kp)
     e.p_fc.n = d1;
     PG_REQUIRE(e.kp <= (d1 + 63) / 64 * 64, "hoisted layer: padded width %d too far from %d", e.kp, d1);
@@ -1110,7 +1193,7 @@ int prepare_edge(PreparedEdge& e, int mode, int c_in, const float* const* weight
   PG_CUDA_OK(e.w1x.alloc(sizeof(float) * 3 * e.kp, s));
   pad_rows_kernel<<<4, 256, 0, s>>>(weights[0] + int64_t(c_in) * d1, 3, d1, e.kp, e.w1x.as<float>());
   PG_LAUNCH_CHECK();
-  if (int rc = prepare_column_blocks(e.last, e.last_col0, weights[1], n, biases[1], d1, n, n, s, max_w)) return rc;
+  if (int rc = prepare_column_blocks(e.last, e.last_col0, weights[1], n, biases[1], d1, n, n, arith, s, max_w)) return rc;
   e.path = EDGE_GNN;
   return PG_OK;
 }
@@ -1352,7 +1435,7 @@ struct PreparedPredictor {
 
 // dims = {D, H, C, box_len}; layers = cls fc0, cls fc1, then per class c: fc0, fc1, fc2
 int prepare_predictor(PreparedPredictor& P, const float* const* weights, const float* const* biases,
-                      const int32_t* dims, int num_layers, int act, bool want_tc, cudaStream_t s) {
+                      const int32_t* dims, int num_layers, int act, bool want_tc, int arith, cudaStream_t s) {
   P.act = act;
   P.D = dims[0];
   P.H = dims[1];
@@ -1401,7 +1484,7 @@ int prepare_predictor(PreparedPredictor& P, const float* const* weights, const f
       P.first.emplace_back();
       P.col0.push_back(h0 * P.H);
       if (int rc = prepare_fc(P.first.back(), P.wcat.as<float>() + h0 * P.H, P.htot, P.bcat.as<float>() + h0 * P.H, P.D,
-                              nh * P.H, nh * P.H, want_tc, s))
+                              nh * P.H, nh * P.H, want_tc, arith, s))
         return rc;
       if (!P.first.back().tc) P.fused = false;   // FFMA kernel needs contiguous weights: per-layer route
     }
@@ -1413,10 +1496,13 @@ int prepare_predictor(PreparedPredictor& P, const float* const* weights, const f
     const int pos = l < 2 ? l : (l - 2) % 3;
     const int k = pos == 0 ? P.D : P.H;
     const int n = l == 1 ? P.C : (l >= 2 && pos == 2 ? P.box : P.H);
-    if (int rc = prepare_fc(P.layers[l], weights[l], n, biases[l], k, n, n, want_tc, s)) return rc;
+    if (int rc = prepare_fc(P.layers[l], weights[l], n, biases[l], k, n, n, want_tc, arith, s)) return rc;
   }
   return PG_OK;
 }
+
+// the tensor-core arithmetic of a precision code (1 BF16x3, 2 FP16); code 0 never reaches the tensor cores
+int arith_of(int precision) { return precision == 2 ? ARITH_F16 : ARITH_BF16X3; }
 
 }  // namespace
 }  // namespace pg
@@ -1433,9 +1519,9 @@ extern "C" int pg_fully_connected(const float* x, int64_t m, int32_t k, const fl
   PG_REQUIRE(act >= 0 && act < PG_ACT_COUNT, "pg_fully_connected: unknown activation %d", act);
   if (m == 0) return PG_OK;
   PG_REQUIRE(x && w && bias && out, "pg_fully_connected: null argument");
-  PG_REQUIRE(precision == 0 || precision == 1, "pg_fully_connected: unknown precision %d", precision);
+  PG_REQUIRE(precision >= 0 && precision <= 2, "pg_fully_connected: unknown precision %d", precision);
   PreparedFc f;
-  if (int rc = prepare_fc(f, w, n, bias, k, n, n, precision == 1 && pg_tc_available(), s)) return rc;
+  if (int rc = prepare_fc(f, w, n, bias, k, n, n, precision != 0 && pg_tc_available(), arith_of(precision), s)) return rc;
   return apply_fc(f, x, m, act, residual, out, n, s);
 }
 
@@ -1456,10 +1542,10 @@ extern "C" int pg_edge_mlp_max(int32_t mode, const float* features, int32_t num_
   const int act = activation_of(precision);
   PG_REQUIRE(act >= 0, "pg_edge_mlp_max: unknown activation");
   precision &= PG_PRECISION_MASK;
-  PG_REQUIRE(precision == 0 || precision == 1, "pg_edge_mlp_max: unknown precision %d", precision);
+  PG_REQUIRE(precision >= 0 && precision <= 2, "pg_edge_mlp_max: unknown precision %d", precision);
   PreparedEdge e;
   if (int rc = prepare_edge(e, mode, num_feature_channels, weights_host, biases_host, dims_host, num_layers, act,
-                            precision == 1 && num_edges > 0 && pg_tc_available(), s))
+                            precision != 0 && num_edges > 0 && pg_tc_available(), arith_of(precision), s))
     return rc;
   return apply_edge(e, features, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst, trusted, out, s);
 }
@@ -1486,7 +1572,7 @@ extern "C" int pg_layer_create(int32_t kind, const float* const* weights_host, c
   const int act = activation_of(precision);
   PG_REQUIRE(act >= 0, "pg_layer_create: unknown activation");
   precision &= ~(PG_FLAG_ACTIVATION | PG_ACT_MASK);
-  PG_REQUIRE(precision == 0 || precision == 1, "pg_layer_create: unknown precision %d", precision);
+  PG_REQUIRE(precision >= 0 && precision <= 2, "pg_layer_create: unknown precision %d", precision);
   PG_REQUIRE(kind == PG_LAYER_MLP || kind == PG_LAYER_EDGE_POOL || kind == PG_LAYER_EDGE_GNN || kind == PG_LAYER_PREDICTOR,
              "pg_layer_create: unknown kind %d", kind);
   for (int l = 0; l < num_layers; ++l) PG_REQUIRE(weights_host[l] && biases_host[l], "pg_layer_create: null weight/bias %d", l);
@@ -1494,22 +1580,23 @@ extern "C" int pg_layer_create(int32_t kind, const float* const* weights_host, c
   L->kind = kind;
   L->num_layers = num_layers;
   L->act = act;
-  const bool want_tc = precision == 1 && pg_tc_available();
+  const bool want_tc = precision != 0 && pg_tc_available();
+  const int arith = arith_of(precision);
   if (kind == PG_LAYER_MLP) {
     L->dims.assign(dims_host, dims_host + num_layers + 1);
     L->fcs.resize(num_layers);
     for (int l = 0; l < num_layers; ++l)
       if (int rc = prepare_fc(L->fcs[l], weights_host[l], dims_host[l + 1], biases_host[l], dims_host[l],
-                              dims_host[l + 1], dims_host[l + 1], want_tc, s))
+                              dims_host[l + 1], dims_host[l + 1], want_tc, arith, s))
         return rc;
   } else if (kind == PG_LAYER_EDGE_POOL || kind == PG_LAYER_EDGE_GNN) {
     L->dims.assign(dims_host, dims_host + num_layers + 1);
     if (int rc = prepare_edge(L->edge, kind == PG_LAYER_EDGE_POOL ? PG_EDGE_POOL : PG_EDGE_GNN, dims_host[0] - 3,
-                              weights_host, biases_host, dims_host, num_layers, act, want_tc, s))
+                              weights_host, biases_host, dims_host, num_layers, act, want_tc, arith, s))
       return rc;
   } else {
     L->dims.assign(dims_host, dims_host + 4);
-    if (int rc = prepare_predictor(L->pred, weights_host, biases_host, dims_host, num_layers, act, want_tc, s))
+    if (int rc = prepare_predictor(L->pred, weights_host, biases_host, dims_host, num_layers, act, want_tc, arith, s))
       return rc;
   }
   *out_layer = L.release();

@@ -41,7 +41,7 @@ charged to the step whose wait it ends:
   total          wall time of the whole loop, file writes included, divided by the number of frames
 
     python -m pointgnn_b200.run CHECKPOINT_PATH [--test] [--no-box-merge] [--no-box-score]
-           [--dataset_root_dir DIR] [--dataset_split_file FILE] [--output_dir DIR] [--precision fp32|bf16x3]
+           [--dataset_root_dir DIR] [--dataset_split_file FILE] [--output_dir DIR] [--precision fp32|bf16x3|fp16]
            [--batch_size N]
 """
 import argparse
@@ -183,8 +183,9 @@ def main(argv=None):
                         help='Path to KITTI dataset split file. Default="DATASET_ROOT_DIR/3DOP_splits/val.txt"')
     parser.add_argument('--output_dir', type=str, default='',
                         help='Path to save the detection results. Default="CHECKPOINT_PATH/eval/"')
-    parser.add_argument('--precision', type=str, default=None, choices=['fp32', 'bf16x3'],
-                        help='Arithmetic of the dense layers (default: bf16x3 on sm_90, fp32-class accuracy)')
+    parser.add_argument('--precision', type=str, default=None, choices=['fp32', 'bf16x3', 'fp16'],
+                        help='Arithmetic of the dense layers (default: bf16x3 on sm_90, fp32-class accuracy; fp16: '
+                             'one FP16 tensor-core pass, ~1e-2 on logits)')
     parser.add_argument('--batch_size', type=int, default=1,
                         help='Frames per forward pass (consecutive frames of the split; default 1)')
     args = parser.parse_args(argv)
