@@ -19,15 +19,15 @@
 //                         bias and every activation are monotone, so they commute with max: raw accumulators
 //                         are reduced across the warp's 16 rows with shuffles and each partial max is flushed
 //                         with one atomic
-//   activation wg_gemm_kernel hard-codes ReLU (linear too in the store epilogue): the kernel of every shipped
-//              config.  wg_gemm_act_kernel, the GNN edge layer with any other activation, is the same body with
+//   activation the kAnyAct = false instances hard-code ReLU (linear too in the store epilogue): the kernel of every
+//              shipped config.  kAnyAct = true, the GNN edge layer with any other activation, is the same body with
 //              activate(p.act, .) in the producer; its segment max flushes the RAW maxima with the sign-aware
 //              atomic_max_float (NONE, LeakyReLU, ELU and Tanh give negative values) and activate_rows applies
 //              act(. + b) once per output element afterwards.  Dense layers with another activation run
 //              wg_gemm_kernel linear, then activate_rows
 //   precision  BF16x3 (kArith = ARITH_BF16X3): every fp32 operand is split x = hi + lo (two BF16), and
 //              hi*hi' + lo*hi' + hi*lo' is accumulated in fp32 registers: ~2^-16 relative per product (fp32-class
-//              accuracy).  FP16 (ARITH_F16, the *_f16_kernel instances): every operand is rounded once to FP16
+//              accuracy).  FP16 (kArith = ARITH_F16): every operand is rounded once to FP16
 //              (nearest, saturating at +-65504), one wgmma per 16-k chunk, fp32 accumulation: ~2^-11 relative per
 //              operand, a third of the wgmmas and half the W bytes.  Everything that is not a tensor-core operand
 //              (the GNN layer's per-edge correction, pooling layer 0, bias, activation, segment max) stays fp32 in both
@@ -158,7 +158,7 @@ struct WgParams {
   // epilogue
   float* out;               // STORE: [num_rows, ldo];  SEGMAX: [num_dst, ldo] pre-filled with -FLT_MAX
   int ldo;
-  int act;                  // STORE: 0 linear, 1 relu;  wg_gemm_act_kernel: the GNN producer's PG_ACT_*
+  int act;                  // STORE: 0 linear, 1 relu;  kAnyAct: the GNN producer's PG_ACT_*
   const float* residual;    // STORE: optional [num_rows, ldr]
   int ldr;
   int* err;
@@ -765,39 +765,15 @@ __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
   }
 }
 
-template <int kProd, int kEpi, int NI, int NS, int kArith>
-__device__ __forceinline__ void wg_kernel_body(const WgParams& p) {
+template <int kProd, int kEpi, int NI, int NS, int kArith, bool kAnyAct>
+__global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
   if constexpr (kProd == PROD_GNN) {
     static_assert(kEpi == EPI_SEGMAX, "the GNN edge layer ends in the segment max");
-    wg_gnn_body<NI, NS, false, kArith>(p);
+    wg_gnn_body<NI, NS, kAnyAct, kArith>(p);
   } else {
+    static_assert(!kAnyAct, "any-activation instances: the GNN edge layer only");
     wg_gemm_body<kProd, kEpi, NI, NS, kArith>(p);
   }
-}
-
-template <int kProd, int kEpi, int NI, int NS>
-__global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
-  wg_kernel_body<kProd, kEpi, NI, NS, ARITH_BF16X3>(p);
-}
-
-// its own name, so that the instance count and the ptxas properties of wg_gemm_kernel stay those of the ReLU build
-template <int kProd, int kEpi, int NI, int NS>
-__global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_act_kernel(WgParams p) {
-  static_assert(kProd == PROD_GNN && kEpi == EPI_SEGMAX, "any-activation instances: the GNN edge layer only");
-  wg_gnn_body<NI, NS, true, ARITH_BF16X3>(p);
-}
-
-// the FP16 instances of the two kernels above (precision = 2): the same bodies, one operand plane and one wgmma per
-// 16-k chunk.  Names of their own, for the same reason
-template <int kProd, int kEpi, int NI, int NS>
-__global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_f16_kernel(WgParams p) {
-  wg_kernel_body<kProd, kEpi, NI, NS, ARITH_F16>(p);
-}
-
-template <int kProd, int kEpi, int NI, int NS>
-__global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_act_f16_kernel(WgParams p) {
-  static_assert(kProd == PROD_GNN && kEpi == EPI_SEGMAX, "any-activation instances: the GNN edge layer only");
-  wg_gnn_body<NI, NS, true, ARITH_F16>(p);
 }
 
 // ---- W [K, N] -> streamed B image ---------------------------------------------------------------
@@ -921,13 +897,13 @@ int prepare_chain(PoolChain& c, const float* const* weights, const float* const*
 
 template <int kProd, int kEpi, int NI, int NS, int kArith>
 int launch_wg_cfg(const WgParams& p, size_t smem, cudaStream_t s) {
-  // the GNN edge layer with an activation other than ReLU runs the twin; everything else is ReLU or linear
-  constexpr bool kF16 = kArith == ARITH_F16;
-  void (*kernel)(WgParams) = kF16 ? wg_gemm_f16_kernel<kProd, kEpi, NI, NS> : wg_gemm_kernel<kProd, kEpi, NI, NS>;
+  // the GNN edge layer with an activation other than ReLU runs the any-activation instance; everything else is ReLU
+  // or linear
+  void (*kernel)(WgParams) = wg_gemm_kernel<kProd, kEpi, NI, NS, kArith, false>;
   bool any_act = false;
   if constexpr (kProd == PROD_GNN) {
     any_act = p.act != PG_ACT_RELU;
-    if (any_act) kernel = kF16 ? wg_gemm_act_f16_kernel<kProd, kEpi, NI, NS> : wg_gemm_act_kernel<kProd, kEpi, NI, NS>;
+    if (any_act) kernel = wg_gemm_kernel<kProd, kEpi, NI, NS, kArith, true>;
   }
   static bool attr_done[2] = {false, false};
   if (!attr_done[any_act]) {
@@ -1288,7 +1264,7 @@ int apply_edge(const PreparedEdge& e, const float* features, const float* xyz_sr
   if (int rc = launch_edge(e, features, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst, out,
                            err.ptr(), s))
     return rc;
-  // wg_gemm_act_kernel left the raw maxima: the last layer's bias and activation, once per element
+  // the any-activation wg_gemm_kernel left the raw maxima: the last layer's bias and activation, once per element
   if (e.path != EDGE_FP32 && e.act != PG_ACT_RELU && num_edges > 0) {
     const int n = e.dims[e.num_layers];
     if (int rc = activate_rows(out, num_dst, n, n, e.b[e.num_layers - 1], e.act, nullptr, 0, true, s)) return rc;

@@ -3,14 +3,11 @@ reference's own script wrote, the exact 1-D k-means against scikit-learn's fits 
 pg_beam.cu without register spills, and the CLI's argument checks."""
 import itertools
 import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
-from test_kernel_build_cpu import CSRC, _make_var
+import cuda_build
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = np.load(os.path.join(ROOT, 'tests', 'golden', 'beam_downsample.npz'))
@@ -82,23 +79,13 @@ def test_exact_kmeans_degenerate_frames():
     assert np.isnan(obd.exact_kmeans_1d(np.array([np.nan]), 4)['centers']).all()
 
 
-def test_beam_kernel_builds_without_spills(tmp_path):
-    if shutil.which('make') is None:
-        pytest.skip('make not found')
-    nvcc = _make_var('NVCC')
-    if not (os.path.isfile(nvcc) or shutil.which(nvcc)):
-        pytest.skip('nvcc not found')
-    assert 'pg_beam.cu' in _make_var('SRCS').split()
-    flags = _make_var('NVCCFLAGS').split()
-    res = subprocess.run([nvcc] + flags + ['-c', 'pg_beam.cu', '-o', str(tmp_path / 'pg_beam.o')], cwd=CSRC,
-                         capture_output=True, text=True)
-    log = res.stdout + res.stderr
-    assert res.returncode == 0, log[-4000:]
-    props = re.findall(r'Function properties for (\S+)\n\s*(\d+) bytes stack frame, (\d+) bytes spill stores, '
-                       r'(\d+) bytes spill loads', log)
-    rows = [p for p in props if 'beam_' in p[0]]
-    assert len(rows) == 12, [p[0] for p in props]
-    assert all(p[2] == '0' and p[3] == '0' for p in rows), rows
+def test_beam_kernel_builds_without_spills():
+    kernels = cuda_build.kernels('pg_beam.cu')
+    assert 'pg_beam.cu' in cuda_build.make_var('SRCS').split()
+    rows = [k for k in kernels.values() if 'beam_' in k.mangled]
+    assert len(rows) == 12, [k.mangled for k in kernels.values()]
+    assert all(k.spill_stores == 0 and k.spill_loads == 0 for k in rows), [(k.name, k.spill_stores, k.spill_loads)
+                                                                           for k in rows]
 
 
 @pytest.mark.parametrize('flag,value', [('--downsample_rate', '0'), ('--downsample_rate', '-2'),

@@ -1,12 +1,5 @@
-"""The FP16 precision (code 2) without a GPU: the FP16 oracle against the fp32 goldens, the Python and run.py
-plumbing, and compile-time checks of the FP16 tensor-core instances.  pg_tc.cu built with the Makefile's flags must
-give every FP16 instance (wg_gemm_f16_kernel, wg_gemm_act_f16_kernel) wgmmas that ptxas does not serialise, no
-spills, and the GNN edge layer's FP16 instances must build A in registers (no shared-memory A store, no warpgroup
-barrier) and issue F16 HGMMAs only."""
-import os
-import re
-import shutil
-import subprocess
+"""The FP16 precision (code 2) without a GPU: the FP16 oracle against the fp32 goldens and the Python and run.py
+plumbing.  The compile-time checks of the FP16 tensor-core instances are in test_tc_build_cpu.py."""
 import tempfile
 
 import numpy as np
@@ -15,9 +8,6 @@ import pytest
 import fp16_oracle
 from conftest import ALL_CHECKPOINTS, load_golden
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, 'point-gnn_b200', 'csrc')
-F16_KERNELS = ('wg_gemm_f16_kernel', 'wg_gemm_act_f16_kernel')
 LOGIT_TOL, BOX_TOL = 2e-2, 1e-2
 
 
@@ -73,92 +63,3 @@ def test_run_parses_precision_fp16():
             run.main([d, '--precision', 'fp16'])
         with pytest.raises(SystemExit):
             run.main([d, '--precision', 'fp8'])
-
-
-# ---- compile-time checks of the FP16 instances ------------------------------------------------------------------
-def _make_var(name):
-    # the Makefile's own value of a variable (an extra makefile on stdin prints it)
-    out = subprocess.run(['make', '--no-print-directory', '-s', '-C', CSRC, '-f', 'Makefile', '-f', '-', 'print-var'],
-                         input='print-var:\n\t@echo $(%s)\n' % name, capture_output=True, text=True, check=True)
-    return out.stdout.strip()
-
-
-@pytest.fixture(scope='module')
-def build(tmp_path_factory):
-    """(ptxas log, SASS per function name) of pg_tc.cu compiled with the Makefile's flags."""
-    if shutil.which('make') is None:
-        pytest.skip('make not found')
-    nvcc = _make_var('NVCC')
-    nvcc = nvcc if os.path.isfile(nvcc) else shutil.which(nvcc)
-    if not nvcc:
-        pytest.skip('nvcc not found')
-    cuobjdump = os.path.join(os.path.dirname(nvcc), 'cuobjdump')
-    if not os.path.isfile(cuobjdump):
-        pytest.skip('cuobjdump not found next to nvcc')
-    flags = _make_var('NVCCFLAGS').split()
-    assert '-v' in flags and 'arch=compute_90a,code=sm_90a' in flags
-    obj = str(tmp_path_factory.mktemp('f16') / 'pg_tc.o')
-    res = subprocess.run([nvcc] + flags + ['-c', 'pg_tc.cu', '-o', obj], cwd=CSRC, capture_output=True, text=True)
-    log = res.stdout + res.stderr
-    assert res.returncode == 0, log[-4000:]
-    sass = subprocess.run([cuobjdump, '-sass', obj], capture_output=True, text=True, check=True).stdout
-    funcs = {}
-    for part in re.split(r'\n\s*Function : ', sass)[1:]:
-        name, _, body = part.partition('\n')
-        funcs[name.strip()] = body
-    return log, funcs
-
-
-def _is_f16(name):
-    return any(k in name for k in F16_KERNELS)
-
-
-def test_fp16_instances_not_serialised_and_no_spills(build):
-    log, _ = build
-    # C7518: wgmmas serialised for a reason in the code; C7512: for want of registers
-    serialised = [m for m in re.findall(r'\(C75(?:18|12)\)[^\n]*\'(\S+)\'', log) if _is_f16(m)]
-    assert not serialised, 'ptxas serialises the wgmmas of %d FP16 instances, e.g. %s' % (len(serialised), serialised[0])
-    props = re.findall(r'Function properties for (\S+)\n\s*(\d+) bytes stack frame, (\d+) bytes spill stores, '
-                       r'(\d+) bytes spill loads', log)
-    f16 = [p for p in props if 'wg_gemm_f16_kernel' in p[0]]
-    act = [p for p in props if 'wg_gemm_act_f16_kernel' in p[0]]
-    # as wg_gemm_kernel: 3 producers x 2 epilogues, minus GNN with the store epilogue, x 5 instruction shapes; the
-    # any-activation GNN instances x 5 shapes
-    assert len(f16) == 25 and len(act) == 5, ([p[0] for p in f16], [p[0] for p in act])
-    spilled = [p for p in f16 + act if p[2] != '0' or p[3] != '0']
-    assert not spilled, 'spills in %s' % [(p[0], p[2], p[3]) for p in spilled]
-
-
-def test_fp16_gnn_edge_layer_takes_a_from_registers(build):
-    _, funcs = build
-    # kProd is the first template argument; PROD_GNN = 1
-    gnn = {n: b for n, b in funcs.items() if any(re.search(k + r'ILi1ELi', n) for k in F16_KERNELS)}
-    assert len(gnn) == 10, sorted(gnn)
-    for name, body in gnn.items():
-        hgmma = re.findall(r'HGMMA\.\S+\s+([^;]*);', body)
-        assert hgmma, name
-        ss = [h for h in hgmma if not re.match(r'R\d+, R\d+, gdesc\[', h)]
-        assert not ss, '%s: %d of %d HGMMAs read A from shared memory, e.g. %s' % (name, len(ss), len(hgmma), ss[0])
-        sts = re.findall(r'\bSTS(?:\.\S+)?\s[^;]*;', body)
-        assert not sts, '%s stores to shared memory: %s' % (name, sts[:4])
-        counted = re.findall(r'\bBAR\.SYNC\S*\s+[^;,]+,[^;]*;', body)
-        assert not counted, '%s syncs a warpgroup: %s' % (name, counted)
-
-
-def test_fp16_instances_issue_f16_hgmmas_only(build):
-    _, funcs = build
-    # the SASS of an HGMMA names its input type after the accumulator's, except FP16, the default:
-    # "HGMMA.64x152x16.F32 ..." is FP16, "HGMMA.64x152x16.F32.BF16 ..." BF16
-    def kinds(body):
-        return [k or 'F16' for k in re.findall(r'HGMMA\.\d+x\d+x16\.F32(?:\.(\w+))?\s', body)]
-    f16 = {n: b for n, b in funcs.items() if _is_f16(n)}
-    assert len(f16) == 30, sorted(f16)
-    n_f16 = 0
-    for name, body in f16.items():
-        k = kinds(body)
-        assert k and set(k) == {'F16'}, (name, sorted(set(k)))
-        n_f16 += len(k)
-    # the BF16x3 instances stay BF16, with three HGMMAs for every FP16 one
-    bf16 = [kinds(b) for n, b in funcs.items() if 'wg_gemm_kernel' in n or 'wg_gemm_act_kernel' in n]
-    assert all(k and set(k) == {'BF16'} for k in bf16)
-    assert sum(len(k) for k in bf16) == 3 * n_f16

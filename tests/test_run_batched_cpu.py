@@ -1,14 +1,9 @@
 """Host side of the batched run.py (no GPU needed): image sizes from the PNG header, the --batch_size check, and
 the Makefile build of pg_kitti.cu without register spills."""
-import os
-import re
-import shutil
-import subprocess
-
 import numpy as np
 import pytest
 
-from test_kernel_build_cpu import CSRC, _make_var
+import cuda_build
 
 
 @pytest.mark.parametrize('width,height', [(1242, 375), (1224, 370), (1238, 374), (1241, 376)])
@@ -34,20 +29,10 @@ def test_batch_size_must_be_positive(capsys):
     assert '--batch_size' in capsys.readouterr().err
 
 
-def test_kitti_rows_kernel_builds_without_spills(tmp_path):
-    if shutil.which('make') is None:
-        pytest.skip('make not found')
-    nvcc = _make_var('NVCC')
-    if not (os.path.isfile(nvcc) or shutil.which(nvcc)):
-        pytest.skip('nvcc not found')
-    assert 'pg_kitti.cu' in _make_var('SRCS').split()
-    flags = _make_var('NVCCFLAGS').split()
-    res = subprocess.run([nvcc] + flags + ['-c', 'pg_kitti.cu', '-o', str(tmp_path / 'pg_kitti.o')], cwd=CSRC,
-                         capture_output=True, text=True)
-    log = res.stdout + res.stderr
-    assert res.returncode == 0, log[-4000:]
-    props = re.findall(r'Function properties for (\S+)\n\s*(\d+) bytes stack frame, (\d+) bytes spill stores, '
-                       r'(\d+) bytes spill loads', log)
-    rows = [p for p in props if 'kitti_rows' in p[0]]
-    assert len(rows) == 2, [p[0] for p in props]
-    assert all(p[2] == '0' and p[3] == '0' for p in rows), rows
+def test_kitti_rows_kernel_builds_without_spills():
+    kernels = cuda_build.kernels('pg_kitti.cu')
+    assert 'pg_kitti.cu' in cuda_build.make_var('SRCS').split()
+    rows = [k for k in kernels.values() if 'kitti_rows' in k.mangled]
+    assert len(rows) == 2, [k.mangled for k in kernels.values()]
+    assert all(k.spill_stores == 0 and k.spill_loads == 0 for k in rows), [(k.name, k.spill_stores, k.spill_loads)
+                                                                           for k in rows]
