@@ -367,16 +367,18 @@ PG_API int pg_fully_connected(const float* x, int64_t m, int32_t k, const float*
  *                       xyz_src = un-offset coords, xyz_dst = coords + auto-offset
  *                       (gnn.py:338-352; SURVEY fact 4)
  *   then num_layers x act(. @ W_l + b_l)       (is_logits=False, gnn.py:99-103)
- *   then out[k,:] = max over the edges of destination k   (gnn.py:362-365)
+ *   then out[k,:] = max over the edges of destination k   (gnn.py:362-365), or their sum or mean
+ *                (the aggregation field below)
  *
- *   src, dst     [E] int32; dst must be non-decreasing (CSR order, as produced by
- *                pg_radius_graph_fill and by the reference generator).
+ *   src, dst     [E] int32; dst should be non-decreasing (CSR order, as produced by
+ *                pg_radius_graph_fill and by the reference generator): edges of one destination that
+ *                are not adjacent give the same result, with more atomic flushes.
  *   dst_index    POOL: keypoint_indices [num_dst] int32 (row of xyz_dst per dst);
  *                GNN: NULL (identity)
  *   weights_host / biases_host: (host) arrays of num_layers DEVICE pointers,
  *                W_l is [dims[l], dims[l+1]] row-major, dims[0] = C_in + 3.
  *   dims_host    (host) [num_layers+1]
- *   out          [num_dst, dims[num_layers]]; empty segments get -FLT_MAX.
+ *   out          [num_dst, dims[num_layers]]; empty segments get -FLT_MAX (max) or 0 (sum, mean).
  *   precision    0 = fp32 FFMA, 1 = wgmma BF16x3, 2 = wgmma FP16 (as pg_fully_connected) for the wide
  *                layers; may be OR-ed with
  *                PG_FLAG_TRUSTED_INDICES: the caller guarantees src / dst are in range (they come from
@@ -384,9 +386,22 @@ PG_API int pg_fully_connected(const float* x, int64_t m, int32_t k, const float*
  *                read-back of the range-error flag and does not synchronise the stream.  Out-of-range
  *                indices are still clamped on the device (never dereferenced), just not reported.
  *                act is ReLU unless precision carries PG_PRECISION_ACTIVATION(code).
+ *                PG_AGGREGATION(code): the reduction over a destination's edges, the aggregation_fn
+ *                plug-ins of the reference (gnn.py:106-119):
+ *                  PG_AGG_MAX   graph_scatter_max_fn   unsorted_segment_max (the default, code 0)
+ *                  PG_AGG_SUM   graph_scatter_sum_fn   unsorted_segment_sum: empty segment -> 0
+ *                  PG_AGG_MEAN  graph_scatter_mean_fn  unsorted_segment_mean: the sum over max(count, 1)
+ *                The sum and the mean add fp32 partial sums with atomics, as TF's GPU kernel does: their
+ *                last bits may differ from run to run.  Code 3 gives PG_ERR_INVALID_ARGUMENT.
  */
 #define PG_PRECISION_MASK 0xff
 #define PG_FLAG_TRUSTED_INDICES 0x100
+#define PG_AGG_MAX 0
+#define PG_AGG_SUM 1
+#define PG_AGG_MEAN 2
+#define PG_AGG_SHIFT 10
+#define PG_AGG_MASK 0xc00
+#define PG_AGGREGATION(code) ((code) << PG_AGG_SHIFT)
 #define PG_EDGE_POOL 0
 #define PG_EDGE_GNN 1
 PG_API int pg_edge_mlp_max(int32_t mode, const float* features, int32_t num_feature_channels,
@@ -445,7 +460,8 @@ PG_API int pg_layer_destroy(pg_layer* layer);
 PG_API int pg_layer_mlp(const pg_layer* layer, const float* x, int64_t m, int32_t last_linear,
                  const float* residual, float* out, void* stream);
 
-/* pg_edge_mlp_max on a prepared edge layer; flags: 0 or PG_FLAG_TRUSTED_INDICES. */
+/* pg_edge_mlp_max on a prepared edge layer; flags: 0, PG_FLAG_TRUSTED_INDICES and / or
+ * PG_AGGREGATION(code) (as pg_edge_mlp_max).  The aggregation is chosen per call: one handle serves all three. */
 PG_API int pg_layer_edge_mlp_max(const pg_layer* layer, const float* features, const float* xyz_src,
                           const float* xyz_dst, const int32_t* dst_index, const int32_t* src,
                           const int32_t* dst, int64_t num_edges, int64_t num_src, int64_t num_dst,

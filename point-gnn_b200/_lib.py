@@ -224,6 +224,18 @@ def _activation_flags(activation):
     return PG_FLAG_ACTIVATION | (_act_code(activation) << PG_ACT_SHIFT)
 
 
+# the reduction over a destination's edges: the aggregation_fn plug-ins of the reference (gnn.py:106-119)
+AGGREGATIONS = {'max': PG_AGG_MAX, 'sum': PG_AGG_SUM, 'mean': PG_AGG_MEAN}  # noqa: F821
+
+
+def _aggregation_flags(aggregation):
+    """The flag bits that select an aggregation by name; an unknown name raises before anything is launched."""
+    if aggregation not in AGGREGATIONS:
+        raise PointGNNError(PG_ERR_INVALID_ARGUMENT, 'unknown aggregation %r (one of %s)'
+                            % (aggregation, ', '.join(AGGREGATIONS)))
+    return AGGREGATIONS[aggregation] << PG_AGG_SHIFT
+
+
 def launch_count():
     return _call('pg_launch_count')
 
@@ -487,10 +499,11 @@ def check_edges(src, dst, num_src, num_dst):
 
 
 def edge_mlp_max(mode, features, xyz_src, xyz_dst, dst_index, src, dst, num_dst, weights, biases, precision=0,
-                 trusted=False, activation=PG_ACT_RELU):
+                 trusted=False, activation=PG_ACT_RELU, aggregation='max'):
     """trusted=True: the caller vouches for the index ranges (graph_gen output / check_edges passed); the call
     then does not read the range-error flag back and does not synchronise the stream.  activation: the PG_ACT_* code
-    applied after every layer."""
+    applied after every layer.  aggregation: 'max', 'sum' or 'mean' over the edges of each destination."""
+    flags = _aggregation_flags(aggregation)
     num_layers = len(weights)
     dims = [weights[0].shape[0]] + [w.shape[1] for w in weights]
     out = torch.empty((int(num_dst), dims[-1]), dtype=torch.float32, device=features.device)
@@ -498,7 +511,7 @@ def edge_mlp_max(mode, features, xyz_src, xyz_dst, dst_index, src, dst, num_dst,
           xyz_src=xyz_src, xyz_dst=xyz_dst, dst_index=dst_index, src=src, dst=dst, num_edges=src.numel(),
           num_src=features.shape[0], num_dst=int(num_dst), weights_host=weights, biases_host=biases,
           dims_host=(c_i32 * (num_layers + 1))(*dims), num_layers=num_layers, out=out,
-          precision=int(precision) | (PG_FLAG_TRUSTED_INDICES if trusted else 0) | _activation_flags(activation))
+          precision=int(precision) | (PG_FLAG_TRUSTED_INDICES if trusted else 0) | _activation_flags(activation) | flags)
     return out
 
 
@@ -542,15 +555,16 @@ class PreparedLayer(object):
               out=out)
         return out
 
-    # fused gather -> edge MLP -> segment max (gnn.py:256-277, 338-365)
-    def edge_mlp_max(self, features, xyz_src, xyz_dst, dst_index, src, dst, num_dst, trusted=False):
+    # fused gather -> edge MLP -> segment max, sum or mean (gnn.py:256-277, 338-365)
+    def edge_mlp_max(self, features, xyz_src, xyz_dst, dst_index, src, dst, num_dst, trusted=False, aggregation='max'):
+        flags = _aggregation_flags(aggregation) | (PG_FLAG_TRUSTED_INDICES if trusted else 0)
         if features.shape[1] + 3 != self.dims[0]:
             raise ValueError('edge layer: %d feature channels + 3 != first weight rows %d'
                              % (features.shape[1], self.dims[0]))
         out = torch.empty((int(num_dst), self.dims[-1]), dtype=torch.float32, device=features.device)
         _call('pg_layer_edge_mlp_max', layer=self._handle, features=features, xyz_src=xyz_src, xyz_dst=xyz_dst,
               dst_index=dst_index, src=src, dst=dst, num_edges=src.numel(), num_src=features.shape[0],
-              num_dst=int(num_dst), out=out, flags=PG_FLAG_TRUSTED_INDICES if trusted else 0)
+              num_dst=int(num_dst), out=out, flags=flags)
         return out
 
     # ClassAwarePredictor (gnn.py:133-163) + softmax (models.py:165-168)

@@ -122,6 +122,12 @@ inline int activation_of(int32_t precision) {
   return act < PG_ACT_COUNT ? int(act) : -1;
 }
 
+// the PG_AGG_* aggregation a flag word selects (max without the field); -1 for the unused code 3
+inline int aggregation_of(int32_t flags) {
+  const int agg = (flags & PG_AGG_MASK) >> PG_AGG_SHIFT;
+  return agg <= PG_AGG_MEAN ? agg : -1;
+}
+
 // float <-> order-preserving uint: a < b iff float_to_ordered(a) < float_to_ordered(b), for any non-NaN values
 __device__ inline uint32_t float_to_ordered(float f) {
   uint32_t b = __float_as_uint(f);
@@ -157,12 +163,15 @@ int fc_fp32_launch(const float* x, int64_t m, int k, const float* w, const float
 // skip_empty leaves -FLT_MAX (an empty segment of a segment max) as it is
 int activate_rows(float* out, int64_t rows, int n, int ldo, const float* bias, int act, const float* residual, int ldr,
                   bool skip_empty, cudaStream_t s);
-// pg_edge_simt.cu: the fp32 FFMA edge MLP (activation act after every layer) + segment max into out (already
-// filled with -FLT_MAX); sets *err on an out-of-range src / dst
+// out [num_dst, n] /= max(number of edges e with dst[e] = row, 1): the segment sum -> unsorted_segment_mean.  Edges
+// whose dst is out of range are not counted
+int divide_by_segment_count(float* out, int64_t num_dst, int n, const int32_t* dst, int64_t num_edges, cudaStream_t s);
+// pg_edge_simt.cu: the fp32 FFMA edge MLP (activation act after every layer) + segment max (agg PG_AGG_MAX) or sum
+// (any other) into out (already filled with -FLT_MAX or 0); sets *err on an out-of-range src / dst
 int edge_mlp_max_fp32(int mode, const float* features, int c_in, const float* xyz_src, const float* xyz_dst,
                       const int32_t* dst_index, const int32_t* src, const int32_t* dst, int64_t num_edges,
                       int64_t num_src, int64_t num_dst, const float* const* weights, const float* const* biases,
-                      const int32_t* dims, int num_layers, int act, float* out, int* err, cudaStream_t s);
+                      const int32_t* dims, int num_layers, int act, int agg, float* out, int* err, cudaStream_t s);
 
 inline int num_sms() {
   static int sms = 0;

@@ -1,15 +1,16 @@
-// Fused per-edge MLP + destination-segment max, fp32 FFMA version (precision = 0).
+// Fused per-edge MLP + destination-segment max or sum, fp32 FFMA version (precision = 0).
 //
 // Replaces, without materialising any [E, *] tensor in HBM:
 //   PointSetPooling.apply_regular   /root/reference/models/gnn.py:256-277
 //   GraphNetAutoCenter.apply_regular /root/reference/models/gnn.py:338-365
-// (gather -> concat(feature, relative xyz) -> L x act(x@W+b) -> unsorted_segment_max).
+// (gather -> concat(feature, relative xyz) -> L x act(x@W+b) -> unsorted_segment_max, or the _sum of the
+// graph_scatter_sum_fn / graph_scatter_mean_fn plug-ins, gnn.py:111-119; the mean divides afterwards).
 //
 // One persistent CTA per SM walks 64-edge tiles.  The tile's activations ping-pong between two
 // shared-memory buffers, each layer is a register-tiled FFMA GEMM against weights streamed
 // through L1/L2 (they are a few hundred KB and stay cache resident), and the epilogue reduces the
 // tile per destination before touching HBM: because edges are grouped by destination, each
-// column thread walks the 64 rows keeping a running max and issues one atomic per (segment,
+// column thread walks the 64 rows keeping a running max (sum) and issues one atomic per (segment,
 // tile, column).  This is the bit-faithful baseline (same fp32 association order as a CPU loop);
 // the wgmma version in pg_tc.cu is the fast path.
 #include "pg_common.cuh"
@@ -44,6 +45,8 @@ struct EdgeMlpParams {
   int* err;
 };
 
+// kSum: the segment sum (atomicAdd into an output filled with 0) instead of the max
+template <bool kSum>
 __global__ void __launch_bounds__(kThreads, 1) edge_mlp_max_fp32_kernel(EdgeMlpParams p) {
   extern __shared__ __align__(16) float smem[];
   float* buf0 = smem;
@@ -131,23 +134,30 @@ __global__ void __launch_bounds__(kThreads, 1) edge_mlp_max_fp32_kernel(EdgeMlpP
       }
       __syncthreads();
     }
-    // ---- per-destination max over the tile, then one atomic per (segment, column) -------------
+    // ---- per-destination max (sum) over the tile, then one atomic per (segment, column) -------
     const float* fin = (p.num_layers & 1) ? buf1 : buf0;
     const int fstride = (p.num_layers & 1) ? p.stride1 : p.stride0;
     const int n_out = p.dims[p.num_layers];
+    auto flush = [&](int d, int c, float m) {
+      if (kSum)
+        atomicAdd(p.out + int64_t(d) * n_out + c, m);
+      else
+        atomic_max_float(p.out + int64_t(d) * n_out + c, m);
+    };
     for (int c = threadIdx.x; c < n_out; c += kThreads) {
       int cur = -1;
-      float m = -FLT_MAX;
+      float m = kSum ? 0.0f : -FLT_MAX;
       for (int r = 0; r < rows; ++r) {
         const int d = s_dst[r];
         if (d != cur) {
-          if (cur >= 0) atomic_max_float(p.out + int64_t(cur) * n_out + c, m);
+          if (cur >= 0) flush(cur, c, m);
           cur = d;
-          m = -FLT_MAX;
+          m = kSum ? 0.0f : -FLT_MAX;
         }
-        m = fmaxf(m, fin[size_t(r) * fstride + c]);
+        const float v = fin[size_t(r) * fstride + c];
+        m = kSum ? m + v : fmaxf(m, v);
       }
-      if (cur >= 0) atomic_max_float(p.out + int64_t(cur) * n_out + c, m);
+      if (cur >= 0) flush(cur, c, m);
     }
   }
 }
@@ -157,7 +167,7 @@ __global__ void __launch_bounds__(kThreads, 1) edge_mlp_max_fp32_kernel(EdgeMlpP
 int edge_mlp_max_fp32(int mode, const float* features, int c_in, const float* xyz_src, const float* xyz_dst,
                       const int32_t* dst_index, const int32_t* src, const int32_t* dst, int64_t num_edges,
                       int64_t num_src, int64_t num_dst, const float* const* weights, const float* const* biases,
-                      const int32_t* dims, int num_layers, int act, float* out, int* err, cudaStream_t s) {
+                      const int32_t* dims, int num_layers, int act, int agg, float* out, int* err, cudaStream_t s) {
   PG_REQUIRE(num_layers >= 1 && num_layers <= kMaxLayers, "edge MLP depth %d not in [1,%d]", num_layers, kMaxLayers);
   PG_REQUIRE(dims[0] == c_in + 3, "dims[0]=%d must equal feature channels + 3 = %d", dims[0], c_in + 3);
   EdgeMlpParams p{};
@@ -192,10 +202,11 @@ int edge_mlp_max_fp32(int mode, const float* features, int c_in, const float* xy
   const size_t smem = size_t(kTileE) * (p.stride0 + p.stride1) * sizeof(float);
   PG_REQUIRE(smem <= 227 * 1024 - 1024, "edge MLP widths need %zu B of shared memory (> 226 KB)", smem);
   if (num_edges > 0) {
-    PG_CUDA_OK(cudaFuncSetAttribute(edge_mlp_max_fp32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+    void (*kernel)(EdgeMlpParams) = agg == PG_AGG_MAX ? edge_mlp_max_fp32_kernel<false> : edge_mlp_max_fp32_kernel<true>;
+    PG_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
     const int64_t tiles = ceil_div(num_edges, kTileE);
     const int grid = int(std::min<int64_t>(tiles, num_sms()));
-    edge_mlp_max_fp32_kernel<<<grid, kThreads, smem, s>>>(p);
+    kernel<<<grid, kThreads, smem, s>>>(p);
     PG_LAUNCH_CHECK();
   }
   return PG_OK;

@@ -268,6 +268,29 @@ int fc_fp32_launch(const float* x, int64_t m, int k, const float* w, const float
   return PG_OK;
 }
 
+// the in-degree histogram of an edge list: one atomic per edge (the counts are integers, exact in fp32 up to 2^24)
+__global__ void count_segments_kernel(const int32_t* __restrict__ dst, int64_t num_edges, int64_t num_dst,
+                                      float* __restrict__ count) {
+  for (int64_t e = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; e < num_edges; e += int64_t(gridDim.x) * blockDim.x) {
+    const int d = __ldg(dst + e);
+    if (d >= 0 && d < num_dst) atomicAdd(count + d, 1.0f);
+  }
+}
+
+int divide_by_segment_count(float* out, int64_t num_dst, int n, const int32_t* dst, int64_t num_edges, cudaStream_t s) {
+  if (num_dst == 0 || num_edges == 0) return PG_OK;
+  Temp count;
+  PG_CUDA_OK(count.alloc(sizeof(float) * num_dst, s));
+  PG_CUDA_OK(cudaMemsetAsync(count.ptr, 0, sizeof(float) * num_dst, s));
+  count_segments_kernel<<<int(std::min<int64_t>(ceil_div(num_edges, 256), int64_t(num_sms()) * 8)), 256, 0, s>>>(
+      dst, num_edges, num_dst, count.as<float>());
+  PG_LAUNCH_CHECK();
+  const int blocks = int(std::min<int64_t>(ceil_div(num_dst * n, 256), int64_t(num_sms()) * 8));
+  divide_rows_kernel<<<blocks, 256, 0, s>>>(out, count.as<float>(), num_dst, n);
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}
+
 int activate_rows(float* out, int64_t rows, int n, int ldo, const float* bias, int act, const float* residual, int ldr,
                   bool skip_empty, cudaStream_t s) {
   if (rows == 0) return PG_OK;

@@ -19,6 +19,12 @@
 //                         bias and every activation are monotone, so they commute with max: raw accumulators
 //                         are reduced across the warp's 16 rows with shuffles and each partial max is flushed
 //                         with one atomic
+//              EPI_SEGSUM sum over the edges of each destination (the mean divides it afterwards, apply_edge): bias
+//                         and activation do not commute with a sum, so the accumulators start at the bias and act is
+//                         applied to every element in registers first; then the same reduction with + and a flush with
+//                         atomicAdd into an output filled with 0.  The order of the fp32 partial sums is not fixed:
+//                         the last bits may differ from run to run.  Its instances are wg_segsum_kernel, the same
+//                         bodies under their own name
 //   activation the kAnyAct = false instances hard-code ReLU (linear too in the store epilogue): the kernel of every
 //              shipped config.  kAnyAct = true, the GNN edge layer with any other activation, is the same body with
 //              activate(p.act, .) in the producer; its segment max flushes the RAW maxima with the sign-aware
@@ -134,7 +140,7 @@ constexpr size_t gnn_smem_bytes(int kp, int ni, int arith) {
 }
 
 enum { PROD_ROWS = 0, PROD_GNN = 1, PROD_POOL = 2 };
-enum { EPI_STORE = 0, EPI_SEGMAX = 1 };
+enum { EPI_STORE = 0, EPI_SEGMAX = 1, EPI_SEGSUM = 2 };
 
 struct WgParams {
   // A producer
@@ -156,7 +162,7 @@ struct WgParams {
   const float* bias;        // [NT] zero padded
   int n;                    // real output columns
   // epilogue
-  float* out;               // STORE: [num_rows, ldo];  SEGMAX: [num_dst, ldo] pre-filled with -FLT_MAX
+  float* out;               // STORE: [num_rows, ldo];  SEGMAX / SEGSUM: [num_dst, ldo] pre-filled with -FLT_MAX / 0
   int ldo;
   int act;                  // STORE: 0 linear, 1 relu;  kAnyAct: the GNN producer's PG_ACT_*
   const float* residual;    // STORE: optional [num_rows, ldr]
@@ -185,10 +191,12 @@ __device__ __forceinline__ float layer_act(int act, float x) {
   return kAnyAct ? activate(act, x) : fmaxf(x, 0.0f);
 }
 
-template <bool kAnyAct>
+template <int kEpi, bool kAnyAct>
 __device__ __forceinline__ void seg_flush(const WgParams& p, int d, int col, float m) {
   float* dst = p.out + int64_t(d) * p.ldo + col;
-  if (kAnyAct) {
+  if (kEpi == EPI_SEGSUM) {
+    atomicAdd(dst, m);   // a partial sum of act(acc + b)
+  } else if (kAnyAct) {
     // the raw maximum, which may be negative: the sign-aware max, still one atomic (bias and activation later)
     atomic_max_float(dst, m);
   } else {
@@ -325,12 +333,38 @@ __device__ __forceinline__ void rs_k_loop(int lk, Frag&& frag, Chunk&& chunk) {
   }
 }
 
-// Segment max of one warpgroup's 64 x (NI x NS) accumulators: output columns col0 + [0, NI x NS), rows r0 (the
-// thread's first, as in RowA) and r0 + 8
-template <int NI, int NS, bool kAnyAct>
+// The segment sum's accumulators start at the bias (value 4 jj + 2 h + c holds column col0 + 8 jj + cq + c) and its
+// first wgmma accumulates onto them: the epilogue then applies the activation alone, with no bias in registers beside
+// the accumulators (bias loads there spill the car GNN instance)
+template <int NI>
+__device__ __forceinline__ void acc_from_bias(const WgParams& p, float (&acc)[NI / 2], int col0, int lane) {
+  const int cq = (lane & 3) * 2;
+#pragma unroll
+  for (int jj = 0; jj < NI / 8; ++jj) {
+    const float2 b = ldg2(p.bias + col0 + jj * 8 + cq);
+    acc[4 * jj] = acc[4 * jj + 2] = b.x;
+    acc[4 * jj + 1] = acc[4 * jj + 3] = b.y;
+  }
+  // the accumulators are defined here, ahead of the wgmma pipeline: otherwise ptxas may place their moves inside a
+  // pooling launch's first stage and serialise its wgmmas (C7515)
+#pragma unroll
+  for (int v = 0; v < NI / 2; ++v) asm volatile("" : "+f"(acc[v])::"memory");
+}
+
+// Segment max (kEpi = EPI_SEGMAX) or sum (EPI_SEGSUM) of one warpgroup's 64 x (NI x NS) accumulators: output
+// columns col0 + [0, NI x NS), rows r0 (the thread's first, as in RowA) and r0 + 8
+template <int NI, int NS, bool kAnyAct, int kEpi>
 __device__ __forceinline__ void seg_epilogue(const WgParams& p, const float (&acc)[NS][NI / 2], int64_t r0, int lane,
                                              int col0) {
+  constexpr bool kSum = kEpi == EPI_SEGSUM;
+  auto combine = [](float a, float b) { return kSum ? a + b : fmaxf(a, b); };
   const int cq = (lane & 3) * 2;
+  // what an edge row contributes to the reduction: the raw accumulator (max), or act(acc) of an accumulator that
+  // started at the bias (acc_from_bias), since bias and activation do not commute with a sum
+  auto value = [&](int i, int jj, int h, int c) {
+    const float a = acc[i][4 * jj + 2 * h + c];
+    return kSum ? layer_act<kAnyAct>(p.act, a) : a;
+  };
   int d[2];
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -348,8 +382,9 @@ __device__ __forceinline__ void seg_epilogue(const WgParams& p, const float (&ac
   if (__all_sync(0xffffffffu, d[0] == dw && d[1] == dw) && dw >= 0) {
     // the warp's 16 rows are one destination.  Value v of a thread is column (v / 2) * 8 + cq + v % 2; the 8
     // lanes sharing cq (lane bits 4, 3, 2) reduce-scatter their V values in three halving exchanges, after which
-    // every lane holds the full maxima of V / 8 (rounded up or down) of them and all 32 lanes flush.  V is padded with
-    // -FLT_MAX values to VP, a multiple of 4, so that the first two exchanges halve evenly (V = 38 at NI = 152, NS = 1)
+    // every lane holds the full maxima (sums) of V / 8 (rounded up or down) of them and all 32 lanes flush.  V is padded
+    // with -FLT_MAX (0) values to VP, a multiple of 4, so that the first two exchanges halve evenly (V = 38 at NI = 152,
+    // NS = 1)
     constexpr int V = NI * NS / 4, VP = (V + 3) / 4 * 4, L1 = VP / 2, L2 = VP / 4, L3 = (L2 + 1) / 2;
     float m[VP];
 #pragma unroll
@@ -357,45 +392,57 @@ __device__ __forceinline__ void seg_epilogue(const WgParams& p, const float (&ac
 #pragma unroll
       for (int jj = 0; jj < NI / 8; ++jj)
 #pragma unroll
-        for (int c = 0; c < 2; ++c) m[(i * (NI / 8) + jj) * 2 + c] = fmaxf(acc[i][4 * jj + c], acc[i][4 * jj + 2 + c]);
+        for (int c = 0; c < 2; ++c) m[(i * (NI / 8) + jj) * 2 + c] = combine(value(i, jj, 0, c), value(i, jj, 1, c));
 #pragma unroll
-    for (int v = V; v < VP; ++v) m[v] = -FLT_MAX;
+    for (int v = V; v < VP; ++v) m[v] = kSum ? 0.0f : -FLT_MAX;
     const bool b4 = lane & 16, b3 = lane & 8, b2 = lane & 4;
     // a lane with the bit set keeps the upper part, its partner the lower; each sends the part it gives up
 #pragma unroll
     for (int k = 0; k < L1; ++k) {
       const float keep = b4 ? m[k + L1] : m[k], give = b4 ? m[k] : m[k + L1];
-      m[k] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, give, 16));
+      m[k] = combine(keep, __shfl_xor_sync(0xffffffffu, give, 16));
     }
 #pragma unroll
     for (int k = 0; k < L2; ++k) {
       const float keep = b3 ? m[k + L2] : m[k], give = b3 ? m[k] : m[k + L2];
-      m[k] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, give, 8));
+      m[k] = combine(keep, __shfl_xor_sync(0xffffffffu, give, 8));
     }
 #pragma unroll
     for (int k = 0; k < L3; ++k) {
       const float up = k + L3 < L2 ? m[k + L3] : m[k];   // L2 odd: the upper part is one value shorter
       const float keep = b2 ? up : m[k], give = b2 ? m[k] : up;
-      m[k] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, give, 4));
+      m[k] = combine(keep, __shfl_xor_sync(0xffffffffu, give, 4));
     }
     const int v0 = (b4 ? L1 : 0) + (b3 ? L2 : 0) + (b2 ? L3 : 0), nv = b2 ? L2 - L3 : L3;
 #pragma unroll
     for (int k = 0; k < L3; ++k) {
       const int v = v0 + k, col = col0 + (v >> 1) * 8 + cq + (v & 1);
-      if (k < nv && v < V && col < p.n) seg_flush<kAnyAct>(p, dw, col, m[k]);
+      if (k < nv && v < V && col < p.n) seg_flush<kEpi, kAnyAct>(p, dw, col, m[k]);
     }
   } else {
-    // segmented max down each 8-row half (rows of one destination are contiguous); the first row of
-    // every run flushes the run's max.  Column by column, both halves: each accumulator dies once used
+    // segmented max (sum) down each 8-row half; the first row of every run flushes the run's max (sum).  Column by
+    // column, both halves: each accumulator dies once used
     bool head[2];
-    bool same[2][3];   // the row 4 << s lanes down has the same destination
+    bool same[2][3];   // the row 4 << s lanes down joins this row's partial
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int up = __shfl_up_sync(0xffffffffu, d[h], 4);
       head[h] = d[h] >= 0 && (lane < 4 || up != d[h]);
+      if (kSum) {
+        // every row must reach exactly one flush, even in an edge list not grouped by destination: the rows up to
+        // 1 << s further down join only when every row in between has this destination too.  One ballot of "the next
+        // row continues this row's run": bit 4 j of m is that flag of the thread's row + j
+        const bool next = __shfl_down_sync(0xffffffffu, d[h], 4) == d[h] && lane + 4 < 32;
+        const uint32_t m = __ballot_sync(0xffffffffu, next) >> (lane & ~3);
+        same[h][0] = (m & 0x1u) != 0;
+        same[h][1] = (m & 0x11u) == 0x11u;
+        same[h][2] = (m & 0x1111u) == 0x1111u;
+      } else {
+        // rows of one destination are contiguous, and a row seen twice does not change a max
 #pragma unroll
-      for (int s = 0; s < 3; ++s)
-        same[h][s] = __shfl_down_sync(0xffffffffu, d[h], 4 << s) == d[h] && lane + (4 << s) < 32;
+        for (int s = 0; s < 3; ++s)
+          same[h][s] = __shfl_down_sync(0xffffffffu, d[h], 4 << s) == d[h] && lane + (4 << s) < 32;
+      }
     }
 #pragma unroll
     for (int i = 0; i < NS; ++i)
@@ -405,14 +452,14 @@ __device__ __forceinline__ void seg_epilogue(const WgParams& p, const float (&ac
         for (int c = 0; c < 2; ++c)
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            float m = acc[i][4 * jj + 2 * h + c];
+            float m = value(i, jj, h, c);
 #pragma unroll
             for (int s = 0; s < 3; ++s) {
               const float o = __shfl_down_sync(0xffffffffu, m, 4 << s);
-              if (same[h][s]) m = fmaxf(m, o);
+              if (same[h][s]) m = combine(m, o);
             }
             const int col = col0 + i * NI + jj * 8 + cq + c;
-            if (head[h] && col < p.n) seg_flush<kAnyAct>(p, d[h], col, m);
+            if (head[h] && col < p.n) seg_flush<kEpi, kAnyAct>(p, d[h], col, m);
           }
   }
 }
@@ -473,7 +520,7 @@ struct GnnGather {
   }
 };
 
-template <int NI, int NS, bool kAnyAct, int kArith>
+template <int kEpi, int NI, int NS, bool kAnyAct, int kArith>
 __device__ __forceinline__ void wg_gnn_body(const WgParams& p) {
   constexpr int NT = NI * NS;
   constexpr uint32_t kSlice = uint32_t(NI) * 32u;   // one group's part of one plane (hi, lo or FP16) of a 16-k chunk
@@ -517,6 +564,7 @@ __device__ __forceinline__ void wg_gnn_body(const WgParams& p) {
   for (int tile = first; tile < num_tiles; tile += stride) {
     const int64_t row0 = int64_t(tile) * kGnnTileRows;
     float acc[1][NI / 2];
+    if constexpr (kEpi == EPI_SEGSUM) acc_from_bias<NI>(p, acc[0], group * NI, lane);
     auto frag = [&](int kc, uint32_t (&hi)[4], uint32_t (&lo)[4]) {
       float2 q[4];
       gather.take(q);
@@ -527,14 +575,14 @@ __device__ __forceinline__ void wg_gnn_body(const WgParams& p) {
       wgmma_fence();
       const uint32_t b = w_base + uint32_t(kc) * kPlanes * kSlice;
       const uint64_t b_hi = make_smem_desc(b, 128, 256), b_lo = make_smem_desc(b + kSlice, 128, 256);
-      mma_rs<kArith, NI>(acc[0], hi, lo, b_hi, b_lo, kc > 0 ? 1 : 0);
+      mma_rs<kArith, NI>(acc[0], hi, lo, b_hi, b_lo, kc > 0 || kEpi == EPI_SEGSUM ? 1 : 0);
       wgmma_commit();
       wgmma_wait<1>();                    // chunk kc - 1 complete: its A fragment is free
     });
     // the next tile's context while the last wgmmas run; its first chunks of P are already in flight
     a.context(p, row0 + int64_t(stride) * kGnnTileRows, warp, lane);
     wgmma_wait<0>();
-    seg_epilogue<NI, 1, kAnyAct>(p, acc, row0 + warp * 16 + (lane >> 2), lane, group * NI);
+    seg_epilogue<NI, 1, kAnyAct, kEpi>(p, acc, row0 + warp * 16 + (lane >> 2), lane, group * NI);
   }
 }
 
@@ -611,7 +659,8 @@ __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
     // ---- one layer's loop over 16-k chunks into acc[ns][ni / 2] --------------------------------------
     // streamed: chunk kc + 1's A fragment is built while chunk kc's wgmmas run.  Otherwise the previous on-chip layer
     // left the whole A in the region, chunk kc at kc * kABytes
-    auto mma_layer = [&](auto& lacc, int lk, bool streamed) {
+    // keep: the first chunk accumulates onto lacc (the segment sum's bias) instead of overwriting it
+    auto mma_layer = [&](auto& lacc, int lk, bool streamed, bool keep = false) {
       using Acc = std::remove_reference_t<decltype(lacc)>;
       constexpr int ns = int(std::extent<Acc, 0>::value), ni = 2 * int(std::extent<Acc, 1>::value);
       // chunk kc's wgmmas on W stage g, A hi / lo (FP16: hi only) from registers (uint32_t[4]) or shared memory
@@ -626,9 +675,9 @@ __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
           const uint64_t b_hi = make_smem_desc(b_base + uint32_t(i * ni) * 32u, 128, 256);
           const uint64_t b_lo = make_smem_desc(b_base + uint32_t(ni * ns) * 32u + uint32_t(i * ni) * 32u, 128, 256);
           if constexpr (std::is_same_v<std::decay_t<decltype(a_hi)>, uint64_t>)
-            mma_ss<kArith, ni>(lacc[i], a_hi, a_lo, b_hi, b_lo, kc > 0 ? 1 : 0);
+            mma_ss<kArith, ni>(lacc[i], a_hi, a_lo, b_hi, b_lo, kc > 0 || keep ? 1 : 0);
           else
-            mma_rs<kArith, ni>(lacc[i], a_hi, a_lo, b_hi, b_lo, kc > 0 ? 1 : 0);
+            mma_rs<kArith, ni>(lacc[i], a_hi, a_lo, b_hi, b_lo, kc > 0 || keep ? 1 : 0);
         }
         wgmma_commit();
         wgmma_wait<1>();                  // chunk kc - 1 complete: its A fragment and W stage are free
@@ -730,12 +779,15 @@ __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
     // every accumulator is defined before its layer (the wgmmas read it, if only to scale it by 0): otherwise the
     // values of the previous tile would stay live through the on-chip layers, next to their accumulators
     float acc[NS][NI / 2];
-    if (kProd == PROD_POOL)
+    if (kEpi == EPI_SEGSUM)
+#pragma unroll
+      for (int i = 0; i < NS; ++i) acc_from_bias<NI>(p, acc[i], i * NI, lane);
+    else if (kProd == PROD_POOL)
 #pragma unroll
       for (int i = 0; i < NS; ++i)
 #pragma unroll
         for (int v = 0; v < NI / 2; ++v) acc[i][v] = 0.0f;
-    mma_layer(acc, nk, nl == 0);
+    mma_layer(acc, nk, nl == 0, kEpi == EPI_SEGSUM);
     // ---- epilogue ----------------------------------------------------------------------------------
     const int64_t r0 = tile * kTileRows + wgi * 64 + warp * 16 + (lane >> 2);
     const int cq = (lane & 3) * 2;
@@ -760,20 +812,43 @@ __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
             }
       }
     } else {
-      seg_epilogue<NI, NS, false>(p, acc, r0, lane, 0);
+      seg_epilogue<NI, NS, false, kEpi>(p, acc, r0, lane, 0);
     }
   }
 }
 
 template <int kProd, int kEpi, int NI, int NS, int kArith, bool kAnyAct>
-__global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
+__device__ __forceinline__ void wg_body(const WgParams& p) {
   if constexpr (kProd == PROD_GNN) {
-    static_assert(kEpi == EPI_SEGMAX, "the GNN edge layer ends in the segment max");
-    wg_gnn_body<NI, NS, kAnyAct, kArith>(p);
+    static_assert(kEpi != EPI_STORE, "the GNN edge layer ends in a segment reduction");
+    wg_gnn_body<kEpi, NI, NS, kAnyAct, kArith>(p);
   } else {
     static_assert(!kAnyAct, "any-activation instances: the GNN edge layer only");
     wg_gemm_body<kProd, kEpi, NI, NS, kArith>(p);
   }
+}
+
+template <int kProd, int kEpi, int NI, int NS, int kArith, bool kAnyAct>
+__global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
+  static_assert(kEpi != EPI_SEGSUM, "the segment-sum instances are wg_segsum_kernel");
+  wg_body<kProd, kEpi, NI, NS, kArith, kAnyAct>(p);
+}
+
+// The segment sum (EPI_SEGSUM) of the edge layers: wg_gemm_kernel's bodies with the sum epilogue, as a kernel of its
+// own so that the max's instances stay exactly the set they were, and the sum's are counted and checked as one family
+// (tests/test_aggregation_build_cpu.py)
+template <int kProd, int NI, int NS, int kArith, bool kAnyAct>
+__global__ void __launch_bounds__(kWgThreads, 1) wg_segsum_kernel(WgParams p) {
+  wg_body<kProd, EPI_SEGSUM, NI, NS, kArith, kAnyAct>(p);
+}
+
+// the __global__ instance of a launch: wg_gemm_kernel, or wg_segsum_kernel for the segment sum
+template <int kProd, int kEpi, int NI, int NS, int kArith, bool kAnyAct>
+void (*wg_kernel())(WgParams) {
+  if constexpr (kEpi == EPI_SEGSUM)
+    return wg_segsum_kernel<kProd, NI, NS, kArith, kAnyAct>;
+  else
+    return wg_gemm_kernel<kProd, kEpi, NI, NS, kArith, kAnyAct>;
 }
 
 // ---- W [K, N] -> streamed B image ---------------------------------------------------------------
@@ -899,11 +974,11 @@ template <int kProd, int kEpi, int NI, int NS, int kArith>
 int launch_wg_cfg(const WgParams& p, size_t smem, cudaStream_t s) {
   // the GNN edge layer with an activation other than ReLU runs the any-activation instance; everything else is ReLU
   // or linear
-  void (*kernel)(WgParams) = wg_gemm_kernel<kProd, kEpi, NI, NS, kArith, false>;
+  void (*kernel)(WgParams) = wg_kernel<kProd, kEpi, NI, NS, kArith, false>();
   bool any_act = false;
   if constexpr (kProd == PROD_GNN) {
     any_act = p.act != PG_ACT_RELU;
-    if (any_act) kernel = wg_gemm_kernel<kProd, kEpi, NI, NS, kArith, true>;
+    if (any_act) kernel = wg_kernel<kProd, kEpi, NI, NS, kArith, true>();
   }
   static bool attr_done[2] = {false, false};
   if (!attr_done[any_act]) {
@@ -919,7 +994,7 @@ int launch_wg_cfg(const WgParams& p, size_t smem, cudaStream_t s) {
     grid = int(std::min<int64_t>(num_sms() / NS, ceil_div(p.num_tiles, kGnnWarpgroups))) * NS;
   kernel<<<grid, kWgThreads, smem, s>>>(p);
   PG_LAUNCH_CHECK();
-  g_tc_launches[kEpi == EPI_SEGMAX ? 0 : 1].fetch_add(1, std::memory_order_relaxed);
+  g_tc_launches[kEpi == EPI_STORE ? 1 : 0].fetch_add(1, std::memory_order_relaxed);
   return PG_OK;
 }
 
@@ -1174,26 +1249,29 @@ int prepare_edge(PreparedEdge& e, int mode, int c_in, const float* const* weight
   return PG_OK;
 }
 
-// the segment-max layer over all column blocks; p carries the producer's inputs
+// the segment-reduction layer over all column blocks: the max (agg PG_AGG_MAX) or the sum; p carries the producer's
+// inputs
 template <int kProd>
-int apply_last(const PreparedEdge& e, WgParams p, int n, float* out, cudaStream_t s) {
+int apply_last(const PreparedEdge& e, WgParams p, int n, int agg, float* out, cudaStream_t s) {
   for (size_t b = 0; b < e.last.size(); ++b) {
     p.out = out + e.last_col0[b];
     p.ldo = n;
-    if (int rc = launch_wg<kProd, EPI_SEGMAX>(p, e.last[b], s, &e.chain)) return rc;
+    const int rc = agg == PG_AGG_MAX ? launch_wg<kProd, EPI_SEGMAX>(p, e.last[b], s, &e.chain)
+                                     : launch_wg<kProd, EPI_SEGSUM>(p, e.last[b], s, &e.chain);
+    if (rc) return rc;
   }
   return PG_OK;
 }
 
-// the launches of one edge call: the segment max into out (pre-filled with -FLT_MAX); an out-of-range src / dst
-// sets *err
+// the launches of one edge call: the segment max (sum) into out (pre-filled with -FLT_MAX or 0); an out-of-range
+// src / dst sets *err
 int launch_edge(const PreparedEdge& e, const float* features, const float* xyz_src, const float* xyz_dst,
                 const int32_t* dst_index, const int32_t* src, const int32_t* dst, int64_t num_edges, int64_t num_src,
-                int64_t num_dst, float* out, int* err, cudaStream_t s) {
+                int64_t num_dst, int agg, float* out, int* err, cudaStream_t s) {
   const int n = e.dims[e.num_layers];
   if (e.path == EDGE_FP32 || num_edges == 0)
     return edge_mlp_max_fp32(e.mode, features, e.c_in, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst,
-                             e.w.data(), e.b.data(), e.dims.data(), e.num_layers, e.act, out, err, s);
+                             e.w.data(), e.b.data(), e.dims.data(), e.num_layers, e.act, agg, out, err, s);
   WgParams p{};
   p.xyz_src = xyz_src;
   p.xyz_dst = xyz_dst;
@@ -1209,7 +1287,7 @@ int launch_edge(const PreparedEdge& e, const float* features, const float* xyz_s
     p.src = src;
     p.dst = dst;
     p.num_rows = num_edges;
-    if (e.chain_end == L - 1) return apply_last<PROD_POOL>(e, p, n, out, s);
+    if (e.chain_end == L - 1) return apply_last<PROD_POOL>(e, p, n, agg, out, s);
     // the last layer is wider than one launch: the chain stores its input once, and its column blocks read it back.
     // The stored rows are bounded by slicing the edge list (a destination whose edges straddle two slices is merged
     // by the atomic max like any tile boundary)
@@ -1235,7 +1313,7 @@ int launch_edge(const PreparedEdge& e, const float* features, const float* xyz_s
       r.dst = dst + e0;
       r.num_dst = num_dst;
       r.err = err;
-      if (int rc = apply_last<PROD_ROWS>(e, r, n, out, s)) return rc;
+      if (int rc = apply_last<PROD_ROWS>(e, r, n, agg, out, s)) return rc;
     }
     return PG_OK;
   }
@@ -1250,25 +1328,27 @@ int launch_edge(const PreparedEdge& e, const float* features, const float* xyz_s
   p.dst = dst;
   p.num_rows = num_edges;
   p.act = e.act;
-  return apply_last<PROD_GNN>(e, p, n, out, s);
+  return apply_last<PROD_GNN>(e, p, n, agg, out, s);
 }
 
-// one edge call on either route: the error word, the -FLT_MAX fill of out, the launches, and the read-back of the
-// error word unless the caller vouched for the indices (trusted: no read-back, no synchronisation)
+// one edge call on either route: the error word, the fill of out (-FLT_MAX for the max, 0 for the sum and the mean),
+// the launches, the division of the mean, and the read-back of the error word unless the caller vouched for the
+// indices (trusted: no read-back, no synchronisation)
 int apply_edge(const PreparedEdge& e, const float* features, const float* xyz_src, const float* xyz_dst,
                const int32_t* dst_index, const int32_t* src, const int32_t* dst, int64_t num_edges, int64_t num_src,
-               int64_t num_dst, bool trusted, float* out, cudaStream_t s) {
+               int64_t num_dst, bool trusted, int agg, float* out, cudaStream_t s) {
+  const int n = e.dims[e.num_layers];
   ErrorWord err;
   if (int rc = err.init(s)) return rc;
-  if (int rc = fill_async(out, num_dst * e.dims[e.num_layers], -FLT_MAX, s)) return rc;
-  if (int rc = launch_edge(e, features, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst, out,
+  if (int rc = fill_async(out, num_dst * n, agg == PG_AGG_MAX ? -FLT_MAX : 0.0f, s)) return rc;
+  if (int rc = launch_edge(e, features, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst, agg, out,
                            err.ptr(), s))
     return rc;
   // the any-activation wg_gemm_kernel left the raw maxima: the last layer's bias and activation, once per element
-  if (e.path != EDGE_FP32 && e.act != PG_ACT_RELU && num_edges > 0) {
-    const int n = e.dims[e.num_layers];
+  if (agg == PG_AGG_MAX && e.path != EDGE_FP32 && e.act != PG_ACT_RELU && num_edges > 0)
     if (int rc = activate_rows(out, num_dst, n, n, e.b[e.num_layers - 1], e.act, nullptr, 0, true, s)) return rc;
-  }
+  if (agg == PG_AGG_MEAN)
+    if (int rc = divide_by_segment_count(out, num_dst, n, dst, num_edges, s)) return rc;
   int h = 0;
   if (int rc = err.read(&h, trusted, s)) return rc;
   PG_REQUIRE(h == 0, "edge index out of range (src in [0,%lld), dst in [0,%lld))", (long long)num_src,
@@ -1517,13 +1597,16 @@ extern "C" int pg_edge_mlp_max(int32_t mode, const float* features, int32_t num_
   const bool trusted = (precision & PG_FLAG_TRUSTED_INDICES) != 0;
   const int act = activation_of(precision);
   PG_REQUIRE(act >= 0, "pg_edge_mlp_max: unknown activation");
+  const int agg = aggregation_of(precision);
+  PG_REQUIRE(agg >= 0, "pg_edge_mlp_max: unknown aggregation");
   precision &= PG_PRECISION_MASK;
   PG_REQUIRE(precision >= 0 && precision <= 2, "pg_edge_mlp_max: unknown precision %d", precision);
   PreparedEdge e;
   if (int rc = prepare_edge(e, mode, num_feature_channels, weights_host, biases_host, dims_host, num_layers, act,
                             precision != 0 && num_edges > 0 && pg_tc_available(), arith_of(precision), s))
     return rc;
-  return apply_edge(e, features, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst, trusted, out, s);
+  return apply_edge(e, features, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst, trusted, agg, out,
+                    s);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -1621,8 +1704,10 @@ extern "C" int pg_layer_edge_mlp_max(const pg_layer* layer, const float* feature
   PG_REQUIRE((features && xyz_src && xyz_dst && src && dst) || num_edges == 0, "pg_layer_edge_mlp_max: null input");
   PG_REQUIRE(layer->kind == PG_LAYER_EDGE_GNN || dst_index != nullptr || num_edges == 0,
              "pg_layer_edge_mlp_max: POOL mode needs keypoint indices");
+  const int agg = aggregation_of(flags);
+  PG_REQUIRE(agg >= 0, "pg_layer_edge_mlp_max: unknown aggregation");
   return apply_edge(layer->edge, features, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst,
-                    (flags & PG_FLAG_TRUSTED_INDICES) != 0, out, s);
+                    (flags & PG_FLAG_TRUSTED_INDICES) != 0, agg, out, s);
 }
 
 extern "C" int pg_layer_predictor(const pg_layer* layer, const float* x, int64_t m, float* logits, float* boxes,

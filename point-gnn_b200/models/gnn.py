@@ -8,9 +8,10 @@ every fully-connected layer draws the next ``fully_connected[_i]`` name of its s
 weights are looked up in the active ``VariableStore`` (name -> CUDA tensor).
 
 When a layer is built from the default plugins (``multi_layer_neural_network_fn`` +
-``graph_scatter_max_fn``, i.e. every layer type models.py:49-74 registers) its gather /
-concat / edge-MLP / segment-max chain runs as ONE fused kernel (``pg_edge_mlp_max``); any
-other plugin combination runs the same chain op by op, still on the GPU.
+``graph_scatter_max_fn``, i.e. every layer type models.py:49-74 registers), or with this module's
+``graph_scatter_sum_fn`` / ``graph_scatter_mean_fn`` as its aggregation, its gather / concat /
+edge-MLP / segment-reduction chain runs as ONE fused kernel (``pg_edge_mlp_max``); any other
+plugin combination runs the same chain op by op, still on the GPU.
 """
 import contextlib
 import threading
@@ -180,16 +181,22 @@ def graph_scatter_max_fn(point_features, point_centers, num_centers):
 
 
 def graph_scatter_sum_fn(point_features, point_centers, num_centers):
-    """gnn.py:111-114 (tf.math.unsorted_segment_sum; empty segment -> 0).  No shipped config selects it; as an
-    ``aggregation_fn`` plug-in it runs the layer op by op (the fused kernels implement the max)."""
+    """gnn.py:111-114 (tf.math.unsorted_segment_sum; empty segment -> 0).  No shipped config selects it; as the
+    ``aggregation_fn`` of PointSetPooling or GraphNetAutoCenter it runs in the fused edge kernels, which add fp32
+    partial sums with atomics: the last bits may differ from run to run, as with TF's GPU kernel."""
     centers = point_centers.reshape(-1).to(torch.int32).contiguous()
     return _lib.scatter_sum(point_features.contiguous(), centers, int(num_centers))
 
 
 def graph_scatter_mean_fn(point_features, point_centers, num_centers):
-    """gnn.py:116-119 (tf.math.unsorted_segment_mean; empty segment -> 0)."""
+    """gnn.py:116-119 (tf.math.unsorted_segment_mean; empty segment -> 0).  As an ``aggregation_fn`` plug-in it
+    runs in the fused edge kernels: their segment sum, divided by each destination's edge count."""
     centers = point_centers.reshape(-1).to(torch.int32).contiguous()
     return _lib.scatter_sum(point_features.contiguous(), centers, int(num_centers), mean=True)
+
+
+# the aggregation_fn plug-ins the fused edge kernels run, by identity (a user's own function runs op by op)
+_FUSED_AGGREGATIONS = {graph_scatter_max_fn: 'max', graph_scatter_sum_fn: 'sum', graph_scatter_mean_fn: 'mean'}
 
 
 def _i32(t):
@@ -271,9 +278,10 @@ class PointSetPooling(object):
         self._output_fn = output_fn
 
     def _fusable(self, normalization_type):
-        return (self._point_feature_fn is multi_layer_neural_network_fn
-                and self._aggregation_fn is graph_scatter_max_fn
-                and normalization_type == 'NONE')
+        """-> the fused kernels' aggregation name, or None for the op-by-op route."""
+        if self._point_feature_fn is multi_layer_neural_network_fn and normalization_type == 'NONE':
+            return _FUSED_AGGREGATIONS.get(self._aggregation_fn)
+        return None
 
     def apply_regular(self, point_features, point_coordinates, keypoint_indices, set_indices,
                       point_MLP_depth_list=None, point_MLP_normalization_type='fused_BN_center',
@@ -282,7 +290,8 @@ class PointSetPooling(object):
         num_keypoints = keypoint_indices.shape[0]
         src, dst = set_indices[:, 0], set_indices[:, 1]
         with variable_scope('extract_vertex_features'):
-            if self._fusable(point_MLP_normalization_type):
+            aggregation = self._fusable(point_MLP_normalization_type)
+            if aggregation is not None:
                 act = _check_types(point_MLP_normalization_type, point_MLP_activation_type)
                 names, ws, bs = _take_mlp(len(point_MLP_depth_list))
                 dims = [point_features.shape[1] + 3] + [int(k) for k in point_MLP_depth_list]
@@ -291,7 +300,7 @@ class PointSetPooling(object):
                 set_features = layer.edge_mlp_max(
                     point_features.contiguous(), point_coordinates.contiguous(), point_coordinates.contiguous(),
                     _i32(keypoint_indices.reshape(-1)), _i32(src), _i32(dst), num_keypoints,
-                    trusted=_ctx.trusted_edges)
+                    trusted=_ctx.trusted_edges, aggregation=aggregation)
             else:
                 # op-by-op composition, gnn.py:256-277
                 psf = _lib.gather_rows(point_features.contiguous(), _i32(src))
@@ -321,9 +330,10 @@ class GraphNetAutoCenter(object):
         self._auto_offset_fn = auto_offset_fn
 
     def _fusable(self, normalization_type):
-        return (self._edge_feature_fn is multi_layer_neural_network_fn
-                and self._aggregation_fn is graph_scatter_max_fn
-                and normalization_type == 'NONE')
+        """-> the fused kernels' aggregation name, or None for the op-by-op route."""
+        if self._edge_feature_fn is multi_layer_neural_network_fn and normalization_type == 'NONE':
+            return _FUSED_AGGREGATIONS.get(self._aggregation_fn)
+        return None
 
     def apply_regular(self, input_vertex_features, input_vertex_coordinates, NOT_USED, edges,
                       edge_MLP_depth_list=None, edge_MLP_normalization_type='fused_BN_center',
@@ -350,7 +360,8 @@ class GraphNetAutoCenter(object):
                     activation_type=auto_offset_MLP_feature_activation_type)
                 dest_coordinates = (source_coordinates + offset).contiguous()
         with variable_scope('extract_vertex_features'):
-            if self._fusable(edge_MLP_normalization_type):
+            aggregation = self._fusable(edge_MLP_normalization_type)
+            if aggregation is not None:
                 act = _check_types(edge_MLP_normalization_type, edge_MLP_activation_type)
                 names, ws, bs = _take_mlp(len(edge_MLP_depth_list))
                 dims = [input_vertex_features.shape[1] + 3] + [int(k) for k in edge_MLP_depth_list]
@@ -358,7 +369,7 @@ class GraphNetAutoCenter(object):
                 layer = _prepared(_lib.PG_LAYER_EDGE_GNN, names, ws, bs, dims, act)
                 aggregated_edge_features = layer.edge_mlp_max(
                     input_vertex_features.contiguous(), source_coordinates, dest_coordinates, None, _i32(src),
-                    _i32(dst), num_vertices, trusted=_ctx.trusted_edges)
+                    _i32(dst), num_vertices, trusted=_ctx.trusted_edges, aggregation=aggregation)
             else:
                 # op-by-op composition, gnn.py:338-365
                 s_feat = _lib.gather_rows(input_vertex_features.contiguous(), _i32(src))
