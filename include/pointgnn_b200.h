@@ -342,6 +342,9 @@ PG_API int pg_gather_rows(const float* params, int64_t num_rows, int32_t num_cha
 #define PG_ACT_SHIFT 16
 #define PG_ACT_MASK 0xff0000
 #define PG_PRECISION_ACTIVATION(code) (PG_FLAG_ACTIVATION | ((code) << PG_ACT_SHIFT))
+/* pg_layer_create(PG_LAYER_PREDICTOR, ...) only: the class-aware SEPARATED predictor (gnn.py:165-209), whose loc
+ * head of class c sees only the c-th of C equal column slices of the features (see pg_layer_create). */
+#define PG_FLAG_SEPARATED 0x1000
 
 /*
  * One slim.fully_connected layer (gnn.py:63-80,93-103), normalizer NONE:
@@ -439,10 +442,14 @@ PG_API int pg_check_edges(const int32_t* src, const int32_t* dst, int64_t num_ed
  *                            reference creates them: cls fc (D->H), cls fc_1 (H->C), then
  *                            for every class c: loc fc (D->H), fc_1 (H->H), fc_2 (H->box_len);
  *                            num_layers = 2 + 3 C.
+ *                            With PG_FLAG_SEPARATED: ClassAwareSeparatedPredictor (gnn.py:165-209), the same
+ *                            layers, but the loc fc of class c is [D/C, H] and reads features columns
+ *                            [c D/C, (c+1) D/C) (tf.split).  D % C != 0 gives PG_ERR_INVALID_ARGUMENT.
  *   precision 0 = fp32 FFMA, 1 = wgmma BF16x3, 2 = wgmma FP16 (as pg_fully_connected) wherever the shapes
  *             allow; may be OR-ed with
  *             PG_PRECISION_ACTIVATION(code): the activation of every layer that has one (default ReLU).
  *             It is fixed here because it selects the kernels the handle launches.
+ *             PG_FLAG_SEPARATED (PG_LAYER_PREDICTOR only, see above).
  * ------------------------------------------------------------------------ */
 typedef struct pg_layer pg_layer;
 #define PG_LAYER_MLP 0
@@ -485,15 +492,23 @@ PG_API int pg_softmax_rows(const float* logits, int64_t num_rows, int32_t num_cl
  *   class_table_host  (host) [C][4] floats per class label: median l, h, w (box_encoding.py:211-229) and the
  *                     yaw offset (0 for the "horizontal" label, pi/2 for the "vertical" one); l <= 0 marks
  *                     labels that are not decoded (Background, DontCare).
- *   out_boxes [K, C, 7] = (x, y, z, l, h, w, yaw), float32 arithmetic as the reference's NumPy code.
+ *   flags             0, or PG_BOX_CANONICAL: classaware_all_class_box_canonical_decoding (box_encoding.py:345-395),
+ *                     x and z rotated by yaw' = e6 pi / 4: x = e0 l cos yaw' + e2 w sin yaw',
+ *                     z = -e0 l sin yaw' + e2 w cos yaw' (l and w swapped for the "vertical" label).  Any other
+ *                     bit gives PG_ERR_INVALID_ARGUMENT.
+ *   out_boxes [K, C, 7] = (x, y, z, l, h, w, yaw), float32 arithmetic as the reference's NumPy code (its float32
+ *                     cos / sin restated: x, y, z and yaw are bit-exact; exp is CUDA's expf, so the sizes are within 4 ulp).
  */
+#define PG_BOX_CANONICAL 8
 PG_API int pg_decode_boxes(const float* box_encodings, const float* xyz, int64_t num_vertices,
-                    int32_t num_classes, const float* class_table_host, float* out_boxes, void* stream);
+                    int32_t num_classes, const float* class_table_host, float* out_boxes, int32_t flags,
+                    void* stream);
 
 /*
  * Candidate selection + decoding + NMS for a batch of frames (run.py:265-325):
  *   candidates      class c of vertex v iff 0 < c < C-1 and probs[v,c] > 1/C (run.py:281-284), labels 2/4/6
- *                   folded onto 1/3/5 (run.py:291-293), decoded with pg_decode_boxes' rule;
+ *                   folded onto 1/3/5 (run.py:291-293), decoded with pg_decode_boxes' rule (the canonical codec
+ *                   when flags carries PG_BOX_CANONICAL);
  *   NMS             nms.nms_boxes_3d_uncertainty (models/nms.py:133-170, 256-270) with
  *                   overlapped_boxes_3d_fast_poly (nms.py:64-88) and top_k = -1: score-sorted greedy
  *                   suppression inside a class; flags bit 0 (PG_NMS_MERGE): the kept box becomes the

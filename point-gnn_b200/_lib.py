@@ -527,8 +527,9 @@ def softmax_rows(logits):
 class PreparedLayer(object):
     """Owner of one ``pg_layer`` handle.  Keeps the weight tensors alive: the C side stores their pointers."""
 
-    def __init__(self, kind, weights, biases, dims, precision=0, activation=PG_ACT_RELU):
-        """activation: the PG_ACT_* code of every layer that has one (the is_logits last layers stay linear)."""
+    def __init__(self, kind, weights, biases, dims, precision=0, activation=PG_ACT_RELU, separated=False):
+        """activation: the PG_ACT_* code of every layer that has one (the is_logits last layers stay linear).
+        separated: a PG_LAYER_PREDICTOR whose loc heads read one of C equal feature slices each (PG_FLAG_SEPARATED)."""
         self.kind = int(kind)
         self.activation = int(activation)
         self.dims = [int(d) for d in dims]
@@ -537,7 +538,8 @@ class PreparedLayer(object):
         self._handle = None
         _call('pg_layer_create', kind=self.kind, weights_host=self._keep[0], biases_host=self._keep[1],
               dims_host=(c_i32 * len(self.dims))(*self.dims), num_layers=len(self._keep[0]),
-              precision=int(precision) | _activation_flags(activation), out_layer=ctypes.byref(handle))
+              precision=int(precision) | _activation_flags(activation) | (PG_FLAG_SEPARATED if separated else 0),
+              out_layer=ctypes.byref(handle))
         self._handle = handle
 
     def __del__(self):
@@ -591,25 +593,27 @@ def _class_table(table):
     return (ctypes.c_float * len(flat))(*flat)
 
 
-def decode_boxes(box_encodings, xyz, class_table):
-    """[K, C, 7] encodings at the K vertices -> [K, C, 7] boxes (box_encoding.py:265-299)."""
+def decode_boxes(box_encodings, xyz, class_table, flags=0):
+    """[K, C, 7] encodings at the K vertices -> [K, C, 7] boxes (box_encoding.py:265-299; with
+    flags=PG_BOX_CANONICAL the canonical codec, box_encoding.py:345-395)."""
     k, c, _ = box_encodings.shape
     out = torch.empty_like(box_encodings)
     _call('pg_decode_boxes', box_encodings=box_encodings, xyz=xyz, num_vertices=k, num_classes=c,
-          class_table_host=_class_table(class_table), out_boxes=out)
+          class_table_host=_class_table(class_table), out_boxes=out, flags=int(flags))
     return out
 
 
 def postprocess(probs, box_encodings, xyz, frame_ptr, class_table, overlapped_thres, merge=True, rescore=True,
-                want_candidates=False):
-    """run.py:265-325 for a batch of frames on the device.
+                want_candidates=False, canonical=False):
+    """run.py:265-325 for a batch of frames on the device; canonical: decode with the canonical box codec.
     -> dict(label [D] int32, box [D,7], score [D], index [D] int32, frame_ptr [F+1] int32
             [, cand_index [B] int32, cand_frame_ptr [F+1] int32])."""
     k, c = probs.shape
     num_frames = frame_ptr.numel() - 1
     dev = probs.device
     cap = max(1024, k)
-    flags = (PG_NMS_MERGE if merge else 0) | (PG_NMS_RESCORE if rescore else 0)
+    flags = ((PG_NMS_MERGE if merge else 0) | (PG_NMS_RESCORE if rescore else 0)
+             | (PG_BOX_CANONICAL if canonical else 0))
     sizes = (c_i64 * 2)()
     cand_index = torch.empty(k * max(c - 2, 1), dtype=torch.int32, device=dev) if want_candidates else None
     cand_fp = torch.empty(num_frames + 1, dtype=torch.int32, device=dev) if want_candidates else None

@@ -13,7 +13,7 @@
 //   float32  the box (x, y, z, l, h, w, yaw) and the score as NMS returns them; l / 2, w / 2, -h; and np.cos / np.sin
 //            of the float32 yaw.  NumPy's float32 cos / sin are not the correctly rounded values: they are its SIMD
 //            routine (Cody-Waite reduction by pi/2 in three FMA steps, then a degree-8 cosine or degree-9 sine
-//            polynomial evaluated with FMA), which np_trig below restates operation for operation.
+//            polynomial evaluated with FMA), which np_trig (pg_geom.cuh) restates operation for operation.
 //   float64  everything else.  np.array([[l / 2, 0.0, w / 2], ...]) holds a Python float, so the corner matrix and
 //            the rotation matrix are float64 (the float32 values widened).  Every matrix product (corners . R^T,
 //            [corners | 1] . cam_to_image^T, wx . p, candidates . normals^T) goes through BLAS dgemm / ddot, whose
@@ -26,6 +26,7 @@
 //   When rescoring finds no candidate inside, occlusion is the Python int 0 and the score stays the float32 value;
 //   the caller restores that type from the inside count of the row.
 #include "pg_common.cuh"
+#include "pg_geom.cuh"
 
 namespace pg {
 namespace {
@@ -34,34 +35,6 @@ constexpr int kBoxLen = 7;
 constexpr int kWarpsPerBlock = 8;
 constexpr double kImageWidth = 1242.0, kImageHeight = 375.0;   // run.py:385-388 hard-codes these, not the image size
 constexpr double kMaxTruncation = 0.4;                           // run.py:392
-
-// NumPy's float32 sin (want_cos = 0) or cos (want_cos = 1) for |x| below its Cody-Waite range; outside it NumPy
-// calls the C library's float routine, which the correctly rounded double result stands in for.
-__device__ float np_trig(float x, int want_cos) {
-  if (!(fabsf(x) <= (want_cos ? 71476.0625f : 117435.992f))) {
-    if (isnan(x) || isinf(x)) return __int_as_float(0x7fc00000);
-    return float(want_cos ? cos(double(x)) : sin(double(x)));
-  }
-  const float magic = 0x1.800000p+23f;
-  float q = __fmul_rn(x, 0x1.45f306p-1f);                      // x * 2 / pi, rounded to an integer:
-  q = __fsub_rn(__fadd_rn(q, magic), magic);
-  float r = __fmaf_rn(q, -0x1.921fb0p+00f, x);                 // x - q * pi / 2 in three parts
-  r = __fmaf_rn(q, -0x1.5110b4p-22f, r);
-  r = __fmaf_rn(q, -0x1.846988p-48f, r);
-  const float r2 = __fmul_rn(r, r);
-  float c = __fmaf_rn(0x1.98e616p-16f, r2, -0x1.6c06dcp-10f);
-  c = __fmaf_rn(c, r2, 0x1.55553cp-05f);
-  c = __fmaf_rn(c, r2, -0x1.000000p-01f);
-  c = __fmaf_rn(c, r2, 0x1.000000p+00f);
-  float s = __fmaf_rn(0x1.7d3bbcp-19f, r2, -0x1.a06bbap-13f);
-  s = __fmaf_rn(s, r2, 0x1.11119ap-07f);
-  s = __fmaf_rn(s, r2, -0x1.555556p-03f);
-  s = __fmaf_rn(s, r2, 0.0f);
-  s = __fmaf_rn(s, r, r);
-  const int quadrant = int(q) + want_cos;
-  const float v = (quadrant & 1) ? c : s;
-  return (quadrant & 2) ? __fsub_rn(0.0f, v) : v;
-}
 
 // BLAS's row . column: fma chain over k from the rounded first product
 __device__ __forceinline__ double dot3(double a0, double a1, double a2, double b0, double b1, double b2) {

@@ -4,6 +4,7 @@
 //   run.py:265-296            candidate selection: class c of vertex v iff 0 < c < C-1 and prob > 1/C,
 //                             "vertical" labels folded onto their class (2->1, 4->3, 6->5)
 //   box_encoding.py:265-299   classaware_all_class_box_decoding (float32 arithmetic, as NumPy does there)
+//   box_encoding.py:345-395   classaware_all_class_box_canonical_decoding (PG_BOX_CANONICAL, likewise)
 //   nms.py:9-27               boxes_3d_to_corners
 //   nms.py:64-88              overlapped_boxes_3d_fast_poly: 3-D IoU, footprints intersected as convex
 //                             polygons (the reference uses shapely; Sutherland-Hodgman in fp64 here)
@@ -34,6 +35,7 @@ constexpr int kBoxLen = 7;
 struct ClassTable {
   float l[kMaxClasses], h[kMaxClasses], w[kMaxClasses], yaw0[kMaxClasses];
   int decoded[kMaxClasses];
+  int canonical;           // PG_BOX_CANONICAL: the box codec is classaware_all_class_box_canonical_encoding
 };
 
 __device__ __forceinline__ int fold_label(int c) { return (c == 2 || c == 4 || c == 6) ? c - 1 : c; }
@@ -48,17 +50,30 @@ __global__ void flag_candidates_kernel(const float* __restrict__ probs, int64_t 
   flags[i] = (c > 0 && c < num_classes - 1 && double(probs[i]) > 1.0 / double(num_classes)) ? 1 : 0;
 }
 
-// classaware_all_class_box_decoding of (vertex, class c): the encoding e [7] at the vertex position p [3] -> b [7]
-// (box_encoding.py:276-298, float32 arithmetic in NumPy's order)
+// The decoding of (vertex, class c): the encoding e [7] at the vertex position p [3] -> b [7], float32 arithmetic in
+// NumPy's order.  classaware_all_class_box_decoding (box_encoding.py:276-298) scales x, y, z by l, h, w;
+// classaware_all_class_box_canonical_decoding (box_encoding.py:353-394) rotates (e0 l, e2 w) by yaw' = e6 pi / 4,
+// with l and w swapped for the "vertical" label, whose yaw is yaw' + pi / 2.  cos / sin are NumPy's float32 routine
+// (np_trig); exp is expf in both rules (within 2 ulp of exp, so a size is within 4 ulp of NumPy's).
 __device__ __forceinline__ void decode_box(const float* __restrict__ e, const float* __restrict__ p, const ClassTable& tab,
                                            int c, float* b) {
 #pragma unroll
   for (int j = 0; j < kBoxLen; ++j) b[j] = e[j];
   if (tab.decoded[c]) {
     const float pi4 = float(M_PI * 0.25), pi2 = float(0.5 * M_PI);
-    b[0] = __fmul_rn(e[0], tab.l[c]);
+    if (tab.canonical) {
+      const float yaw = __fmul_rn(e[6], pi4);
+      const float cs = np_trig(yaw, 1), sn = np_trig(yaw, 0);
+      const bool vertical = tab.yaw0[c] != 0.0f;
+      const float ex = __fmul_rn(e[0], vertical ? tab.w[c] : tab.l[c]);
+      const float ez = __fmul_rn(e[2], vertical ? tab.l[c] : tab.w[c]);
+      b[0] = __fadd_rn(__fmul_rn(ex, cs), __fmul_rn(ez, sn));
+      b[2] = __fadd_rn(__fmul_rn(-ex, sn), __fmul_rn(ez, cs));
+    } else {
+      b[0] = __fmul_rn(e[0], tab.l[c]);
+      b[2] = __fmul_rn(e[2], tab.w[c]);
+    }
     b[1] = __fmul_rn(e[1], tab.h[c]);
-    b[2] = __fmul_rn(e[2], tab.w[c]);
     b[3] = __fmul_rn(expf(e[3]), tab.l[c]);
     b[4] = __fmul_rn(expf(e[4]), tab.h[c]);
     b[5] = __fmul_rn(expf(e[5]), tab.w[c]);
@@ -513,7 +528,8 @@ static int nms_stage(Candidates& c, const Detections& out, double overlapped_thr
   return PG_OK;
 }
 
-static void make_class_table(const float* class_table_host, int num_classes, ClassTable* tab) {
+static void make_class_table(const float* class_table_host, int num_classes, int32_t flags, ClassTable* tab) {
+  tab->canonical = (flags & PG_BOX_CANONICAL) ? 1 : 0;
   for (int c = 0; c < kMaxClasses; ++c) {
     tab->l[c] = tab->h[c] = tab->w[c] = 1.0f;
     tab->yaw0[c] = 0.0f;
@@ -532,14 +548,15 @@ static void make_class_table(const float* class_table_host, int num_classes, Cla
 }
 
 extern "C" int pg_decode_boxes(const float* box_encodings, const float* xyz, int64_t num_vertices, int32_t num_classes,
-                               const float* class_table_host, float* out_boxes, void* stream) {
+                               const float* class_table_host, float* out_boxes, int32_t flags, void* stream) {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
+  PG_REQUIRE((flags & ~PG_BOX_CANONICAL) == 0, "pg_decode_boxes: unknown flags 0x%x", unsigned(flags));
   if (num_vertices == 0) return PG_OK;
   PG_REQUIRE(box_encodings && xyz && class_table_host && out_boxes, "pg_decode_boxes: null argument");
   PG_REQUIRE(num_classes >= 1 && num_classes <= kMaxClasses, "pg_decode_boxes: num_classes %d not in [1, %d]", num_classes,
              kMaxClasses);
   ClassTable tab;
-  make_class_table(class_table_host, num_classes, &tab);
+  make_class_table(class_table_host, num_classes, flags, &tab);
   decode_all_kernel<<<ceil_div(num_vertices * num_classes, 256), 256, 0, s>>>(box_encodings, xyz, num_vertices, num_classes, tab,
                                                                               out_boxes);
   PG_LAUNCH_CHECK();
@@ -563,7 +580,7 @@ extern "C" int pg_postprocess(const float* probs, const float* box_encodings, co
   PG_REQUIRE(num_vertices * num_classes < (int64_t(1) << 31), "pg_postprocess: too many (vertex, class) pairs");
   PG_REQUIRE(max_candidates_per_frame >= 32, "pg_postprocess: max_candidates_per_frame must be >= 32");
   ClassTable tab;
-  make_class_table(class_table_host, num_classes, &tab);
+  make_class_table(class_table_host, num_classes, flags, &tab);
   const int64_t cap = num_vertices * (num_classes - 2);      // at most C - 2 candidate classes per vertex
   const int64_t pairs = num_vertices * num_classes;
   Candidates cand;

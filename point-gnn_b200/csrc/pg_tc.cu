@@ -1487,11 +1487,16 @@ struct PreparedPredictor {
   size_t smem = 0;
   // per-layer route: every layer prepared on its own
   std::vector<PreparedFc> layers;
+  Temp wsep;                               // separated predictor, per-layer route: the C zero-padded [D, H] loc fc0
 };
 
-// dims = {D, H, C, box_len}; layers = cls fc0, cls fc1, then per class c: fc0, fc1, fc2
+// dims = {D, H, C, box_len}; layers = cls fc0, cls fc1, then per class c: fc0, fc1, fc2.
+// separated (ClassAwareSeparatedPredictor): loc fc0 of class c is [D/C, H] on feature columns [c D/C, (c+1) D/C).
+// It is packed as the [D, H] weight that is zero outside those rows, so both routes run the shared predictor's
+// kernels on the same GEMM shapes.
 int prepare_predictor(PreparedPredictor& P, const float* const* weights, const float* const* biases,
-                      const int32_t* dims, int num_layers, int act, bool want_tc, int arith, cudaStream_t s) {
+                      const int32_t* dims, int num_layers, int act, bool separated, bool want_tc, int arith,
+                      cudaStream_t s) {
   P.act = act;
   P.D = dims[0];
   P.H = dims[1];
@@ -1499,6 +1504,9 @@ int prepare_predictor(PreparedPredictor& P, const float* const* weights, const f
   P.box = dims[3];
   PG_REQUIRE(num_layers == 2 + 3 * P.C && P.C >= 1 && P.C <= 16 && P.H >= 1 && P.box >= 1,
              "pg_layer_create: predictor needs 2 + 3 C layers, 1 <= C <= 16");
+  PG_REQUIRE(!separated || P.D % P.C == 0,
+             "pg_layer_create: separated predictor: D = %d features do not split into C = %d equal slices", P.D, P.C);
+  const int slice = separated ? P.D / P.C : P.D;   // rows of a loc fc0
   P.htot = P.H * (P.C + 1);
   auto pad4 = [](int v) { return (v + 3) & ~3; };
   P.wfloats = pad4(P.H * P.C) + pad4(P.C) + P.C * (pad4(P.H * P.H) + pad4(P.H) + pad4(P.H * P.box) + pad4(P.box));
@@ -1511,10 +1519,14 @@ int prepare_predictor(PreparedPredictor& P, const float* const* weights, const f
     PG_CUDA_OK(P.wcat.alloc(sizeof(float) * size_t(P.D) * P.htot, s));
     PG_CUDA_OK(P.bcat.alloc(sizeof(float) * P.htot, s));
     PG_CUDA_OK(P.wpack.alloc(sizeof(float) * P.wfloats, s));
-    // concatenated first layers: column block h = 0 is the cls head, h = 1 + c the loc head of class c
+    // concatenated first layers: column block h = 0 is the cls head, h = 1 + c the loc head of class c (separated:
+    // rows [c slice, (c+1) slice) of it, the rest zero)
+    if (separated) PG_CUDA_OK(cudaMemsetAsync(P.wcat.ptr, 0, sizeof(float) * size_t(P.D) * P.htot, s));
     for (int h = 0; h <= P.C; ++h) {
       const int l = h == 0 ? 0 : 2 + 3 * (h - 1);
-      copy_block_kernel<<<32, 256, 0, s>>>(weights[l], P.D, P.H, P.htot, P.wcat.as<float>() + h * P.H);
+      const int rows = h == 0 ? P.D : slice, row0 = (h > 0 && separated) ? (h - 1) * slice : 0;
+      copy_block_kernel<<<32, 256, 0, s>>>(weights[l], rows, P.H, P.htot,
+                                           P.wcat.as<float>() + size_t(row0) * P.htot + h * P.H);
       PG_LAUNCH_CHECK();
       PG_CUDA_OK(cudaMemcpyAsync(P.bcat.as<float>() + h * P.H, biases[l], sizeof(float) * P.H, cudaMemcpyDeviceToDevice, s));
     }
@@ -1547,12 +1559,24 @@ int prepare_predictor(PreparedPredictor& P, const float* const* weights, const f
   }
   if (P.fused) return PG_OK;
   P.first.clear();
+  if (separated) {
+    const size_t dh = size_t(P.D) * P.H;
+    PG_CUDA_OK(P.wsep.alloc(sizeof(float) * dh * P.C, s));
+    PG_CUDA_OK(cudaMemsetAsync(P.wsep.ptr, 0, sizeof(float) * dh * P.C, s));
+    for (int c = 0; c < P.C; ++c) {
+      copy_block_kernel<<<32, 256, 0, s>>>(weights[2 + 3 * c], slice, P.H, P.H,
+                                           P.wsep.as<float>() + dh * c + size_t(c) * slice * P.H);
+      PG_LAUNCH_CHECK();
+    }
+  }
   P.layers.resize(num_layers);
   for (int l = 0; l < num_layers; ++l) {
     const int pos = l < 2 ? l : (l - 2) % 3;
     const int k = pos == 0 ? P.D : P.H;
     const int n = l == 1 ? P.C : (l >= 2 && pos == 2 ? P.box : P.H);
-    if (int rc = prepare_fc(P.layers[l], weights[l], n, biases[l], k, n, n, want_tc, arith, s)) return rc;
+    const float* w = (separated && l >= 2 && pos == 0) ? P.wsep.as<float>() + size_t(P.D) * P.H * ((l - 2) / 3)
+                                                       : weights[l];
+    if (int rc = prepare_fc(P.layers[l], w, n, biases[l], k, n, n, want_tc, arith, s)) return rc;
   }
   return PG_OK;
 }
@@ -1630,10 +1654,12 @@ extern "C" int pg_layer_create(int32_t kind, const float* const* weights_host, c
   PG_REQUIRE(weights_host && biases_host && dims_host && num_layers >= 1 && num_layers <= 64, "pg_layer_create: bad layer tables");
   const int act = activation_of(precision);
   PG_REQUIRE(act >= 0, "pg_layer_create: unknown activation");
-  precision &= ~(PG_FLAG_ACTIVATION | PG_ACT_MASK);
+  const bool separated = (precision & PG_FLAG_SEPARATED) != 0;
+  precision &= ~(PG_FLAG_ACTIVATION | PG_ACT_MASK | PG_FLAG_SEPARATED);
   PG_REQUIRE(precision >= 0 && precision <= 2, "pg_layer_create: unknown precision %d", precision);
   PG_REQUIRE(kind == PG_LAYER_MLP || kind == PG_LAYER_EDGE_POOL || kind == PG_LAYER_EDGE_GNN || kind == PG_LAYER_PREDICTOR,
              "pg_layer_create: unknown kind %d", kind);
+  PG_REQUIRE(!separated || kind == PG_LAYER_PREDICTOR, "pg_layer_create: PG_FLAG_SEPARATED is a predictor flag");
   for (int l = 0; l < num_layers; ++l) PG_REQUIRE(weights_host[l] && biases_host[l], "pg_layer_create: null weight/bias %d", l);
   auto L = std::make_unique<pg_layer>();
   L->kind = kind;
@@ -1655,7 +1681,8 @@ extern "C" int pg_layer_create(int32_t kind, const float* const* weights_host, c
       return rc;
   } else {
     L->dims.assign(dims_host, dims_host + 4);
-    if (int rc = prepare_predictor(L->pred, weights_host, biases_host, dims_host, num_layers, act, want_tc, arith, s))
+    if (int rc = prepare_predictor(L->pred, weights_host, biases_host, dims_host, num_layers, act, separated, want_tc,
+                                   arith, s))
       return rc;
   }
   *out_layer = L.release();

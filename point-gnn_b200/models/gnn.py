@@ -31,7 +31,7 @@ class VariableStore(object):
 
     def __init__(self, variables=None, device=None):
         self.vars = {}
-        self.prepared = {}      # (kind, first variable, depth, precision, activation) -> _lib.PreparedLayer
+        self.prepared = {}      # (kind, first variable, depth, precision, activation, separated) -> _lib.PreparedLayer
         if variables:
             self.load(variables, device)
 
@@ -108,14 +108,15 @@ def _take_mlp(num_layers):
     return names, ws, bs
 
 
-def _prepared(kind, names, weights, biases, dims, activation):
+def _prepared(kind, names, weights, biases, dims, activation, separated=False):
     """The prepared (weights packed once) layer for these variables and this activation, cached on the bound
-    VariableStore - the stand-in for TF creating / restoring its variables once and only computing at sess.run."""
+    VariableStore - the stand-in for TF creating / restoring its variables once and only computing at sess.run.
+    separated: the predictor is ClassAwareSeparatedPredictor (a different pack of the same variable names)."""
     store = _ctx.store
-    key = (kind, names[0], len(names), get_precision(), activation)
+    key = (kind, names[0], len(names), get_precision(), activation, separated)
     layer = store.prepared.get(key)
     if layer is None:
-        layer = _lib.PreparedLayer(kind, weights, biases, dims, get_precision(), activation)
+        layer = _lib.PreparedLayer(kind, weights, biases, dims, get_precision(), activation, separated=separated)
         store.prepared[key] = layer
     return layer
 
@@ -205,6 +206,7 @@ def _i32(t):
 
 class ClassAwarePredictor(object):
     """gnn.py:121-163."""
+    _separated = False      # ClassAwareSeparatedPredictor: the loc head of class c sees the c-th feature slice
 
     def __init__(self, cls_fn, loc_fn):
         self._cls_fn = cls_fn
@@ -225,8 +227,18 @@ class ClassAwarePredictor(object):
         h = int(ck['Ks'][0])
         return h if (int(lk['Ks'][0]) == h and int(lk['Ks'][1]) == h) else None
 
+    def _loc_inputs(self, features, num_classes):
+        """The input of every class's loc head: the features themselves, or (separated) tf.split's C slices."""
+        if not self._separated:
+            return [features] * num_classes
+        return [s.contiguous() for s in features.split(features.shape[1] // num_classes, dim=1)]
+
     def apply_regular(self, features, num_classes, box_encoding_len,
                       normalization_type='fused_BN_center', activation_type='ReLU'):
+        if self._separated and features.shape[1] % num_classes:
+            # tf.split's error at graph build (gnn.py:196)
+            raise ValueError('classaware_separated_predictor: D = %d features do not split into C = %d equal '
+                             'slices' % (features.shape[1], num_classes))
         h = self._head_width()
         if h is not None and normalization_type == 'NONE':
             act = _check_types(normalization_type, activation_type)
@@ -244,10 +256,13 @@ class ClassAwarePredictor(object):
                             names, ws, bs = names + n, ws + w, bs + b
             d = ws[0].shape[0]
             assert tuple(ws[1].shape) == (h, num_classes) and tuple(ws[0].shape) == (d, h)
+            loc_rows = d // num_classes if self._separated else d
             for class_idx in range(num_classes):
                 w0, w1, w2 = ws[2 + 3 * class_idx:5 + 3 * class_idx]
-                assert tuple(w0.shape) == (d, h) and tuple(w1.shape) == (h, h) and tuple(w2.shape) == (h, box_encoding_len)
-            layer = _prepared(_lib.PG_LAYER_PREDICTOR, names, ws, bs, [d, h, num_classes, box_encoding_len], act)
+                assert (tuple(w0.shape) == (loc_rows, h) and tuple(w1.shape) == (h, h)
+                        and tuple(w2.shape) == (h, box_encoding_len)), 'inconsistent layer shapes in the checkpoint'
+            layer = _prepared(_lib.PG_LAYER_PREDICTOR, names, ws, bs, [d, h, num_classes, box_encoding_len], act,
+                              separated=self._separated)
             logits, box_encodings, probs = layer.predictor(features.contiguous())
             logits._pg_probs = (probs, logits._version)      # models.postprocess returns these (softmax fused)
             return logits, box_encodings
@@ -258,14 +273,22 @@ class ClassAwarePredictor(object):
                                       normalization_type=normalization_type,
                                       activation_type=activation_type)
             with variable_scope('loc'):
-                for class_idx in range(num_classes):
+                for class_idx, loc_features in enumerate(self._loc_inputs(features, num_classes)):
                     with variable_scope('cls_%d' % class_idx):
-                        box_encodings = self._loc_fn(features, num_classes=box_encoding_len, is_logits=True,
+                        box_encodings = self._loc_fn(loc_features, num_classes=box_encoding_len, is_logits=True,
                                                      normalization_type=normalization_type,
                                                      activation_type=activation_type)
                         box_encodings_list.append(box_encodings.unsqueeze(1))
             box_encodings = torch.cat(box_encodings_list, dim=1)
         return logits, box_encodings
+
+
+class ClassAwareSeparatedPredictor(ClassAwarePredictor):
+    """gnn.py:165-209: ClassAwarePredictor whose loc head of class c sees only tf.split(features, C, axis=-1)[c].
+    The registry's heads run on the shared predictor's kernels, each loc head's first weight packed as the [D, H]
+    weight that is zero outside its slice's rows (PG_FLAG_SEPARATED); other cls_fn / loc_fn run op by op on the
+    slices."""
+    _separated = True
 
 
 class PointSetPooling(object):

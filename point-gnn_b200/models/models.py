@@ -47,6 +47,9 @@ class MultiLayerFastLocalGraphModelV2(object):
             'classaware_predictor_128': gnn.ClassAwarePredictor(
                 cls_fn=partial(gnn.multi_layer_fc_fn, Ks=(128,), num_layer=2),
                 loc_fn=partial(gnn.multi_layer_fc_fn, Ks=(128, 128), num_layer=3)),
+            'classaware_separated_predictor': gnn.ClassAwareSeparatedPredictor(
+                cls_fn=partial(gnn.multi_layer_fc_fn, Ks=(64,), num_layer=2),
+                loc_fn=partial(gnn.multi_layer_fc_fn, Ks=(64, 64,), num_layer=3)),
         }
         assert mode in ['train', 'eval', 'test'], 'Unsupported mode'
         self._mode = mode
@@ -131,9 +134,6 @@ class MultiLayerFastLocalGraphModelV2(object):
             predictor_config = self._layer_configs[-1]
             assert predictor_config['type'] in ('classaware_predictor', 'classaware_predictor_128',
                                                 'classaware_separated_predictor')
-            if predictor_config['type'] not in self._default_layers_type:
-                raise NotImplementedError('layer type %r (models.py:65-71) is used by no shipped config and is not '
-                                          'built' % predictor_config['type'])
             predictor = self._default_layers_type[predictor_config['type']]
             with gnn.variable_scope(predictor_config['scope']):
                 logits, box_encodings = predictor.apply_regular(

@@ -20,18 +20,31 @@ CLASS_NAMES = {  # run.py:371-383
 }
 
 
+def decoding_flags(box_encoding_method):
+    """The PG_BOX_* flag of a config's box_encoding_method.  Only the four-argument decoders run.py calls are
+    built; any other name raises ValueError (the reference's run.py raises TypeError at its first decode)."""
+    if box_encoding_method not in box_encoding.DECODING_FLAGS:
+        raise ValueError('box_encoding_method %r: run.py decodes with (labels, xyz, boxes, label_map), which only %s '
+                         'take' % (box_encoding_method, ' and '.join(sorted(box_encoding.DECODING_FLAGS))))
+    return box_encoding.DECODING_FLAGS[box_encoding_method]
+
+
 def detect(probs, box_encodings, last_layer_points_xyz, frame_ptr, label_method, nms_overlapped_thres,
-           use_box_merge=True, use_box_score=True, want_candidates=False):
+           use_box_merge=True, use_box_score=True, want_candidates=False,
+           box_encoding_method='classaware_all_class_box_encoding'):
     """probs [K, C], box_encodings [K, C, 7], last_layer_points_xyz [K, 3] (CUDA tensors, frames concatenated,
     frame_ptr [F+1] int32) -> dict of CUDA tensors: label, box [D,7], score, index (flat v*C + c), frame_ptr [F+1]
-    (+ cand_index / cand_frame_ptr = run.py's box_indices when want_candidates)."""
+    (+ cand_index / cand_frame_ptr = run.py's box_indices when want_candidates).  box_encoding_method: the config's
+    codec, which selects the decoding rule."""
+    canonical = decoding_flags(box_encoding_method) == _lib.PG_BOX_CANONICAL
     num_classes = probs.shape[1]
     table = box_encoding.class_table(LABEL_MAPS[label_method], num_classes)
     if frame_ptr is None:
         frame_ptr = torch.tensor([0, probs.shape[0]], dtype=torch.int32, device=probs.device)
     return _lib.postprocess(probs.contiguous(), box_encodings.contiguous(), last_layer_points_xyz.contiguous(),
                             frame_ptr.to(torch.int32).contiguous(), table, nms_overlapped_thres,
-                            merge=use_box_merge, rescore=use_box_score, want_candidates=want_candidates)
+                            merge=use_box_merge, rescore=use_box_score, want_candidates=want_candidates,
+                            canonical=canonical)
 
 
 def kitti_rows(det, last_layer_points_xyz, cam_to_image, num_classes, use_box_score=True):

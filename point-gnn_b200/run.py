@@ -209,6 +209,8 @@ def main(argv=None):
     CONFIG_PATH = os.path.join(CHECKPOINT_PATH, 'config')
     assert os.path.isfile(CONFIG_PATH), 'No config file found in %s' % CONFIG_PATH
     config = load_config(CONFIG_PATH)
+    # the decoding rule of the model's box codec; a codec run.py cannot decode fails here, before any frame is read
+    postprocess.decoding_flags(config['box_encoding_method'])
     # setup dataset ===========================================================
     if IS_TEST:
         dataset = KittiDataset(
@@ -310,7 +312,8 @@ def main(argv=None):
             det = postprocess.detect(probs, pred_box, last_layer_points_xyz,
                                      ticket.frame_ptrs[last_layer_graph_level + 1], config['label_method'],
                                      config['nms_overlapped_thres'], use_box_merge=USE_BOX_MERGE,
-                                     use_box_score=USE_BOX_SCORE, want_candidates=USE_BOX_SCORE)
+                                     use_box_score=USE_BOX_SCORE, want_candidates=USE_BOX_SCORE,
+                                     box_encoding_method=config['box_encoding_method'])
             t3 = time.time()
             charge('decode box', t3 - t2)
             # convert to KITTI ===============================================

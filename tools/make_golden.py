@@ -119,6 +119,40 @@ def post_goldens():
         print('post', name, 'candidates', len(out['cand_index']), 'kept', len(out['uncertainty_label']))
 
 
+BOX_CANONICAL_ROWS = 600
+
+
+def box_canonical_inputs(label_method, seed, rows=BOX_CANONICAL_ROWS):
+    """Seeded inputs of the canonical box decoder for one label map: every label of the map (Background and DontCare
+    included) on rows [M, 1] int32, vertices [M, 3] float32 (a quarter of them hundreds of metres out) and
+    encodings [M, 2, 7] float32 with |e6| up to 4 (slot 1 is only offset by the vertex)."""
+    from oracle import postprocess as pp
+    num_labels = max(pp.LABEL_MAPS[label_method].values()) + 1
+    rng = np.random.default_rng(seed)
+    labels = (np.arange(rows) % num_labels).astype(np.int32)[:, None]
+    xyz = np.c_[rng.uniform(-40, 40, rows), rng.uniform(-3, 3, rows), rng.uniform(0, 70, rows)]
+    xyz[: rows // 4] *= rng.uniform(5, 20, (rows // 4, 1))
+    enc = rng.standard_normal((rows, 2, 7))
+    enc[:, :, 3:6] *= 0.5
+    enc[:, :, 6] = rng.uniform(-4, 4, (rows, 2))
+    return labels, xyz.astype(np.float32), enc.astype(np.float32)
+
+
+def box_canonical_goldens():
+    """tests/golden/box_canonical.npz: the reference's own classaware_all_class_box_canonical_decoding
+    (box_encoding.py:345-395) on box_canonical_inputs for the three label maps of run.py."""
+    from oracle import postprocess as pp
+    be, _ = pp.reference_modules()
+    out = {}
+    for seed, method in enumerate(sorted(pp.LABEL_MAPS)):
+        labels, xyz, enc = box_canonical_inputs(method, 100 + seed)
+        dec = be.classaware_all_class_box_canonical_decoding(labels, xyz, enc, pp.LABEL_MAPS[method])
+        assert dec.dtype == np.float32
+        out.update({'labels_' + method: labels, 'xyz_' + method: xyz, 'enc_' + method: enc, 'dec_' + method: dec})
+        print('box_canonical', method, 'rows', len(labels))
+    np.savez_compressed(os.path.join(GOLDEN, 'box_canonical.npz'), **out)
+
+
 def kitti_goldens():
     """tests/golden/kitti_io.npz + kitti_result_car.txt: the reference's own dataset/kitti_dataset.py (Open3D stubbed)
     on a synthetic KITTI-format frame - calibration matrices, camera points in image with colours - and run.py:361-429
@@ -569,6 +603,8 @@ if __name__ == '__main__':
         main()
     if which in ('all', 'post'):
         post_goldens()
+    if which in ('all', 'box_canonical'):
+        box_canonical_goldens()
     if which in ('all', 'kitti'):
         kitti_goldens()
     if which in ('all', 'kitti_voxel_avg'):
