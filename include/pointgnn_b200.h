@@ -311,6 +311,18 @@ PG_API int pg_scatter_sum(const float* features, const int32_t* centers, int64_t
                    int32_t num_channels, int64_t num_centers, float* out, void* stream);
 PG_API int pg_scatter_mean(const float* features, const int32_t* centers, int64_t num_edges,
                     int32_t num_channels, int64_t num_centers, float* out, void* stream);
+/*
+ * pg_scatter_sum / pg_scatter_mean with a flag word.  flags 0: the same as those.  PG_FLAG_DETERMINISTIC (below): the
+ * ids are first stable-sorted (position order kept within an id; num_edges < 2^31), then each destination is the fp32
+ * sum in one fixed order: the sorted edges in tiles of PG_ORDERED_SCATTER_TILE, a sequential sum (from 0) per
+ * destination and tile, then those partial sums added one after another in ascending tile order.  The same bits on
+ * every run.  Any other bit gives PG_ERR_INVALID_ARGUMENT.
+ */
+#define PG_ORDERED_SCATTER_TILE 64
+PG_API int pg_scatter_sum_flags(const float* features, const int32_t* centers, int64_t num_edges,
+                   int32_t num_channels, int64_t num_centers, float* out, int32_t flags, void* stream);
+PG_API int pg_scatter_mean_flags(const float* features, const int32_t* centers, int64_t num_edges,
+                    int32_t num_channels, int64_t num_centers, float* out, int32_t flags, void* stream);
 
 /* tf.gather(params, indices) for [R,C] fp32 rows (gnn.py:256-262,338-348). */
 PG_API int pg_gather_rows(const float* params, int64_t num_rows, int32_t num_channels,
@@ -396,6 +408,13 @@ PG_API int pg_fully_connected(const float* x, int64_t m, int32_t k, const float*
  *                  PG_AGG_MEAN  graph_scatter_mean_fn  unsorted_segment_mean: the sum over max(count, 1)
  *                The sum and the mean add fp32 partial sums with atomics, as TF's GPU kernel does: their
  *                last bits may differ from run to run.  Code 3 gives PG_ERR_INVALID_ARGUMENT.
+ *                PG_FLAG_DETERMINISTIC: the sum and the mean add their partial sums in a fixed order instead,
+ *                the same bits on every run for the same inputs (torch.use_deterministic_algorithms).  The
+ *                call first stable-sorts the edges by dst (an edge list in any order works; num_edges < 2^31),
+ *                then the order follows where the sorted list's 16-edge units fall (64 on the fp32 path), so a
+ *                different packing of the same edges may round differently.  Temporary memory: the sorted
+ *                src / dst, and one side buffer of 2 partial rows per unit, at most 2^18 edges at a time
+ *                (DESIGN 4.1.2).  The max ignores the flag: it is order-independent already.
  */
 #define PG_PRECISION_MASK 0xff
 #define PG_FLAG_TRUSTED_INDICES 0x100
@@ -405,6 +424,7 @@ PG_API int pg_fully_connected(const float* x, int64_t m, int32_t k, const float*
 #define PG_AGG_SHIFT 10
 #define PG_AGG_MASK 0xc00
 #define PG_AGGREGATION(code) ((code) << PG_AGG_SHIFT)
+#define PG_FLAG_DETERMINISTIC 0x2000
 #define PG_EDGE_POOL 0
 #define PG_EDGE_GNN 1
 PG_API int pg_edge_mlp_max(int32_t mode, const float* features, int32_t num_feature_channels,
@@ -467,8 +487,9 @@ PG_API int pg_layer_destroy(pg_layer* layer);
 PG_API int pg_layer_mlp(const pg_layer* layer, const float* x, int64_t m, int32_t last_linear,
                  const float* residual, float* out, void* stream);
 
-/* pg_edge_mlp_max on a prepared edge layer; flags: 0, PG_FLAG_TRUSTED_INDICES and / or
- * PG_AGGREGATION(code) (as pg_edge_mlp_max).  The aggregation is chosen per call: one handle serves all three. */
+/* pg_edge_mlp_max on a prepared edge layer; flags: 0, PG_FLAG_TRUSTED_INDICES, PG_AGGREGATION(code) and / or
+ * PG_FLAG_DETERMINISTIC (as pg_edge_mlp_max).  The aggregation is chosen per call: one handle serves all three;
+ * pg_layer_create rejects PG_FLAG_DETERMINISTIC. */
 PG_API int pg_layer_edge_mlp_max(const pg_layer* layer, const float* features, const float* xyz_src,
                           const float* xyz_dst, const int32_t* dst_index, const int32_t* src,
                           const int32_t* dst, int64_t num_edges, int64_t num_src, int64_t num_dst,
@@ -627,7 +648,9 @@ PG_API int pg_kitti_eval(const double* gt, const int32_t* gt_class, const double
 
 /* wgmma kernel launches so far (which: 0 = segment-max launches of the edge layers, 1 = store launches:
  * dense layers and the stored per-edge layers of point-set pooling);
- * lets callers and tests verify that the tensor-core path, not the FFMA path, actually ran. */
+ * lets callers and tests verify that the tensor-core path, not the FFMA path, actually ran.
+ * which = 2: the fix-up launches of the ordered segment sums (PG_FLAG_DETERMINISTIC) on any path, tensor-core,
+ * fp32 or pg_scatter_sum_flags / _mean_flags: one per ordered call or edge slice; never without the flag. */
 PG_API int64_t pg_tc_launch_count(int32_t which);
 
 /* Number of kernels this library has launched in the calling process (bench.py). */

@@ -236,6 +236,13 @@ def _aggregation_flags(aggregation):
     return AGGREGATIONS[aggregation] << PG_AGG_SHIFT
 
 
+def _deterministic_flags():
+    """PG_FLAG_DETERMINISTIC while ``torch.use_deterministic_algorithms(True)`` is in force (its warn-only form too,
+    as torch's own scatter_add_ stays deterministic there and warns about nothing): the segment sum and mean then add
+    their partial sums in a fixed order, the same bits on every run.  Read at each call; the max ignores the flag."""
+    return PG_FLAG_DETERMINISTIC if torch.are_deterministic_algorithms_enabled() else 0  # noqa: F821
+
+
 def launch_count():
     return _call('pg_launch_count')
 
@@ -245,7 +252,8 @@ def device_is_sm90():
 
 
 def tc_launch_count(which=0):
-    """tensor-core launches so far: which=0 segment-max (edge layer) launches, 1 dense-layer launches."""
+    """tensor-core launches so far: which=0 segment-max (edge layer) launches, 1 dense-layer launches; 2 the fix-up
+    launches of the ordered segment sums (PG_FLAG_DETERMINISTIC) on any path."""
     return _call('pg_tc_launch_count', which=int(which))
 
 
@@ -453,10 +461,11 @@ def scatter_max(features, centers, num_centers):
 
 
 def scatter_sum(features, centers, num_centers, mean=False):
+    """unsorted_segment_sum (mean); in a fixed order under torch.use_deterministic_algorithms(True)."""
     e, c = features.shape
     out = torch.empty((int(num_centers), c), dtype=torch.float32, device=features.device)
-    _call('pg_scatter_mean' if mean else 'pg_scatter_sum', features=features, centers=centers, num_edges=e,
-          num_channels=c, num_centers=int(num_centers), out=out)
+    _call('pg_scatter_mean_flags' if mean else 'pg_scatter_sum_flags', features=features, centers=centers,
+          num_edges=e, num_channels=c, num_centers=int(num_centers), out=out, flags=_deterministic_flags())
     return out
 
 
@@ -502,8 +511,9 @@ def edge_mlp_max(mode, features, xyz_src, xyz_dst, dst_index, src, dst, num_dst,
                  trusted=False, activation=PG_ACT_RELU, aggregation='max'):
     """trusted=True: the caller vouches for the index ranges (graph_gen output / check_edges passed); the call
     then does not read the range-error flag back and does not synchronise the stream.  activation: the PG_ACT_* code
-    applied after every layer.  aggregation: 'max', 'sum' or 'mean' over the edges of each destination."""
-    flags = _aggregation_flags(aggregation)
+    applied after every layer.  aggregation: 'max', 'sum' or 'mean' over the edges of each destination; the sum and
+    the mean in a fixed order under torch.use_deterministic_algorithms(True)."""
+    flags = _aggregation_flags(aggregation) | _deterministic_flags()
     num_layers = len(weights)
     dims = [weights[0].shape[0]] + [w.shape[1] for w in weights]
     out = torch.empty((int(num_dst), dims[-1]), dtype=torch.float32, device=features.device)
@@ -559,7 +569,7 @@ class PreparedLayer(object):
 
     # fused gather -> edge MLP -> segment max, sum or mean (gnn.py:256-277, 338-365)
     def edge_mlp_max(self, features, xyz_src, xyz_dst, dst_index, src, dst, num_dst, trusted=False, aggregation='max'):
-        flags = _aggregation_flags(aggregation) | (PG_FLAG_TRUSTED_INDICES if trusted else 0)
+        flags = _aggregation_flags(aggregation) | (PG_FLAG_TRUSTED_INDICES if trusted else 0) | _deterministic_flags()
         if features.shape[1] + 3 != self.dims[0]:
             raise ValueError('edge layer: %d feature channels + 3 != first weight rows %d'
                              % (features.shape[1], self.dims[0]))

@@ -166,12 +166,42 @@ int activate_rows(float* out, int64_t rows, int n, int ldo, const float* bias, i
 // out [num_dst, n] /= max(number of edges e with dst[e] = row, 1): the segment sum -> unsorted_segment_mean.  Edges
 // whose dst is out of range are not counted
 int divide_by_segment_count(float* out, int64_t num_dst, int n, const int32_t* dst, int64_t num_edges, cudaStream_t s);
+// The ordered segment sum (PG_FLAG_DETERMINISTIC) of the three sum paths (pg_tc.cu, pg_edge_simt.cu, pg_ops.cu), DESIGN
+// §4.1.2.  A kernel cuts its rows into units it reduces in a fixed order (a warp's 16 edges, a 64-edge tile).  The
+// rows of one destination are adjacent (the edge calls stable-sort their edges by dst first, pg_scatter_* their ids),
+// so a run of them that holds neither the first nor the last row of its unit
+// is the whole destination: it is stored into out.  The run that holds the unit's first row goes to slot 2 u of a side
+// buffer, the run that holds its last row to slot 2 u + 1, each with the destination's id (-1: no run there).
+// ordered_fixup then adds each destination's partial rows one after another in ascending slot order, and adds that
+// into out (still 0 unless an earlier slice of the same edge list left a partial sum there).
+// The launches that write a side buffer take at most kOrderedSlice edges each, which bounds the buffer: 2 rows of n
+// floats per unit, for the tensor-core path (16-edge units) 2^15 rows.
+constexpr int64_t kOrderedSlice = int64_t(1) << 18;
+struct OrderedParts {
+  Temp val, id;           // [slots, n] partial rows, [slots] destination ids
+  int64_t slots = 0;
+  int n = 0;
+  int alloc(int64_t units, int cols, cudaStream_t s);   // ids filled with -1
+  int reset(cudaStream_t s);                            // ids back to -1 for the next slice
+  float* v() const { return val.as<float>(); }
+  int32_t* i() const { return id.as<int32_t>(); }
+};
+int ordered_fixup(const OrderedParts& parts, float* out, int ldo, cudaStream_t s);
+// pg_ops.cu: the stable order of ids [n] (ids outside [0, num_ids) last, as num_ids): keys_sorted [n] uint64, order
+// [n] int32 (input positions); n < 2^31.  sort_edges_by_dst: src / dst in that order of dst, into src_s / dst_s
+int stable_order(const int32_t* ids, int64_t n, int64_t num_ids, Temp& keys_sorted, Temp& order, cudaStream_t s);
+int sort_edges_by_dst(const int32_t* src, const int32_t* dst, int64_t n, int64_t num_dst, Temp& src_s, Temp& dst_s,
+                      cudaStream_t s);
+// pg_tc.cu: count one fix-up launch (pg_tc_launch_count(2))
+void count_ordered_launch();
 // pg_edge_simt.cu: the fp32 FFMA edge MLP (activation act after every layer) + segment max (agg PG_AGG_MAX) or sum
-// (any other) into out (already filled with -FLT_MAX or 0); sets *err on an out-of-range src / dst
+// (any other) into out (already filled with -FLT_MAX or 0), the sum in a fixed order when ordered; sets *err on an
+// out-of-range src / dst
 int edge_mlp_max_fp32(int mode, const float* features, int c_in, const float* xyz_src, const float* xyz_dst,
                       const int32_t* dst_index, const int32_t* src, const int32_t* dst, int64_t num_edges,
                       int64_t num_src, int64_t num_dst, const float* const* weights, const float* const* biases,
-                      const int32_t* dims, int num_layers, int act, int agg, float* out, int* err, cudaStream_t s);
+                      const int32_t* dims, int num_layers, int act, int agg, bool ordered, float* out, int* err,
+                      cudaStream_t s);
 
 inline int num_sms() {
   static int sms = 0;

@@ -43,10 +43,13 @@ struct EdgeMlpParams {
   int stride0, stride1;  // row strides (floats) of the two activation buffers
   float* out;
   int* err;
+  float* part;           // kOrdered: the side buffer of the ordered sum (pg_common.cuh), unit = tile
+  int32_t* part_id;
 };
 
-// kSum: the segment sum (atomicAdd into an output filled with 0) instead of the max
-template <bool kSum>
+// kSum: the segment sum (atomicAdd into an output filled with 0) instead of the max.  kOrdered (with kSum): the tile's
+// first run to slot 0 of the side buffer, its last to slot 1, every other run stored: no atomics, a fixed order
+template <bool kSum, bool kOrdered = false>
 __global__ void __launch_bounds__(kThreads, 1) edge_mlp_max_fp32_kernel(EdgeMlpParams p) {
   extern __shared__ __align__(16) float smem[];
   float* buf0 = smem;
@@ -138,26 +141,37 @@ __global__ void __launch_bounds__(kThreads, 1) edge_mlp_max_fp32_kernel(EdgeMlpP
     const float* fin = (p.num_layers & 1) ? buf1 : buf0;
     const int fstride = (p.num_layers & 1) ? p.stride1 : p.stride0;
     const int n_out = p.dims[p.num_layers];
-    auto flush = [&](int d, int c, float m) {
-      if (kSum)
+    int runs = 0;   // kOrdered: runs of the tile flushed so far by this thread (column)
+    auto flush = [&](int d, int c, float m, bool last) {
+      if (kOrdered) {
+        const int slot = runs++ == 0 ? 0 : last ? 1 : -1;
+        if (slot < 0) {
+          p.out[int64_t(d) * n_out + c] = m;
+        } else {
+          p.part[(2 * tile + slot) * n_out + c] = m;
+          if (c == 0) p.part_id[2 * tile + slot] = d;
+        }
+      } else if (kSum) {
         atomicAdd(p.out + int64_t(d) * n_out + c, m);
-      else
+      } else {
         atomic_max_float(p.out + int64_t(d) * n_out + c, m);
+      }
     };
     for (int c = threadIdx.x; c < n_out; c += kThreads) {
       int cur = -1;
+      runs = 0;
       float m = kSum ? 0.0f : -FLT_MAX;
       for (int r = 0; r < rows; ++r) {
         const int d = s_dst[r];
         if (d != cur) {
-          if (cur >= 0) flush(cur, c, m);
+          if (cur >= 0) flush(cur, c, m, false);
           cur = d;
           m = kSum ? 0.0f : -FLT_MAX;
         }
         const float v = fin[size_t(r) * fstride + c];
         m = kSum ? m + v : fmaxf(m, v);
       }
-      if (cur >= 0) flush(cur, c, m);
+      if (cur >= 0) flush(cur, c, m, true);
     }
   }
 }
@@ -167,7 +181,8 @@ __global__ void __launch_bounds__(kThreads, 1) edge_mlp_max_fp32_kernel(EdgeMlpP
 int edge_mlp_max_fp32(int mode, const float* features, int c_in, const float* xyz_src, const float* xyz_dst,
                       const int32_t* dst_index, const int32_t* src, const int32_t* dst, int64_t num_edges,
                       int64_t num_src, int64_t num_dst, const float* const* weights, const float* const* biases,
-                      const int32_t* dims, int num_layers, int act, int agg, float* out, int* err, cudaStream_t s) {
+                      const int32_t* dims, int num_layers, int act, int agg, bool ordered, float* out, int* err,
+                      cudaStream_t s) {
   PG_REQUIRE(num_layers >= 1 && num_layers <= kMaxLayers, "edge MLP depth %d not in [1,%d]", num_layers, kMaxLayers);
   PG_REQUIRE(dims[0] == c_in + 3, "dims[0]=%d must equal feature channels + 3 = %d", dims[0], c_in + 3);
   EdgeMlpParams p{};
@@ -201,13 +216,30 @@ int edge_mlp_max_fp32(int mode, const float* features, int c_in, const float* xy
   p.err = err;
   const size_t smem = size_t(kTileE) * (p.stride0 + p.stride1) * sizeof(float);
   PG_REQUIRE(smem <= 227 * 1024 - 1024, "edge MLP widths need %zu B of shared memory (> 226 KB)", smem);
-  if (num_edges > 0) {
-    void (*kernel)(EdgeMlpParams) = agg == PG_AGG_MAX ? edge_mlp_max_fp32_kernel<false> : edge_mlp_max_fp32_kernel<true>;
+  if (num_edges == 0) return PG_OK;
+  auto launch = [&](void (*kernel)(EdgeMlpParams), const EdgeMlpParams& q) -> int {
     PG_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-    const int64_t tiles = ceil_div(num_edges, kTileE);
-    const int grid = int(std::min<int64_t>(tiles, num_sms()));
-    kernel<<<grid, kThreads, smem, s>>>(p);
+    const int grid = int(std::min<int64_t>(ceil_div(q.num_edges, kTileE), num_sms()));
+    kernel<<<grid, kThreads, smem, s>>>(q);
     PG_LAUNCH_CHECK();
+    return PG_OK;
+  };
+  if (agg == PG_AGG_MAX) return launch(edge_mlp_max_fp32_kernel<false>, p);
+  if (!ordered) return launch(edge_mlp_max_fp32_kernel<true>, p);
+  // the ordered sum, kOrderedSlice edges (a multiple of the tile) per launch and fix-up
+  OrderedParts parts;
+  if (int rc = parts.alloc(ceil_div(std::min(num_edges, kOrderedSlice), kTileE), p.dims[num_layers], s)) return rc;
+  for (int64_t e0 = 0; e0 < num_edges; e0 += kOrderedSlice) {
+    EdgeMlpParams q = p;
+    q.src = src + e0;
+    q.dst = dst + e0;
+    q.num_edges = std::min(kOrderedSlice, num_edges - e0);
+    q.part = parts.v();
+    q.part_id = parts.i();
+    if (e0 > 0)
+      if (int rc = parts.reset(s)) return rc;
+    if (int rc = launch(edge_mlp_max_fp32_kernel<true, true>, q)) return rc;
+    if (int rc = ordered_fixup(parts, out, p.dims[num_layers], s)) return rc;
   }
   return PG_OK;
 }

@@ -142,6 +142,84 @@ __global__ void scatter_sum_kernel(const float* __restrict__ feat, const int32_t
   }
 }
 
+// The same with PG_FLAG_DETERMINISTIC, over the edges stable-sorted by id (order [e] = the input position of sorted edge
+// e, sorted [e] its id; dropped ids sort last as num_centers): tile t of PG_ORDERED_SCATTER_TILE sorted edges is unit t
+// of the ordered sum (pg_common.cuh), summed sequentially from 0 per destination.  The counts of the mean are integers
+// added as floats: exact up to 2^24 edges per destination in any order, so they keep their atomics
+__global__ void scatter_sum_ordered_kernel(const float* __restrict__ feat, const int32_t* __restrict__ order,
+                                           const uint64_t* __restrict__ sorted, int64_t num_edges, int num_channels,
+                                           int64_t num_centers, float* __restrict__ out, float* __restrict__ count,
+                                           float* __restrict__ part, int32_t* __restrict__ part_id) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= num_channels) return;
+  const int64_t num_chunks = (num_edges + PG_ORDERED_SCATTER_TILE - 1) / PG_ORDERED_SCATTER_TILE;
+  for (int64_t chunk = blockIdx.y; chunk < num_chunks; chunk += gridDim.y) {
+    const int64_t e0 = chunk * PG_ORDERED_SCATTER_TILE, e1 = min(e0 + PG_ORDERED_SCATTER_TILE, num_edges);
+    int64_t cur = -1;
+    int runs = 0;
+    float acc = 0.0f, n = 0.0f;
+    auto flush = [&](bool last) {
+      if (cur < 0 || cur >= num_centers) return;
+      const int slot = runs == 0 ? 0 : last ? 1 : -1;
+      if (slot < 0) {
+        out[cur * num_channels + c] = acc;
+      } else {
+        part[(2 * chunk + slot) * num_channels + c] = acc;
+        if (c == 0) part_id[2 * chunk + slot] = int32_t(cur);
+      }
+      if (count != nullptr && c == 0) atomicAdd(count + cur, n);
+      ++runs;
+    };
+    for (int64_t e = e0; e < e1; ++e) {
+      const int64_t d = int64_t(__ldg(sorted + e));
+      if (d != cur) {
+        flush(false);
+        cur = d;
+        acc = 0.0f;
+        n = 0.0f;
+      }
+      acc += __ldg(feat + int64_t(__ldg(order + e)) * num_channels + c);
+      n += 1.0f;
+    }
+    flush(true);
+  }
+}
+
+// The fix-up of the ordered segment sum (pg_common.cuh): thread (slot, column).  A destination's chain can only go on
+// from one unit into the next through the next unit's slot 0 (its run holds that unit's first row), so an empty slot 0
+// ends every chain and the walks stay within one chain.  The first slot of a chain (no slot of the previous unit
+// continues into it) adds the chain's partial rows in ascending slot order and adds the total into out; the edges are
+// grouped by destination, so no other thread writes that row
+__global__ void ordered_fixup_kernel(const float* __restrict__ part, const int32_t* __restrict__ part_id, int64_t slots,
+                                     int n, float* __restrict__ out, int ldo) {
+  for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < slots * n; i += int64_t(gridDim.x) * blockDim.x) {
+    const int64_t slot = i / n;
+    const int c = int(i - slot * n);
+    const int32_t d = part_id[slot];
+    if (d < 0) continue;
+    if ((slot & 1) == 0 && slot > 0) {
+      // slot 0 of its unit: a chain goes on into it from the previous unit's last run (slot 1, or slot 0 when that
+      // unit had one run)
+      const int32_t prev = part_id[slot - 1] >= 0 ? part_id[slot - 1] : part_id[slot - 2];
+      if (prev == d) continue;
+    } else if (slot & 1) {
+      if (part_id[slot - 1] == d) continue;   // cannot happen (two runs of one unit), kept for safety
+    }
+    float t = part[slot * n + c];
+    for (int64_t j = slot + 1; j < slots; ++j) {
+      const int32_t dj = part_id[j];
+      if (dj < 0) {
+        if ((j & 1) == 0) break;   // an empty slot 0: the next unit does not continue the chain
+        continue;
+      }
+      if (dj != d) break;
+      t += part[j * n + c];
+    }
+    float* o = out + int64_t(d) * ldo + c;
+    *o = *o + t;
+  }
+}
+
 __global__ void divide_rows_kernel(float* __restrict__ out, const float* __restrict__ count, int64_t num_centers,
                                    int num_channels) {
   const int64_t total = num_centers * num_channels;
@@ -268,7 +346,30 @@ int fc_fp32_launch(const float* x, int64_t m, int k, const float* w, const float
   return PG_OK;
 }
 
-// the in-degree histogram of an edge list: one atomic per edge (the counts are integers, exact in fp32 up to 2^24)
+int OrderedParts::alloc(int64_t units, int cols, cudaStream_t s) {
+  slots = 2 * units;
+  n = cols;
+  PG_CUDA_OK(val.alloc(sizeof(float) * size_t(slots) * n, s));
+  PG_CUDA_OK(id.alloc(sizeof(int32_t) * size_t(slots), s));
+  return reset(s);
+}
+
+int OrderedParts::reset(cudaStream_t s) {
+  PG_CUDA_OK(cudaMemsetAsync(id.ptr, 0xff, sizeof(int32_t) * size_t(slots), s));
+  return PG_OK;
+}
+
+int ordered_fixup(const OrderedParts& parts, float* out, int ldo, cudaStream_t s) {
+  if (parts.slots == 0) return PG_OK;
+  const int blocks = int(std::min<int64_t>(ceil_div(parts.slots * parts.n, 256), int64_t(num_sms()) * 8));
+  ordered_fixup_kernel<<<blocks, 256, 0, s>>>(parts.v(), parts.i(), parts.slots, parts.n, out, ldo);
+  PG_LAUNCH_CHECK();
+  count_ordered_launch();
+  return PG_OK;
+}
+
+// the in-degree histogram of an edge list: one atomic per edge (the counts are integers, exact in fp32 up to 2^24 in
+// any order: the ordered segment sum's mean divides by them as they are)
 __global__ void count_segments_kernel(const int32_t* __restrict__ dst, int64_t num_edges, int64_t num_dst,
                                       float* __restrict__ count) {
   for (int64_t e = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; e < num_edges; e += int64_t(gridDim.x) * blockDim.x) {
@@ -296,6 +397,58 @@ int activate_rows(float* out, int64_t rows, int n, int ldo, const float* bias, i
   if (rows == 0) return PG_OK;
   const int grid = int(std::min<int64_t>(ceil_div(rows * n, 256), int64_t(num_sms()) * 8));
   activate_rows_kernel<<<grid, 256, 0, s>>>(out, rows, n, ldo, bias, act, residual, ldr, skip_empty);
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}
+
+namespace {
+
+// the keys of the stable order by id: ids outside [0, num_ids) become num_ids and sort after every kept one
+__global__ void order_keys_kernel(const int32_t* __restrict__ ids, int64_t n, int64_t num_ids, uint64_t* __restrict__ keys,
+                                  int32_t* __restrict__ pos) {
+  for (int64_t e = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; e < n; e += int64_t(gridDim.x) * blockDim.x) {
+    const int32_t d = ids[e];
+    keys[e] = d >= 0 && d < num_ids ? uint64_t(d) : uint64_t(num_ids);
+    pos[e] = int32_t(e);
+  }
+}
+
+__global__ void gather_i32_kernel(const int32_t* __restrict__ in, const int32_t* __restrict__ order, int64_t n,
+                                  int32_t* __restrict__ out) {
+  for (int64_t e = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; e < n; e += int64_t(gridDim.x) * blockDim.x)
+    out[e] = in[order[e]];
+}
+
+}  // namespace
+
+int stable_order(const int32_t* ids, int64_t n, int64_t num_ids, Temp& keys_sorted, Temp& order, cudaStream_t s) {
+  PG_REQUIRE(n < (int64_t(1) << 31), "ordered segment sum: %lld edges (int32 positions)", (long long)n);
+  Temp keys, pos;
+  PG_CUDA_OK(keys.alloc(sizeof(uint64_t) * n, s));
+  PG_CUDA_OK(keys_sorted.alloc(sizeof(uint64_t) * n, s));
+  PG_CUDA_OK(pos.alloc(sizeof(int32_t) * n, s));
+  PG_CUDA_OK(order.alloc(sizeof(int32_t) * n, s));
+  if (n == 0) return PG_OK;
+  order_keys_kernel<<<int(std::min<int64_t>(ceil_div(n, 256), int64_t(num_sms()) * 8)), 256, 0, s>>>(
+      ids, n, num_ids, keys.as<uint64_t>(), pos.as<int32_t>());
+  PG_LAUNCH_CHECK();
+  int end_bit = 1;
+  while (end_bit < 64 && (uint64_t(num_ids) >> end_bit) != 0) ++end_bit;
+  return sort_pairs(keys.as<uint64_t>(), keys_sorted.as<uint64_t>(), pos.as<int32_t>(), order.as<int32_t>(), n, end_bit,
+                    s);
+}
+
+int sort_edges_by_dst(const int32_t* src, const int32_t* dst, int64_t n, int64_t num_dst, Temp& src_s, Temp& dst_s,
+                      cudaStream_t s) {
+  Temp keys, order;
+  if (int rc = stable_order(dst, n, num_dst, keys, order, s)) return rc;
+  PG_CUDA_OK(src_s.alloc(sizeof(int32_t) * n, s));
+  PG_CUDA_OK(dst_s.alloc(sizeof(int32_t) * n, s));
+  if (n == 0) return PG_OK;
+  const int blocks = int(std::min<int64_t>(ceil_div(n, 256), int64_t(num_sms()) * 8));
+  gather_i32_kernel<<<blocks, 256, 0, s>>>(src, order.as<int32_t>(), n, src_s.as<int32_t>());
+  PG_LAUNCH_CHECK();
+  gather_i32_kernel<<<blocks, 256, 0, s>>>(dst, order.as<int32_t>(), n, dst_s.as<int32_t>());
   PG_LAUNCH_CHECK();
   return PG_OK;
 }
@@ -329,9 +482,11 @@ extern "C" int pg_scatter_max(const float* features, const int32_t* centers, int
 }
 
 static int scatter_sum_impl(const float* features, const int32_t* centers, int64_t num_edges, int32_t num_channels,
-                            int64_t num_centers, float* out, bool mean, cudaStream_t s) {
+                            int64_t num_centers, float* out, bool mean, int32_t flags, cudaStream_t s) {
   PG_REQUIRE(out != nullptr || num_centers == 0, "pg_scatter_sum: out is null");
   PG_REQUIRE(num_channels >= 1 && num_edges >= 0 && num_centers >= 0, "pg_scatter_sum: bad sizes");
+  PG_REQUIRE((flags & ~PG_FLAG_DETERMINISTIC) == 0, "pg_scatter_sum: unknown flags 0x%x", flags);
+  const bool ordered = (flags & PG_FLAG_DETERMINISTIC) != 0;
   if (num_centers == 0) return PG_OK;
   PG_CUDA_OK(cudaMemsetAsync(out, 0, sizeof(float) * num_centers * num_channels, s));
   if (num_edges == 0) return PG_OK;
@@ -341,12 +496,26 @@ static int scatter_sum_impl(const float* features, const int32_t* centers, int64
     PG_CUDA_OK(count.alloc(sizeof(float) * num_centers, s));
     PG_CUDA_OK(cudaMemsetAsync(count.ptr, 0, sizeof(float) * num_centers, s));
   }
-  const int64_t chunks = ceil_div(num_edges, kScatterChunk);
   const int threads = num_channels >= 256 ? 256 : (num_channels >= 128 ? 128 : (num_channels >= 64 ? 64 : 32));
-  dim3 grid(ceil_div(num_channels, threads), int(std::min<int64_t>(chunks, 65535)));
-  scatter_sum_kernel<<<grid, threads, 0, s>>>(features, centers, num_edges, num_channels, num_centers, out,
-                                              mean ? count.as<float>() : nullptr);
-  PG_LAUNCH_CHECK();
+  if (ordered) {
+    Temp keys_s, order;
+    if (int rc = stable_order(centers, num_edges, num_centers, keys_s, order, s)) return rc;
+    const int64_t chunks = ceil_div(num_edges, PG_ORDERED_SCATTER_TILE);
+    OrderedParts parts;
+    if (int rc = parts.alloc(chunks, num_channels, s)) return rc;
+    dim3 grid(ceil_div(num_channels, threads), int(std::min<int64_t>(chunks, 65535)));
+    scatter_sum_ordered_kernel<<<grid, threads, 0, s>>>(features, order.as<int32_t>(), keys_s.as<uint64_t>(), num_edges,
+                                                        num_channels, num_centers, out,
+                                                        mean ? count.as<float>() : nullptr, parts.v(), parts.i());
+    PG_LAUNCH_CHECK();
+    if (int rc = ordered_fixup(parts, out, num_channels, s)) return rc;
+  } else {
+    const int64_t chunks = ceil_div(num_edges, kScatterChunk);
+    dim3 grid(ceil_div(num_channels, threads), int(std::min<int64_t>(chunks, 65535)));
+    scatter_sum_kernel<<<grid, threads, 0, s>>>(features, centers, num_edges, num_channels, num_centers, out,
+                                                mean ? count.as<float>() : nullptr);
+    PG_LAUNCH_CHECK();
+  }
   if (mean) {
     const int blocks = int(std::min<int64_t>(ceil_div(num_centers * num_channels, 256), int64_t(num_sms()) * 8));
     divide_rows_kernel<<<blocks, 256, 0, s>>>(out, count.as<float>(), num_centers, num_channels);
@@ -357,13 +526,26 @@ static int scatter_sum_impl(const float* features, const int32_t* centers, int64
 
 extern "C" int pg_scatter_sum(const float* features, const int32_t* centers, int64_t num_edges, int32_t num_channels,
                               int64_t num_centers, float* out, void* stream) {
-  return scatter_sum_impl(features, centers, num_edges, num_channels, num_centers, out, false,
+  return scatter_sum_impl(features, centers, num_edges, num_channels, num_centers, out, false, 0,
                           static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int pg_scatter_mean(const float* features, const int32_t* centers, int64_t num_edges, int32_t num_channels,
                                int64_t num_centers, float* out, void* stream) {
-  return scatter_sum_impl(features, centers, num_edges, num_channels, num_centers, out, true,
+  return scatter_sum_impl(features, centers, num_edges, num_channels, num_centers, out, true, 0,
+                          static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int pg_scatter_sum_flags(const float* features, const int32_t* centers, int64_t num_edges,
+                                    int32_t num_channels, int64_t num_centers, float* out, int32_t flags, void* stream) {
+  return scatter_sum_impl(features, centers, num_edges, num_channels, num_centers, out, false, flags,
+                          static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int pg_scatter_mean_flags(const float* features, const int32_t* centers, int64_t num_edges,
+                                     int32_t num_channels, int64_t num_centers, float* out, int32_t flags,
+                                     void* stream) {
+  return scatter_sum_impl(features, centers, num_edges, num_channels, num_centers, out, true, flags,
                           static_cast<cudaStream_t>(stream));
 }
 

@@ -25,6 +25,11 @@
 //                         atomicAdd into an output filled with 0.  The order of the fp32 partial sums is not fixed:
 //                         the last bits may differ from run to run.  Its instances are wg_segsum_kernel, the same
 //                         bodies under their own name
+//              EPI_SEGSUM_ORDERED the same sum in a fixed order (PG_FLAG_DETERMINISTIC, pg_common.cuh): a warp's 16
+//                         rows are a unit; its runs are reduced with the same shuffles, the halves' runs that meet at
+//                         rows 7 / 8 joined in registers (half 0 + half 1), and instead of atomics a run that holds
+//                         neither row 0 nor row 15 is stored, the two that do go to the side buffer for
+//                         ordered_fixup.  Its instances are wg_segsum_ordered_kernel
 //   activation the kAnyAct = false instances hard-code ReLU (linear too in the store epilogue): the kernel of every
 //              shipped config.  kAnyAct = true, the GNN edge layer with any other activation, is the same body with
 //              activate(p.act, .) in the producer; its segment max flushes the RAW maxima with the sign-aware
@@ -79,12 +84,15 @@
 #include "pg_wgmma.cuh"
 
 namespace pg {
-static std::atomic<long long> g_tc_launches[2];   // [0] segment-max (edge) launches, [1] store (dense) launches
+// [0] segment-max (edge) launches, [1] store (dense) launches, [2] ordered segment-sum fix-ups (any path)
+static std::atomic<long long> g_tc_launches[3];
+void count_ordered_launch() { g_tc_launches[2].fetch_add(1, std::memory_order_relaxed); }
 }
 
-// tensor-core kernel launches so far: which = 0 segment-max (edge layer) launches, 1 dense-layer launches
+// tensor-core kernel launches so far: which = 0 segment-max (edge layer) launches, 1 dense-layer launches, 2 the
+// fix-up launches of the ordered segment sum
 extern "C" int64_t pg_tc_launch_count(int32_t which) {
-  return (which == 0 || which == 1) ? pg::g_tc_launches[which].load(std::memory_order_relaxed) : -1;
+  return (which >= 0 && which <= 2) ? pg::g_tc_launches[which].load(std::memory_order_relaxed) : -1;
 }
 
 namespace pg {
@@ -140,7 +148,8 @@ constexpr size_t gnn_smem_bytes(int kp, int ni, int arith) {
 }
 
 enum { PROD_ROWS = 0, PROD_GNN = 1, PROD_POOL = 2 };
-enum { EPI_STORE = 0, EPI_SEGMAX = 1, EPI_SEGSUM = 2 };
+enum { EPI_STORE = 0, EPI_SEGMAX = 1, EPI_SEGSUM = 2, EPI_SEGSUM_ORDERED = 3 };
+constexpr bool is_sum(int epi) { return epi == EPI_SEGSUM || epi == EPI_SEGSUM_ORDERED; }
 
 struct WgParams {
   // A producer
@@ -177,6 +186,12 @@ struct WgParams {
   uint32_t stage_bytes;     // POOL: one W ring stage (the widest chunk of any layer of the launch)
   uint32_t region_bytes;    // POOL: one consumer warpgroup's A region
   int ring_log2;            // POOL: log2 of the ring depth
+  // SEGSUM_ORDERED: the side buffer (pg_common.cuh), slot 2 u + {0, 1} of 16-row unit u at part + slot * ldp; the
+  // launch of the first column block writes the slots' ids
+  float* part;
+  int32_t* part_id;
+  int ldp;
+  int write_ids;
 };
 
 __device__ __forceinline__ float2 ldg_nc(const float* ptr) {
@@ -203,6 +218,13 @@ __device__ __forceinline__ void seg_flush(const WgParams& p, int d, int col, flo
     // + 0.0f turns a -0.0f into +0.0f, which must win against the -FLT_MAX fill as an integer
     atomicMax(reinterpret_cast<int*>(dst), __float_as_int(fmaxf(m + __ldg(p.bias + col), 0.0f) + 0.0f));
   }
+}
+
+// EPI_SEGSUM_ORDERED: where the sums of destination d's run in unit u go, column by column: slot 2 u + slot of the side
+// buffer, or (slot < 0, a run that is the whole destination) d's row of out.  Computed once per run, so that the
+// epilogue's flushes are plain stores at a column offset (per-flush address arithmetic spills the car instances)
+__device__ __forceinline__ float* ordered_row(const WgParams& p, int64_t u, int slot, int d) {
+  return slot < 0 ? p.out + int64_t(max(d, 0)) * p.ldo : p.part + (2 * u + slot) * p.ldp;
 }
 
 // ptr[0 .. 2) through the read-only cache; ptr is 8-byte aligned
@@ -356,7 +378,8 @@ __device__ __forceinline__ void acc_from_bias(const WgParams& p, float (&acc)[NI
 template <int NI, int NS, bool kAnyAct, int kEpi>
 __device__ __forceinline__ void seg_epilogue(const WgParams& p, const float (&acc)[NS][NI / 2], int64_t r0, int lane,
                                              int col0) {
-  constexpr bool kSum = kEpi == EPI_SEGSUM;
+  constexpr bool kSum = is_sum(kEpi);
+  constexpr bool kOrdered = kEpi == EPI_SEGSUM_ORDERED;
   auto combine = [](float a, float b) { return kSum ? a + b : fmaxf(a, b); };
   const int cq = (lane & 3) * 2;
   // what an edge row contributes to the reduction: the raw accumulator (max), or act(acc) of an accumulator that
@@ -379,6 +402,8 @@ __device__ __forceinline__ void seg_epilogue(const WgParams& p, const float (&ac
     }
   }
   const int dw = __shfl_sync(0xffffffffu, d[0], 0);
+  // EPI_SEGSUM_ORDERED: the warp's 16 rows are unit u of the side buffer
+  const int64_t u = (r0 - (lane >> 2)) >> 4;
   if (__all_sync(0xffffffffu, d[0] == dw && d[1] == dw) && dw >= 0) {
     // the warp's 16 rows are one destination.  Value v of a thread is column (v / 2) * 8 + cq + v % 2; the 8
     // lanes sharing cq (lane bits 4, 3, 2) reduce-scatter their V values in three halving exchanges, after which
@@ -417,7 +442,69 @@ __device__ __forceinline__ void seg_epilogue(const WgParams& p, const float (&ac
 #pragma unroll
     for (int k = 0; k < L3; ++k) {
       const int v = v0 + k, col = col0 + (v >> 1) * 8 + cq + (v & 1);
-      if (k < nv && v < V && col < p.n) seg_flush<kEpi, kAnyAct>(p, dw, col, m[k]);
+      if constexpr (kOrdered) {
+        if (k < nv && v < V && col < p.n) ordered_row(p, u, 0, dw)[col] = m[k];   // the unit's one run: slot 0
+      } else {
+        if (k < nv && v < V && col < p.n) seg_flush<kEpi, kAnyAct>(p, dw, col, m[k]);
+      }
+    }
+    if (kOrdered && lane == 0 && p.write_ids && col0 == 0) p.part_id[2 * u] = dw;
+  } else if constexpr (kOrdered) {
+    // each half's runs as in the sum below; then the run that holds row 7 takes the sum of the one that holds row 8
+    // when they are one destination (half 0 + half 1).  The run that holds row 0 goes to slot 0, the one that holds
+    // row 15 to slot 1 (in this branch they are two runs), every other run is a whole destination and is stored
+    bool head[2];
+    bool same[2][3];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int up = __shfl_up_sync(0xffffffffu, d[h], 4);
+      head[h] = d[h] >= 0 && (lane < 4 || up != d[h]);
+      const bool next = __shfl_down_sync(0xffffffffu, d[h], 4) == d[h] && lane + 4 < 32;
+      const uint32_t m = __ballot_sync(0xffffffffu, next) >> (lane & ~3);
+      same[h][0] = (m & 0x1u) != 0;
+      same[h][1] = (m & 0x11u) == 0x11u;
+      same[h][2] = (m & 0x1111u) == 0x1111u;
+    }
+    const int d0 = __shfl_sync(0xffffffffu, d[0], 0), d7 = __shfl_sync(0xffffffffu, d[0], 28);
+    const int d8 = __shfl_sync(0xffffffffu, d[1], 0), d15 = __shfl_sync(0xffffffffu, d[1], 28);
+    const bool join = d8 >= 0 && d7 == d8;
+    // the last run head of each half (-1: none), as a row of the half
+    const int last0 = (31 - __clz(__ballot_sync(0xffffffffu, head[0]) & 0x11111111u)) >> 2;
+    const int last1 = (31 - __clz(__ballot_sync(0xffffffffu, head[1]) & 0x11111111u)) >> 2;
+    const int q = lane >> 2;
+    const bool take = join && q == last0;     // this row's half-0 run continues into half 1
+    const bool skip = join && q == 0;         // this row's half-1 run was taken by half 0
+    float* const to0 = ordered_row(p, u, q == 0 ? 0 : (take && last1 == 0 && d15 >= 0) ? 1 : -1, d[0]);
+    float* const to1 = ordered_row(p, u, (q == last1 && d15 >= 0) ? 1 : -1, d[1]);
+#pragma unroll
+    for (int i = 0; i < NS; ++i)
+#pragma unroll
+      for (int jj = 0; jj < NI / 8; ++jj)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          // half 1 first, so that one half's sum is live at a time (the any-activation car instance spills otherwise)
+          const int col = col0 + i * NI + jj * 8 + cq + c;
+          float first1 = 0.0f;   // the sum of the run that holds row 8
+#pragma unroll
+          for (int h = 1; h >= 0; --h) {
+            float m = value(i, jj, h, c);
+#pragma unroll
+            for (int s = 0; s < 3; ++s) {
+              const float o = __shfl_down_sync(0xffffffffu, m, 4 << s);
+              if (same[h][s]) m = m + o;
+            }
+            if (h == 1) {
+              first1 = __shfl_sync(0xffffffffu, m, lane & 3);
+              if (head[1] && !skip && col < p.n) to1[col] = m;
+            } else {
+              if (take) m = m + first1;
+              if (head[0] && col < p.n) to0[col] = m;
+            }
+          }
+        }
+    if (lane == 0 && p.write_ids && col0 == 0) {
+      if (d0 >= 0) p.part_id[2 * u] = d0;
+      if (d15 >= 0) p.part_id[2 * u + 1] = d15;
     }
   } else {
     // segmented max (sum) down each 8-row half; the first row of every run flushes the run's max (sum).  Column by
@@ -564,7 +651,7 @@ __device__ __forceinline__ void wg_gnn_body(const WgParams& p) {
   for (int tile = first; tile < num_tiles; tile += stride) {
     const int64_t row0 = int64_t(tile) * kGnnTileRows;
     float acc[1][NI / 2];
-    if constexpr (kEpi == EPI_SEGSUM) acc_from_bias<NI>(p, acc[0], group * NI, lane);
+    if constexpr (is_sum(kEpi)) acc_from_bias<NI>(p, acc[0], group * NI, lane);
     auto frag = [&](int kc, uint32_t (&hi)[4], uint32_t (&lo)[4]) {
       float2 q[4];
       gather.take(q);
@@ -575,7 +662,7 @@ __device__ __forceinline__ void wg_gnn_body(const WgParams& p) {
       wgmma_fence();
       const uint32_t b = w_base + uint32_t(kc) * kPlanes * kSlice;
       const uint64_t b_hi = make_smem_desc(b, 128, 256), b_lo = make_smem_desc(b + kSlice, 128, 256);
-      mma_rs<kArith, NI>(acc[0], hi, lo, b_hi, b_lo, kc > 0 || kEpi == EPI_SEGSUM ? 1 : 0);
+      mma_rs<kArith, NI>(acc[0], hi, lo, b_hi, b_lo, kc > 0 || is_sum(kEpi) ? 1 : 0);
       wgmma_commit();
       wgmma_wait<1>();                    // chunk kc - 1 complete: its A fragment is free
     });
@@ -779,7 +866,7 @@ __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
     // every accumulator is defined before its layer (the wgmmas read it, if only to scale it by 0): otherwise the
     // values of the previous tile would stay live through the on-chip layers, next to their accumulators
     float acc[NS][NI / 2];
-    if (kEpi == EPI_SEGSUM)
+    if (is_sum(kEpi))
 #pragma unroll
       for (int i = 0; i < NS; ++i) acc_from_bias<NI>(p, acc[i], i * NI, lane);
     else if (kProd == PROD_POOL)
@@ -787,7 +874,7 @@ __device__ __forceinline__ void wg_gemm_body(const WgParams& p) {
       for (int i = 0; i < NS; ++i)
 #pragma unroll
         for (int v = 0; v < NI / 2; ++v) acc[i][v] = 0.0f;
-    mma_layer(acc, nk, nl == 0, kEpi == EPI_SEGSUM);
+    mma_layer(acc, nk, nl == 0, is_sum(kEpi));
     // ---- epilogue ----------------------------------------------------------------------------------
     const int64_t r0 = tile * kTileRows + wgi * 64 + warp * 16 + (lane >> 2);
     const int cq = (lane & 3) * 2;
@@ -830,7 +917,7 @@ __device__ __forceinline__ void wg_body(const WgParams& p) {
 
 template <int kProd, int kEpi, int NI, int NS, int kArith, bool kAnyAct>
 __global__ void __launch_bounds__(kWgThreads, 1) wg_gemm_kernel(WgParams p) {
-  static_assert(kEpi != EPI_SEGSUM, "the segment-sum instances are wg_segsum_kernel");
+  static_assert(!is_sum(kEpi), "the segment-sum instances are wg_segsum_kernel and wg_segsum_ordered_kernel");
   wg_body<kProd, kEpi, NI, NS, kArith, kAnyAct>(p);
 }
 
@@ -842,10 +929,19 @@ __global__ void __launch_bounds__(kWgThreads, 1) wg_segsum_kernel(WgParams p) {
   wg_body<kProd, EPI_SEGSUM, NI, NS, kArith, kAnyAct>(p);
 }
 
-// the __global__ instance of a launch: wg_gemm_kernel, or wg_segsum_kernel for the segment sum
+// The ordered segment sum (EPI_SEGSUM_ORDERED, PG_FLAG_DETERMINISTIC): the same bodies again, under a third name so
+// that the atomic sum's family stays exactly the set it was
+template <int kProd, int NI, int NS, int kArith, bool kAnyAct>
+__global__ void __launch_bounds__(kWgThreads, 1) wg_segsum_ordered_kernel(WgParams p) {
+  wg_body<kProd, EPI_SEGSUM_ORDERED, NI, NS, kArith, kAnyAct>(p);
+}
+
+// the __global__ instance of a launch: wg_gemm_kernel, or wg_segsum_kernel / wg_segsum_ordered_kernel for the sums
 template <int kProd, int kEpi, int NI, int NS, int kArith, bool kAnyAct>
 void (*wg_kernel())(WgParams) {
-  if constexpr (kEpi == EPI_SEGSUM)
+  if constexpr (kEpi == EPI_SEGSUM_ORDERED)
+    return wg_segsum_ordered_kernel<kProd, NI, NS, kArith, kAnyAct>;
+  else if constexpr (kEpi == EPI_SEGSUM)
     return wg_segsum_kernel<kProd, NI, NS, kArith, kAnyAct>;
   else
     return wg_gemm_kernel<kProd, kEpi, NI, NS, kArith, kAnyAct>;
@@ -1249,10 +1345,41 @@ int prepare_edge(PreparedEdge& e, int mode, int c_in, const float* const* weight
   return PG_OK;
 }
 
-// the segment-reduction layer over all column blocks: the max (agg PG_AGG_MAX) or the sum; p carries the producer's
-// inputs
+// the ordered segment sum (pg_common.cuh) over all column blocks: kOrderedSlice edges at a time (a multiple of every
+// tile), each slice's launches writing their columns of one side buffer (the first block its ids), then its fix-up
 template <int kProd>
-int apply_last(const PreparedEdge& e, WgParams p, int n, int agg, float* out, cudaStream_t s) {
+int apply_last_ordered(const PreparedEdge& e, const WgParams& p, int n, float* out, cudaStream_t s) {
+  OrderedParts parts;
+  if (int rc = parts.alloc(ceil_div(std::min(p.num_rows, kOrderedSlice), 16), n, s)) return rc;
+  for (int64_t e0 = 0; e0 < p.num_rows; e0 += kOrderedSlice) {
+    if (e0 > 0)
+      if (int rc = parts.reset(s)) return rc;
+    WgParams q = p;
+    q.num_rows = std::min(kOrderedSlice, p.num_rows - e0);
+    q.dst = p.dst + e0;
+    if (kProd == PROD_ROWS)
+      q.x = p.x + e0 * p.ldx;   // the stored per-edge rows (GNN: x is the per-vertex table P)
+    else
+      q.src = p.src + e0;
+    q.part_id = parts.i();
+    q.ldp = n;
+    for (size_t b = 0; b < e.last.size(); ++b) {
+      q.out = out + e.last_col0[b];
+      q.ldo = n;
+      q.part = parts.v() + e.last_col0[b];
+      q.write_ids = b == 0;
+      if (int rc = launch_wg<kProd, EPI_SEGSUM_ORDERED>(q, e.last[b], s, &e.chain)) return rc;
+    }
+    if (int rc = ordered_fixup(parts, out, n, s)) return rc;
+  }
+  return PG_OK;
+}
+
+// the segment-reduction layer over all column blocks: the max (agg PG_AGG_MAX) or the sum, in a fixed order when
+// ordered; p carries the producer's inputs
+template <int kProd>
+int apply_last(const PreparedEdge& e, WgParams p, int n, int agg, bool ordered, float* out, cudaStream_t s) {
+  if (agg != PG_AGG_MAX && ordered) return apply_last_ordered<kProd>(e, p, n, out, s);
   for (size_t b = 0; b < e.last.size(); ++b) {
     p.out = out + e.last_col0[b];
     p.ldo = n;
@@ -1263,15 +1390,15 @@ int apply_last(const PreparedEdge& e, WgParams p, int n, int agg, float* out, cu
   return PG_OK;
 }
 
-// the launches of one edge call: the segment max (sum) into out (pre-filled with -FLT_MAX or 0); an out-of-range
-// src / dst sets *err
+// the launches of one edge call: the segment max (sum, ordered or not) into out (pre-filled with -FLT_MAX or 0); an
+// out-of-range src / dst sets *err
 int launch_edge(const PreparedEdge& e, const float* features, const float* xyz_src, const float* xyz_dst,
                 const int32_t* dst_index, const int32_t* src, const int32_t* dst, int64_t num_edges, int64_t num_src,
-                int64_t num_dst, int agg, float* out, int* err, cudaStream_t s) {
+                int64_t num_dst, int agg, bool ordered, float* out, int* err, cudaStream_t s) {
   const int n = e.dims[e.num_layers];
   if (e.path == EDGE_FP32 || num_edges == 0)
     return edge_mlp_max_fp32(e.mode, features, e.c_in, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst,
-                             e.w.data(), e.b.data(), e.dims.data(), e.num_layers, e.act, agg, out, err, s);
+                             e.w.data(), e.b.data(), e.dims.data(), e.num_layers, e.act, agg, ordered, out, err, s);
   WgParams p{};
   p.xyz_src = xyz_src;
   p.xyz_dst = xyz_dst;
@@ -1287,7 +1414,7 @@ int launch_edge(const PreparedEdge& e, const float* features, const float* xyz_s
     p.src = src;
     p.dst = dst;
     p.num_rows = num_edges;
-    if (e.chain_end == L - 1) return apply_last<PROD_POOL>(e, p, n, agg, out, s);
+    if (e.chain_end == L - 1) return apply_last<PROD_POOL>(e, p, n, agg, ordered, out, s);
     // the last layer is wider than one launch: the chain stores its input once, and its column blocks read it back.
     // The stored rows are bounded by slicing the edge list (a destination whose edges straddle two slices is merged
     // by the atomic max like any tile boundary)
@@ -1313,7 +1440,7 @@ int launch_edge(const PreparedEdge& e, const float* features, const float* xyz_s
       r.dst = dst + e0;
       r.num_dst = num_dst;
       r.err = err;
-      if (int rc = apply_last<PROD_ROWS>(e, r, n, agg, out, s)) return rc;
+      if (int rc = apply_last<PROD_ROWS>(e, r, n, agg, ordered, out, s)) return rc;
     }
     return PG_OK;
   }
@@ -1328,21 +1455,32 @@ int launch_edge(const PreparedEdge& e, const float* features, const float* xyz_s
   p.dst = dst;
   p.num_rows = num_edges;
   p.act = e.act;
-  return apply_last<PROD_GNN>(e, p, n, agg, out, s);
+  return apply_last<PROD_GNN>(e, p, n, agg, ordered, out, s);
 }
 
 // one edge call on either route: the error word, the fill of out (-FLT_MAX for the max, 0 for the sum and the mean),
 // the launches, the division of the mean, and the read-back of the error word unless the caller vouched for the
-// indices (trusted: no read-back, no synchronisation)
+// indices (trusted: no read-back, no synchronisation).  ordered (PG_FLAG_DETERMINISTIC): the sum and the mean in a
+// fixed order; the max ignores it
 int apply_edge(const PreparedEdge& e, const float* features, const float* xyz_src, const float* xyz_dst,
                const int32_t* dst_index, const int32_t* src, const int32_t* dst, int64_t num_edges, int64_t num_src,
-               int64_t num_dst, bool trusted, int agg, float* out, cudaStream_t s) {
+               int64_t num_dst, bool trusted, int agg, bool ordered, float* out, cudaStream_t s) {
   const int n = e.dims[e.num_layers];
   ErrorWord err;
   if (int rc = err.init(s)) return rc;
   if (int rc = fill_async(out, num_dst * n, agg == PG_AGG_MAX ? -FLT_MAX : 0.0f, s)) return rc;
-  if (int rc = launch_edge(e, features, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst, agg, out,
-                           err.ptr(), s))
+  // the ordered sum stores each destination that lies inside one unit, so it needs every destination's edges adjacent:
+  // it runs on the edge list stable-sorted by dst (the same list for one in CSR order; out-of-range dst last, still
+  // reported)
+  ordered = ordered && agg != PG_AGG_MAX && num_edges > 0;
+  Temp src_s, dst_s;
+  if (ordered) {
+    if (int rc = sort_edges_by_dst(src, dst, num_edges, num_dst, src_s, dst_s, s)) return rc;
+    src = src_s.as<int32_t>();
+    dst = dst_s.as<int32_t>();
+  }
+  if (int rc = launch_edge(e, features, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst, agg, ordered,
+                           out, err.ptr(), s))
     return rc;
   // the any-activation wg_gemm_kernel left the raw maxima: the last layer's bias and activation, once per element
   if (agg == PG_AGG_MAX && e.path != EDGE_FP32 && e.act != PG_ACT_RELU && num_edges > 0)
@@ -1619,6 +1757,7 @@ extern "C" int pg_edge_mlp_max(int32_t mode, const float* features, int32_t num_
   PG_REQUIRE(mode == PG_EDGE_GNN || dst_index != nullptr || num_edges == 0,
              "pg_edge_mlp_max: POOL mode needs keypoint indices");
   const bool trusted = (precision & PG_FLAG_TRUSTED_INDICES) != 0;
+  const bool ordered = (precision & PG_FLAG_DETERMINISTIC) != 0;
   const int act = activation_of(precision);
   PG_REQUIRE(act >= 0, "pg_edge_mlp_max: unknown activation");
   const int agg = aggregation_of(precision);
@@ -1629,8 +1768,8 @@ extern "C" int pg_edge_mlp_max(int32_t mode, const float* features, int32_t num_
   if (int rc = prepare_edge(e, mode, num_feature_channels, weights_host, biases_host, dims_host, num_layers, act,
                             precision != 0 && num_edges > 0 && pg_tc_available(), arith_of(precision), s))
     return rc;
-  return apply_edge(e, features, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst, trusted, agg, out,
-                    s);
+  return apply_edge(e, features, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst, trusted, agg,
+                    ordered, out, s);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -1655,6 +1794,8 @@ extern "C" int pg_layer_create(int32_t kind, const float* const* weights_host, c
   const int act = activation_of(precision);
   PG_REQUIRE(act >= 0, "pg_layer_create: unknown activation");
   const bool separated = (precision & PG_FLAG_SEPARATED) != 0;
+  PG_REQUIRE(!(precision & PG_FLAG_DETERMINISTIC),
+             "pg_layer_create: PG_FLAG_DETERMINISTIC is a flag of the edge calls (the aggregation is chosen per call)");
   precision &= ~(PG_FLAG_ACTIVATION | PG_ACT_MASK | PG_FLAG_SEPARATED);
   PG_REQUIRE(precision >= 0 && precision <= 2, "pg_layer_create: unknown precision %d", precision);
   PG_REQUIRE(kind == PG_LAYER_MLP || kind == PG_LAYER_EDGE_POOL || kind == PG_LAYER_EDGE_GNN || kind == PG_LAYER_PREDICTOR,
@@ -1734,7 +1875,7 @@ extern "C" int pg_layer_edge_mlp_max(const pg_layer* layer, const float* feature
   const int agg = aggregation_of(flags);
   PG_REQUIRE(agg >= 0, "pg_layer_edge_mlp_max: unknown aggregation");
   return apply_edge(layer->edge, features, xyz_src, xyz_dst, dst_index, src, dst, num_edges, num_src, num_dst,
-                    (flags & PG_FLAG_TRUSTED_INDICES) != 0, agg, out, s);
+                    (flags & PG_FLAG_TRUSTED_INDICES) != 0, agg, (flags & PG_FLAG_DETERMINISTIC) != 0, out, s);
 }
 
 extern "C" int pg_layer_predictor(const pg_layer* layer, const float* x, int64_t m, float* logits, float* boxes,

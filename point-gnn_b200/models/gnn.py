@@ -184,7 +184,9 @@ def graph_scatter_max_fn(point_features, point_centers, num_centers):
 def graph_scatter_sum_fn(point_features, point_centers, num_centers):
     """gnn.py:111-114 (tf.math.unsorted_segment_sum; empty segment -> 0).  No shipped config selects it; as the
     ``aggregation_fn`` of PointSetPooling or GraphNetAutoCenter it runs in the fused edge kernels, which add fp32
-    partial sums with atomics: the last bits may differ from run to run, as with TF's GPU kernel."""
+    partial sums with atomics: the last bits may differ from run to run, as with TF's GPU kernel.  Under
+    ``torch.use_deterministic_algorithms(True)`` this function and the fused kernels add them in a fixed order instead:
+    the same bits on every run."""
     centers = point_centers.reshape(-1).to(torch.int32).contiguous()
     return _lib.scatter_sum(point_features.contiguous(), centers, int(num_centers))
 
