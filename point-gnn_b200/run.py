@@ -40,13 +40,26 @@ charged to the step whose wait it ends:
                  conversion, which its ``nms`` timer covers)
   total          wall time of the whole loop, file writes included, divided by the number of frames
 
+Processes.  ``--processes N`` (default 1) runs the split in N spawned worker processes: rank r takes positions
+r, r + N, r + 2N, ... of the split (``rank_batches``), batches them ``--batch_size`` at a time and runs them on device
+``r % torch.cuda.device_count()``, so ``CUDA_VISIBLE_DEVICES`` picks the devices and N above the device count puts
+several ranks on one device, whose host work then overlaps.  Each rank has its own reader thread, graph prefetcher,
+model and prepared layers and writes its own frames' files; the files are those of one process.  The parent checks
+the command line, the config and the split before it spawns anything, prints the timers of the whole job (each stage
+summed over the ranks, ``total`` the slowest rank's loop) and returns them.  A rank that raises, or a Ctrl-C, stops
+every rank before ``main`` raises.  With N = 1 nothing is spawned: the run happens in the calling process.
+
     python -m pointgnn_b200.run CHECKPOINT_PATH [--test] [--no-box-merge] [--no-box-score]
            [--dataset_root_dir DIR] [--dataset_split_file FILE] [--output_dir DIR] [--precision fp32|bf16x3|fp16]
-           [--batch_size N]
+           [--batch_size N] [--processes N]
 """
 import argparse
+import multiprocessing
 import os
+import queue
+import signal
 import time
+import traceback
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
@@ -62,6 +75,7 @@ from pointgnn_b200.models.graph_gen import get_graph_generate_fn
 from pointgnn_b200.models.models import get_model
 from pointgnn_b200.util.config_util import load_config
 from pointgnn_b200.utils.prefetch import GraphPrefetcher
+from pointgnn_b200.utils.sharding import frames_for_rank
 
 
 def occlusion(label, xyz):
@@ -168,34 +182,10 @@ def write_kitti_file(filename, pred_labels):
         f.write('\n')
 
 
-def main(argv=None):
-    parser = argparse.ArgumentParser(description='Point-GNN inference on KITTI (H100 twin of run.py)')
-    parser.add_argument('checkpoint_path', type=str, help='Path to checkpoint')
-    parser.add_argument('-l', '--level', type=int, default=0, help='Visualization level: only 0 (disabled) is built')
-    parser.add_argument('--test', dest='test', action='store_true', default=False, help='Enable test model')
-    parser.add_argument('--no-box-merge', dest='use_box_merge', action='store_false', default=True,
-                        help='Disable box merge.')
-    parser.add_argument('--no-box-score', dest='use_box_score', action='store_false', default=True,
-                        help='Disable box score.')
-    parser.add_argument('--dataset_root_dir', type=str, default='../dataset/kitti/',
-                        help='Path to KITTI dataset. Default="../dataset/kitti/"')
-    parser.add_argument('--dataset_split_file', type=str, default='',
-                        help='Path to KITTI dataset split file. Default="DATASET_ROOT_DIR/3DOP_splits/val.txt"')
-    parser.add_argument('--output_dir', type=str, default='',
-                        help='Path to save the detection results. Default="CHECKPOINT_PATH/eval/"')
-    parser.add_argument('--precision', type=str, default=None, choices=['fp32', 'bf16x3', 'fp16'],
-                        help='Arithmetic of the dense layers (default: bf16x3 on sm_90, fp32-class accuracy; fp16: '
-                             'one FP16 tensor-core pass, ~1e-2 on logits)')
-    parser.add_argument('--batch_size', type=int, default=1,
-                        help='Frames per forward pass (consecutive frames of the split; default 1)')
-    args = parser.parse_args(argv)
-    if args.batch_size < 1:
-        parser.error('--batch_size must be >= 1, got %d' % args.batch_size)
-    if args.level != 0:
-        raise NotImplementedError('visualisation levels 1 / 2 (Open3D windows) are not built')
+def open_job(args):
+    """What ``main`` reads and checks before the first frame: the config (its codec must be one run.py decodes) and
+    the split -> (config, dataset, output directory)."""
     IS_TEST = args.test
-    USE_BOX_MERGE = args.use_box_merge
-    USE_BOX_SCORE = args.use_box_score
     DATASET_DIR = args.dataset_root_dir
     if args.dataset_split_file == '':
         DATASET_SPLIT_FILE = os.path.join(DATASET_DIR, './3DOP_splits/val.txt')
@@ -205,8 +195,7 @@ def main(argv=None):
         OUTPUT_DIR = os.path.join(args.checkpoint_path, './eval/')
     else:
         OUTPUT_DIR = args.output_dir
-    CHECKPOINT_PATH = args.checkpoint_path
-    CONFIG_PATH = os.path.join(CHECKPOINT_PATH, 'config')
+    CONFIG_PATH = os.path.join(args.checkpoint_path, 'config')
     assert os.path.isfile(CONFIG_PATH), 'No config file found in %s' % CONFIG_PATH
     config = load_config(CONFIG_PATH)
     # the decoding rule of the model's box codec; a codec run.py cannot decode fails here, before any frame is read
@@ -229,15 +218,24 @@ def main(argv=None):
             DATASET_SPLIT_FILE,
             num_classes=config['num_classes'],
             is_training=False)       # labels are only read for visualisation in the reference; not needed here
-    NUM_TEST_SAMPLE = dataset.num_files
+    return config, dataset, OUTPUT_DIR
+
+
+def run_batches(args, config, dataset, output_dir, batches):
+    """Run ``batches`` (lists of positions in the split) on the current device and write their files -> the timers'
+    sums in seconds.  The work of one process: ``main`` calls it in-process, each rank of ``--processes`` in its
+    worker."""
+    USE_BOX_MERGE = args.use_box_merge
+    USE_BOX_SCORE = args.use_box_score
+    OUTPUT_DIR = output_dir
     NUM_CLASSES = dataset.num_classes
     # setup model =============================================================
     BOX_ENCODING_LEN = get_encoding_len(config['box_encoding_method'])
     pointgnn_b200.set_precision(args.precision or ('bf16x3' if _lib.tc_available() else 'fp32'))
     model = get_model(config['model_name'])(num_classes=NUM_CLASSES, box_encoding_len=BOX_ENCODING_LEN, mode='test',
                                             **config['model_kwargs'])
-    print('Restore from checkpoint %s' % CHECKPOINT_PATH)
-    model.load_checkpoint(CHECKPOINT_PATH)
+    print('Restore from checkpoint %s' % args.checkpoint_path)
+    model.load_checkpoint(args.checkpoint_path)
     graph_generate_fn = get_graph_generate_fn(config['graph_gen_method'])
     device = torch.device('cuda', torch.cuda.current_device())
     # running network =========================================================
@@ -248,8 +246,6 @@ def main(argv=None):
 
     want_rgb = config['input_features'] in ('irgb', '0rgb')
     last_layer_graph_level = config['model_kwargs']['layer_configs'][-1]['graph_level']
-    batches = [list(range(first, min(first + args.batch_size, NUM_TEST_SAMPLE)))
-               for first in range(0, NUM_TEST_SAMPLE, args.batch_size)]
 
     def read_files(frames):
         """Host file work of one batch (worker thread): velodyne, calibration, image or only its size."""
@@ -330,6 +326,131 @@ def main(argv=None):
             charge('total', time.time() - start_time)
     finally:
         reader.shutdown(wait=True, cancel_futures=True)
+    return time_dict
+
+
+def rank_batches(num_frames, batch_size, rank, world):
+    """Batches of rank ``rank`` of ``world``: its positions in the split (``frames_for_rank``: rank, rank + world,
+    ...) cut ``batch_size`` at a time, the last batch possibly shorter.  World 1 gives consecutive frames."""
+    frames = frames_for_rank(num_frames, rank, world)
+    return [frames[first:first + batch_size] for first in range(0, len(frames), batch_size)]
+
+
+def merge_rank_times(per_rank):
+    """The ranks' timer sums, in rank order -> the job's: each stage summed over the ranks, ``total`` the slowest
+    rank's loop, so that frames / total is the job's frames/s."""
+    merged = {}
+    for times in per_rank:
+        for key, seconds in times.items():
+            merged[key] = max(merged.get(key, 0), seconds) if key == 'total' else merged.get(key, 0) + seconds
+    return merged
+
+
+def _rank_main(args, rank, device, deterministic, results):
+    """Worker process of rank ``rank``: its batches on ``device`` -> ('done', rank, timers) or ('failed', rank,
+    traceback text) on ``results``.  A rank without frames loads nothing and reports no time."""
+    # the parent alone answers Ctrl-C, by stopping every rank
+    signal.signal(signal.SIGINT, signal.SIG_IGN)
+    try:
+        # a spawned interpreter starts with the switch off; turn it on as the caller had it (only then: the call
+        # imports torch._inductor, seconds of start-up)
+        if deterministic[0]:
+            torch.use_deterministic_algorithms(True, warn_only=deterministic[1])
+        config, dataset, output_dir = open_job(args)
+        batches = rank_batches(dataset.num_files, args.batch_size, rank, args.processes)
+        time_dict = {}
+        if batches:
+            torch.cuda.set_device(device)
+            time_dict = run_batches(args, config, dataset, output_dir, batches)
+        results.put(('done', rank, time_dict))
+    except BaseException:
+        results.put(('failed', rank, traceback.format_exc()))
+
+
+def run_ranks(args):
+    """Run the ``args.processes`` ranks in spawned processes (CUDA cannot be forked), rank r on device
+    r % device count -> ``merge_rank_times`` of their timers.  If a rank fails, or on Ctrl-C, every rank is stopped
+    and waited for before the exception, which names the failing rank and carries its traceback, propagates."""
+    devices = torch.cuda.device_count()
+    if devices == 0:
+        raise RuntimeError('point-gnn_b200 needs a CUDA device (no CPU fallback)')
+    world = args.processes
+    deterministic = (torch.are_deterministic_algorithms_enabled(),
+                     torch.is_deterministic_algorithms_warn_only_enabled())
+    context = multiprocessing.get_context('spawn')
+    results = context.Queue()
+    started, done, finished = [], {}, False
+    try:
+        for rank in range(world):
+            proc = context.Process(target=_rank_main, args=(args, rank, rank % devices, deterministic, results),
+                                   name='pointgnn_b200.run rank %d' % rank)
+            proc.start()
+            started.append(proc)
+        while len(done) < world:
+            try:
+                status, rank, payload = results.get(timeout=1.0)
+            except queue.Empty:
+                # a rank reports before it returns, so a non-zero exit code without a report is a crash
+                for r, proc in enumerate(started):
+                    if r not in done and proc.exitcode not in (None, 0):
+                        raise RuntimeError('run.py rank %d of %d exited with code %d without a report'
+                                           % (r, world, proc.exitcode))
+                continue
+            if status == 'failed':
+                raise RuntimeError('run.py rank %d of %d failed:\n%s' % (rank, world, payload))
+            done[rank] = payload
+        finished = True
+    finally:
+        for proc in started:
+            if not finished:
+                proc.terminate()
+        for proc in started:
+            proc.join(None if finished else 30)
+            if proc.is_alive():
+                proc.kill()
+                proc.join()
+        results.close()
+    return merge_rank_times([done[rank] for rank in range(world)])
+
+
+def main(argv=None):
+    parser = argparse.ArgumentParser(description='Point-GNN inference on KITTI (H100 twin of run.py)')
+    parser.add_argument('checkpoint_path', type=str, help='Path to checkpoint')
+    parser.add_argument('-l', '--level', type=int, default=0, help='Visualization level: only 0 (disabled) is built')
+    parser.add_argument('--test', dest='test', action='store_true', default=False, help='Enable test model')
+    parser.add_argument('--no-box-merge', dest='use_box_merge', action='store_false', default=True,
+                        help='Disable box merge.')
+    parser.add_argument('--no-box-score', dest='use_box_score', action='store_false', default=True,
+                        help='Disable box score.')
+    parser.add_argument('--dataset_root_dir', type=str, default='../dataset/kitti/',
+                        help='Path to KITTI dataset. Default="../dataset/kitti/"')
+    parser.add_argument('--dataset_split_file', type=str, default='',
+                        help='Path to KITTI dataset split file. Default="DATASET_ROOT_DIR/3DOP_splits/val.txt"')
+    parser.add_argument('--output_dir', type=str, default='',
+                        help='Path to save the detection results. Default="CHECKPOINT_PATH/eval/"')
+    parser.add_argument('--precision', type=str, default=None, choices=['fp32', 'bf16x3', 'fp16'],
+                        help='Arithmetic of the dense layers (default: bf16x3 on sm_90, fp32-class accuracy; fp16: '
+                             'one FP16 tensor-core pass, ~1e-2 on logits)')
+    parser.add_argument('--batch_size', type=int, default=1,
+                        help='Frames per forward pass (consecutive frames of the split, or of a rank\'s share of it '
+                             'with --processes; default 1)')
+    parser.add_argument('--processes', type=int, default=1,
+                        help='Worker processes, frames sharded round-robin over them; rank r runs on device '
+                             'r %% torch.cuda.device_count() (default 1: run in this process, spawn nothing)')
+    args = parser.parse_args(argv)
+    if args.batch_size < 1:
+        parser.error('--batch_size must be >= 1, got %d' % args.batch_size)
+    if args.processes < 1:
+        parser.error('--processes must be >= 1, got %d' % args.processes)
+    if args.level != 0:
+        raise NotImplementedError('visualisation levels 1 / 2 (Open3D windows) are not built')
+    config, dataset, output_dir = open_job(args)
+    NUM_TEST_SAMPLE = dataset.num_files
+    if args.processes == 1:
+        time_dict = run_batches(args, config, dataset, output_dir,
+                                rank_batches(NUM_TEST_SAMPLE, args.batch_size, 0, 1))
+    else:
+        time_dict = run_ranks(args)
     # time statics ============================================================
     for key in time_dict:
         print(key + ' time : ' + str(time_dict[key] / max(NUM_TEST_SAMPLE, 1)))
