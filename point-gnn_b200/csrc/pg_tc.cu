@@ -18,7 +18,7 @@
 //              EPI_SEGMAX max over the edges of each destination (edges are grouped by destination):
 //                         bias and every activation are monotone, so they commute with max: raw accumulators
 //                         are reduced across the warp's 16 rows with shuffles and each partial max is flushed
-//                         with one atomic
+//                         with one atomic; a warp holding two destinations (rows 0 and 15) reduces each in turn
 //              EPI_SEGSUM sum over the edges of each destination (the mean divides it afterwards, apply_edge): bias
 //                         and activation do not commute with a sum, so the accumulators start at the bias and act is
 //                         applied to every element in registers first; then the same reduction with + and a flush with
@@ -404,48 +404,69 @@ __device__ __forceinline__ void seg_epilogue(const WgParams& p, const float (&ac
   const int dw = __shfl_sync(0xffffffffu, d[0], 0);
   // EPI_SEGSUM_ORDERED: the warp's 16 rows are unit u of the side buffer
   const int64_t u = (r0 - (lane >> 2)) >> 4;
-  if (__all_sync(0xffffffffu, d[0] == dw && d[1] == dw) && dw >= 0) {
-    // the warp's 16 rows are one destination.  Value v of a thread is column (v / 2) * 8 + cq + v % 2; the 8
-    // lanes sharing cq (lane bits 4, 3, 2) reduce-scatter their V values in three halving exchanges, after which
-    // every lane holds the full maxima (sums) of V / 8 (rounded up or down) of them and all 32 lanes flush.  V is padded
-    // with -FLT_MAX (0) values to VP, a multiple of 4, so that the first two exchanges halve evenly (V = 38 at NI = 152,
-    // NS = 1)
+  const bool uniform = __all_sync(0xffffffffu, d[0] == dw && d[1] == dw) && dw >= 0;
+  // EPI_SEGMAX: a warp whose every row has the destination of row 0 or that of row 15 (-1 included), as at a run
+  // boundary of a grouped edge list, reduce-scatters each of the two in turn with the other's rows masked to
+  // -FLT_MAX.  Two passes of L3 flushes each, where the segmented scan below issues 2 x NI x NS / 4 flush instructions
+  // after three shuffles per column and half.  Max is exact and each row still reaches a flush of its own destination.
+  // One accumulator group only (NS = 1: every GNN edge launch): the 152 x 2 ROWS instance spills with it
+  int dz = dw;
+  bool two = false;
+  if constexpr (kEpi == EPI_SEGMAX && NS == 1) {
+    dz = __shfl_sync(0xffffffffu, d[1], 28);
+    two = !uniform && __all_sync(0xffffffffu, (d[0] == dw || d[0] == dz) && (d[1] == dw || d[1] == dz));
+  }
+  if (uniform || two) {
+    // the warp's 16 rows are one destination (or two, one pass each).  Value v of a thread is column (v / 2) * 8 +
+    // cq + v % 2; the 8 lanes sharing cq (lane bits 4, 3, 2) reduce-scatter their V values in three halving
+    // exchanges, after which every lane holds the full maxima (sums) of V / 8 (rounded up or down) of them and all 32
+    // lanes flush.  V is padded with -FLT_MAX (0) values to VP, a multiple of 4, so that the first two exchanges
+    // halve evenly (V = 38 at NI = 152, NS = 1)
     constexpr int V = NI * NS / 4, VP = (V + 3) / 4 * 4, L1 = VP / 2, L2 = VP / 4, L3 = (L2 + 1) / 2;
-    float m[VP];
+#pragma unroll 1
+    for (int pass = 0; pass < (two ? 2 : 1); ++pass) {
+      const int t = pass ? dz : dw;   // the destination of this pass
+      if (t < 0) continue;
+      float m[VP];
 #pragma unroll
-    for (int i = 0; i < NS; ++i)
+      for (int i = 0; i < NS; ++i)
 #pragma unroll
-      for (int jj = 0; jj < NI / 8; ++jj)
+        for (int jj = 0; jj < NI / 8; ++jj)
 #pragma unroll
-        for (int c = 0; c < 2; ++c) m[(i * (NI / 8) + jj) * 2 + c] = combine(value(i, jj, 0, c), value(i, jj, 1, c));
+          for (int c = 0; c < 2; ++c) {
+            const float a0 = value(i, jj, 0, c), a1 = value(i, jj, 1, c);
+            m[(i * (NI / 8) + jj) * 2 + c] =
+                two ? combine(d[0] == t ? a0 : -FLT_MAX, d[1] == t ? a1 : -FLT_MAX) : combine(a0, a1);
+          }
 #pragma unroll
-    for (int v = V; v < VP; ++v) m[v] = kSum ? 0.0f : -FLT_MAX;
-    const bool b4 = lane & 16, b3 = lane & 8, b2 = lane & 4;
-    // a lane with the bit set keeps the upper part, its partner the lower; each sends the part it gives up
+      for (int v = V; v < VP; ++v) m[v] = kSum ? 0.0f : -FLT_MAX;
+      const bool b4 = lane & 16, b3 = lane & 8, b2 = lane & 4;
+      // a lane with the bit set keeps the upper part, its partner the lower; each sends the part it gives up
 #pragma unroll
-    for (int k = 0; k < L1; ++k) {
-      const float keep = b4 ? m[k + L1] : m[k], give = b4 ? m[k] : m[k + L1];
-      m[k] = combine(keep, __shfl_xor_sync(0xffffffffu, give, 16));
-    }
+      for (int k = 0; k < L1; ++k) {
+        const float keep = b4 ? m[k + L1] : m[k], give = b4 ? m[k] : m[k + L1];
+        m[k] = combine(keep, __shfl_xor_sync(0xffffffffu, give, 16));
+      }
 #pragma unroll
-    for (int k = 0; k < L2; ++k) {
-      const float keep = b3 ? m[k + L2] : m[k], give = b3 ? m[k] : m[k + L2];
-      m[k] = combine(keep, __shfl_xor_sync(0xffffffffu, give, 8));
-    }
+      for (int k = 0; k < L2; ++k) {
+        const float keep = b3 ? m[k + L2] : m[k], give = b3 ? m[k] : m[k + L2];
+        m[k] = combine(keep, __shfl_xor_sync(0xffffffffu, give, 8));
+      }
 #pragma unroll
-    for (int k = 0; k < L3; ++k) {
-      const float up = k + L3 < L2 ? m[k + L3] : m[k];   // L2 odd: the upper part is one value shorter
-      const float keep = b2 ? up : m[k], give = b2 ? m[k] : up;
-      m[k] = combine(keep, __shfl_xor_sync(0xffffffffu, give, 4));
-    }
-    const int v0 = (b4 ? L1 : 0) + (b3 ? L2 : 0) + (b2 ? L3 : 0), nv = b2 ? L2 - L3 : L3;
+      for (int k = 0; k < L3; ++k) {
+        const float up = k + L3 < L2 ? m[k + L3] : m[k];   // L2 odd: the upper part is one value shorter
+        const float keep = b2 ? up : m[k], give = b2 ? m[k] : up;
+        m[k] = combine(keep, __shfl_xor_sync(0xffffffffu, give, 4));
+      }
+      const int v0 = (b4 ? L1 : 0) + (b3 ? L2 : 0) + (b2 ? L3 : 0), nv = b2 ? L2 - L3 : L3;
 #pragma unroll
-    for (int k = 0; k < L3; ++k) {
-      const int v = v0 + k, col = col0 + (v >> 1) * 8 + cq + (v & 1);
-      if constexpr (kOrdered) {
-        if (k < nv && v < V && col < p.n) ordered_row(p, u, 0, dw)[col] = m[k];   // the unit's one run: slot 0
-      } else {
-        if (k < nv && v < V && col < p.n) seg_flush<kEpi, kAnyAct>(p, dw, col, m[k]);
+      for (int k = 0; k < L3; ++k) {
+        const int v = v0 + k, col = col0 + (v >> 1) * 8 + cq + (v & 1);
+        if constexpr (kOrdered) {
+          if (k < nv && v < V && col < p.n) ordered_row(p, u, 0, dw)[col] = m[k];   // the unit's one run: slot 0
+        } else {
+          if (k < nv && v < V && col < p.n) seg_flush<kEpi, kAnyAct>(p, t, col, m[k]);
+        }
       }
     }
     if (kOrdered && lane == 0 && p.write_ids && col0 == 0) p.part_id[2 * u] = dw;
