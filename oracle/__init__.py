@@ -20,7 +20,10 @@ build container, with the fixtures and the generating script committed
   interpreted node by node by ``oracle/graphdef.py`` (NumPy; TensorFlow itself
   cannot be installed) with the trained weights -> tests/golden/gnn_*.npz for all
   seven shipped checkpoints.  ``oracle/gnn.py`` reproduces those vectors exactly
-  (tests/test_graphdef_cpu.py), so it is a checked restatement, not a guess.
+  (tests/test_graphdef_cpu.py), so it is a checked restatement, not a guess.  The
+  vectors pin what the shipped configs run: ReLU, the segment max, fp32.  The other
+  activations and aggregations of the reference's table, and the library's FP16
+  arithmetic, are arguments of the same functions, so they share that structure.
 
 What remains a definition rather than a verified fact: Open3D 0.7's
 ``voxel_down_sample`` (binary package, source absent) - see oracle/graph.py.

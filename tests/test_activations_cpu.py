@@ -1,10 +1,9 @@
 """Every activation of the reference's table (gnn.py:24-32): ReLU, ReLU6, LeakyReLU, ELU, Sigmoid, Tanh and NONE.
 
-The CPU oracle package implements ReLU, the activation of every shipped config, and stays as it is: the ReLU goldens
-pin its structure (concat order, scopes, is_logits handling).  ``activation_oracle()`` runs that same oracle with the
-other activations, defined below from TF 1.15's documented behaviour (TF cannot run here and no shipped checkpoint was
-trained with them), by substituting its two MLP functions.  The GPU tests compare the kernels against it."""
-import contextlib
+The oracle (oracle/gnn.py) takes the activation from each ``*_activation_type`` of the config.  Its structure (concat
+order, scopes, is_logits handling) is pinned by the ReLU goldens; the other activations are defined there from TF
+1.15's documented behaviour (TF cannot run here and no shipped checkpoint was trained with them).  The GPU tests
+compare the kernels against it."""
 import copy
 import os
 import re
@@ -13,77 +12,9 @@ import numpy as np
 import pytest
 
 from oracle import gnn as ognn
+from oracle.gnn import ACTIVATIONS, NAMES, activate
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NAMES = ['NONE', 'ReLU', 'ReLU6', 'LeakyReLU', 'ELU', 'Sigmoid', 'Tanh']
-
-
-def _elu(x):
-    with np.errstate(over='ignore'):
-        return np.where(x > 0, x, np.exp(np.minimum(x, 0)) - x.dtype.type(1))
-
-
-def _sigmoid(x):
-    with np.errstate(over='ignore'):
-        return x.dtype.type(1) / (x.dtype.type(1) + np.exp(-x))
-
-
-# tf.nn.relu, relu6, leaky_relu(alpha=0.01) (gnn.py:28), elu (exp(x) - 1 below zero), sigmoid, tanh; None = linear
-ACTIVATIONS = {
-    'ReLU': lambda x: np.maximum(x, x.dtype.type(0)),
-    'ReLU6': lambda x: np.minimum(np.maximum(x, x.dtype.type(0)), x.dtype.type(6)),
-    'LeakyReLU': lambda x: np.where(x > 0, x, x.dtype.type(0.01) * x),
-    'ELU': _elu,
-    'NONE': None,
-    'Sigmoid': _sigmoid,
-    'Tanh': np.tanh,
-}
-
-
-def activate(name, x):
-    fn = ACTIVATIONS[name]
-    return x if fn is None else fn(x).astype(x.dtype, copy=False)
-
-
-def _fc(x, scope, act):
-    w, b = scope.next_fc()
-    assert x.shape[1] == w.shape[0], (x.shape, w.shape, scope.prefix)
-    return activate(act, x @ w.astype(x.dtype) + b.astype(x.dtype)[None, :])
-
-
-def _mlp(features, scope, Ks=(64, 32, 64), is_logits=False, normalization_type='NONE', activation_type='ReLU'):
-    """oracle.gnn.multi_layer_neural_network_fn with any activation (gnn.py:86-104)."""
-    assert normalization_type == 'NONE'
-    for i in range(len(Ks)):
-        last = i == len(Ks) - 1
-        features = _fc(features, scope, 'NONE' if (is_logits and last) else activation_type)
-        assert features.shape[1] == Ks[i]
-    return features
-
-
-def _fc_fn(sv, scope, Ks=(64, 32, 64), num_classes=4, is_logits=False, num_layer=4, normalization_type='NONE',
-           activation_type='ReLU'):
-    """oracle.gnn.multi_layer_fc_fn with any activation (gnn.py:34-84)."""
-    assert normalization_type == 'NONE' and len(Ks) == num_layer - 1
-    features = sv
-    for _ in range(num_layer - 1):
-        features = _fc(features, scope, activation_type)
-    features = _fc(features, scope, 'NONE' if is_logits else activation_type)
-    assert features.shape[1] == num_classes
-    return features
-
-
-@contextlib.contextmanager
-def activation_oracle():
-    """The oracle package with every activation of the table (its layer functions look these names up at call time)."""
-    saved = ognn.multi_layer_neural_network_fn, ognn.multi_layer_fc_fn
-    ognn.multi_layer_neural_network_fn, ognn.multi_layer_fc_fn = _mlp, _fc_fn
-    try:
-        yield ognn
-    finally:
-        ognn.multi_layer_neural_network_fn, ognn.multi_layer_fc_fn = saved
-
-
 ACTIVATION_KEYS = ('point_MLP_activation_type', 'output_MLP_activation_type', 'edge_MLP_activation_type',
                    'update_MLP_activation_type', 'auto_offset_MLP_feature_activation_type', 'activation_type')
 
@@ -125,9 +56,8 @@ def test_monotone_non_decreasing(name):
 def test_activation_oracle_with_relu_reproduces_goldens(name, request):
     g = request.getfixturevalue(name)
     coords, keypoints, edges = g.graph_tuple()
-    with activation_oracle() as o:
-        logits, boxes = o.predict(g.weights, g.layer_configs, g.config['num_classes'], 7, g.graph['intensity'],
-                                  coords, keypoints, edges)
+    logits, boxes = ognn.predict(g.weights, g.layer_configs, g.config['num_classes'], 7, g.graph['intensity'], coords,
+                                 keypoints, edges)
     assert np.abs(logits - g.gnn['logits']).max() < 2e-5
     assert np.abs(boxes - g.gnn['boxes']).max() < 2e-5
 
@@ -138,13 +68,12 @@ def test_activation_oracle_runs_every_activation():
     g = load_golden('car_auto_T1_train')
     coords, keypoints, edges = g.graph_tuple()
     outs = {}
-    with activation_oracle() as o:
-        for name in NAMES:
-            lcs = with_activation(g.layer_configs, name)
-            logits, boxes = o.predict(g.weights, lcs, g.config['num_classes'], 7, g.graph['intensity'], coords,
-                                      keypoints, edges)
-            assert logits.dtype == np.float32 and np.isfinite(logits).all() and np.isfinite(boxes).all(), name
-            outs[name] = logits
+    for name in NAMES:
+        lcs = with_activation(g.layer_configs, name)
+        logits, boxes = ognn.predict(g.weights, lcs, g.config['num_classes'], 7, g.graph['intensity'], coords,
+                                     keypoints, edges)
+        assert logits.dtype == np.float32 and np.isfinite(logits).all() and np.isfinite(boxes).all(), name
+        outs[name] = logits
     assert np.abs(outs['ReLU'] - g.gnn['logits']).max() < 2e-5
     for a in NAMES:
         if a not in ('ReLU', 'ReLU6'):    # this model's ReLU features stay below 6

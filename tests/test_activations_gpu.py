@@ -1,5 +1,5 @@
 """Every activation of the reference's table through the dense, pooling, GNN edge and predictor layers and the whole
-model, at both precisions, against the activation oracle of test_activations_cpu."""
+model, at both precisions, against the oracle (oracle/gnn.py) with each activation."""
 import ctypes
 from functools import partial
 
@@ -7,7 +7,9 @@ import numpy as np
 import pytest
 import torch
 
-from test_activations_cpu import NAMES, activate, activation_oracle, with_activation
+from oracle import gnn as ognn
+from oracle.gnn import NAMES, activate
+from test_activations_cpu import with_activation
 
 pytestmark = pytest.mark.gpu
 FLT_MIN = np.finfo(np.float32).min
@@ -93,7 +95,6 @@ def _pool_case(rng, dims, e, nv=900, nk=400):
 
 
 def _mlp_max(name, h, ws, bs, dst, nk):
-    from oracle import gnn as ognn
     for w, b in zip(ws, bs):
         h = activate(name, h @ w + b)
     return ognn.graph_scatter_max_fn(h, dst, nk)
@@ -165,9 +166,8 @@ def test_predictor_fast_path(name, precision):
                 weights[base + '/weights'] = (rng.standard_normal((a, b)) / np.sqrt(a)).astype(np.float32)
                 weights[base + '/biases'] = (rng.standard_normal(b) * 0.1).astype(np.float32)
         x = rng.standard_normal((700, d)).astype(np.float32)
-        with activation_oracle() as o:
-            want_l, want_b = o.class_aware_predictor(weights, '', x, c, box, activation_type=name,
-                                                     cls_Ks=(h,), loc_Ks=(h, h))
+        want_l, want_b = ognn.class_aware_predictor(weights, '', x, c, box, activation_type=name, cls_Ks=(h,),
+                                                    loc_Ks=(h, h))
         pointgnn_b200.set_precision(precision)
         try:
             pred = gnn.ClassAwarePredictor(partial(gnn.multi_layer_fc_fn, Ks=(h,), num_layer=2),
@@ -195,13 +195,6 @@ def _model(g, layer_configs, precision):
         pointgnn_b200.set_precision('fp32')
 
 
-def _oracle(g, layer_configs):
-    coords, keypoints, edges = g.graph_tuple()
-    with activation_oracle() as o:
-        return o.predict(g.weights, layer_configs, g.config['num_classes'], 7, g.graph['intensity'], coords,
-                         keypoints, edges)
-
-
 MIXED = {'edge_MLP_activation_type': 'ELU', 'update_MLP_activation_type': 'Tanh',
          'auto_offset_MLP_feature_activation_type': 'LeakyReLU', 'point_MLP_activation_type': 'Sigmoid',
          'output_MLP_activation_type': 'ReLU', 'activation_type': 'ReLU6'}
@@ -215,7 +208,9 @@ def test_whole_model(model, name, precision, request):
     _prec(precision)
     g = request.getfixturevalue(model)
     lcs = with_activation(g.layer_configs, per_key=MIXED) if name == 'mixed' else with_activation(g.layer_configs, name)
-    want_l, want_b = _oracle(g, lcs)
+    coords, keypoints, edges = g.graph_tuple()
+    want_l, want_b = ognn.predict(g.weights, lcs, g.config['num_classes'], 7, g.graph['intensity'], coords, keypoints,
+                                  edges)
     logits, boxes = _model(g, lcs, precision)
     err = max(_close(logits, want_l, name, True), _close(boxes, want_b, name, True))
     print('max |err| %s %s %s: %.3g' % (model, name, precision, err))

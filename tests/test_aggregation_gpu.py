@@ -1,6 +1,6 @@
 """The sum and the mean of the reference's aggregation table (gnn.py:111-119) through the fused edge layers: the GNN
 edge layer, the car pooling chain and the ped pooling split (256 -> 512: a store launch, then the row launches), at
-fp32, BF16x3 and FP16, against the aggregation oracles of test_aggregation_cpu.  No shipped checkpoint was trained
+fp32, BF16x3 and FP16, against the oracle (oracle/gnn.py) with each aggregation.  No shipped checkpoint was trained
 with a sum or a mean: the shipped weights run with the aggregation swapped.
 
 Bounds.  fp32 and BF16x3: max|got - want| <= 1e-3 max(1, max|want|) against float64, the bound of the max's tests in
@@ -13,9 +13,9 @@ import numpy as np
 import pytest
 import torch
 
-from test_activations_cpu import NAMES, activate
-from test_aggregation_cpu import (_scope_weights, aggregation_oracle, f16_aggregation_oracle, f16_gnn_edge,
-                                  f16_pool_edge, segment_reduce)
+from oracle import gnn as ognn
+from oracle.gnn import NAMES, activate, segment_reduce
+from test_aggregation_cpu import _scope_weights
 
 pytestmark = pytest.mark.gpu
 PRECISIONS = ['fp32', 'bf16x3', 'fp16']
@@ -79,9 +79,11 @@ def _reference(mode, inputs, src, dst, num_dst, ws, bs, aggregation, precision, 
     feat, xyz_src, xyz_dst, dst_index = inputs
     drow = dst if dst_index is None else dst_index[dst]
     if precision == 'fp16' and mode == 1:
-        return f16_gnn_edge(feat, xyz_src, xyz_dst, src, dst, num_dst, ws, bs, act, aggregation)
+        return ognn.gnn_edge_layer(feat, xyz_src, xyz_dst, src, dst, num_dst, ws, bs, act=act, aggregation=aggregation,
+                                   fp16=True)
     if precision == 'fp16':
-        return f16_pool_edge(feat, xyz_src, xyz_dst[dst_index], src, dst, num_dst, ws, bs, act, aggregation)
+        return ognn.pool_edge_layer(feat, xyz_src, xyz_dst[dst_index], src, dst, num_dst, ws, bs, act=act,
+                                    aggregation=aggregation, fp16=True)
     h = np.concatenate([feat[src], xyz_src[src] - xyz_dst[drow]], axis=1).astype(np.float64)
     return segment_reduce(_mlp64(h, ws, bs, act), dst, num_dst, aggregation)
 
@@ -270,12 +272,7 @@ def test_whole_model(model, aggregation, precision, request):
     g = request.getfixturevalue(model)
     coords, keypoints, edges = g.graph_tuple()
     args = (g.weights, g.layer_configs, g.config['num_classes'], 7, g.graph['intensity'], coords, keypoints, edges)
-    if precision == 'fp16':
-        with f16_aggregation_oracle(aggregation) as o:
-            want_l, want_b = o.predict(*args)
-    else:
-        with aggregation_oracle(aggregation) as o:
-            want_l, want_b = o.predict(*args)
+    want_l, want_b = ognn.predict(*args, aggregation=aggregation, fp16=precision == 'fp16')
     logits, boxes = _predict(g, getattr(gnn, 'graph_scatter_%s_fn' % aggregation), precision)
     if precision == 'fp16':
         el, eb = np.abs(logits - want_l).max(), np.abs(boxes - want_b).max()

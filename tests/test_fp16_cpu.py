@@ -5,8 +5,8 @@ import tempfile
 import numpy as np
 import pytest
 
-import fp16_oracle
 from conftest import ALL_CHECKPOINTS, load_golden
+from oracle import gnn as ognn
 
 LOGIT_TOL, BOX_TOL = 2e-2, 1e-2
 
@@ -16,8 +16,8 @@ def test_oracle_within_bounds_of_fp32_golden(name):
     """The FP16 arithmetic of every shipped checkpoint stays within the bounds the GPU tests hold the kernels to."""
     g = load_golden(name)
     coords, kp, edges = g.graph_tuple()
-    logits, boxes = fp16_oracle.predict(g.weights, g.layer_configs, g.config['num_classes'], 7, g.graph['intensity'],
-                                        coords, kp, edges)
+    logits, boxes = ognn.predict(g.weights, g.layer_configs, g.config['num_classes'], 7, g.graph['intensity'], coords,
+                                 kp, edges, fp16=True)
     assert logits.shape == g.gnn['logits'].shape and boxes.shape == g.gnn['boxes'].shape
     dl, db = np.abs(logits - g.gnn['logits']).max(), np.abs(boxes - g.gnn['boxes']).max()
     assert dl <= LOGIT_TOL and db <= BOX_TOL, (name, dl, db)
@@ -27,16 +27,16 @@ def test_oracle_within_bounds_of_fp32_golden(name):
 
 def test_oracle_rounding():
     x = np.array([[1.0 + 2.0 ** -12, 70000.0, -1e9, 3.0]], np.float32)
-    r = fp16_oracle.f16(x)
+    r = ognn.f16(x)
     assert r[0, 0] == 1.0 and r[0, 1] == 65504.0 and r[0, 2] == -65504.0 and r[0, 3] == 3.0
     # exact products and sums of the rounded operands, rounded once to fp32
     w = np.full((4, 1), 1.0, np.float32)
-    assert fp16_oracle.tc_gemm(x, w)[0, 0] == np.float32(1.0 + 65504.0 - 65504.0 + 3.0)
-    assert fp16_oracle.fc_uses_tc(300, 64) and not fp16_oracle.fc_uses_tc(64, 7) and not fp16_oracle.fc_uses_tc(32, 64)
+    assert ognn.tc_gemm(x, w)[0, 0] == np.float32(1.0 + 65504.0 - 65504.0 + 3.0)
+    assert ognn.fc_uses_tc(300, 64) and not ognn.fc_uses_tc(64, 7) and not ognn.fc_uses_tc(32, 64)
     # the car GNN layer (303 -> 300 -> 300): W resident in 152-wide column groups, 92 KB of FP16 each
-    assert fp16_oracle.gnn_uses_tc([303, 300, 300]) and not fp16_oracle.gnn_uses_tc([303, 300, 300, 300])
-    assert fp16_oracle.pool_uses_tc([4, 32, 64, 128, 300], 'ReLU')
-    assert not fp16_oracle.pool_uses_tc([4, 32, 64, 128, 300], 'Tanh')
+    assert ognn.gnn_uses_tc([303, 300, 300]) and not ognn.gnn_uses_tc([303, 300, 300, 300])
+    assert ognn.pool_uses_tc([4, 32, 64, 128, 300], 'ReLU')
+    assert not ognn.pool_uses_tc([4, 32, 64, 128, 300], 'Tanh')
 
 
 def test_set_precision_fp16():

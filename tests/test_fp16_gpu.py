@@ -1,6 +1,7 @@
-"""The FP16 precision (code 2, ``set_precision('fp16')``) on the GPU against the FP16 oracle (fp16_oracle): the dense
-kernel, the pooling and GNN edge layers (prepared and per call, car and ped), every non-ReLU activation of the GNN
-edge layer, the whole model on all seven checkpoints, saturation at FP16's range, and the rejected precision codes.
+"""The FP16 precision (code 2, ``set_precision('fp16')``) on the GPU against the FP16 oracle (oracle/gnn.py with
+``fp16=True``): the dense kernel, the pooling and GNN edge layers (prepared and per call, car and ped), every non-ReLU
+activation of the GNN edge layer, the whole model on all seven checkpoints, saturation at FP16's range, and the
+rejected precision codes.
 
 Bounds.  Dense layers: 1e-4, both sides round the same operands and only the fp32 summation order differs.  Edge
 layers: 1e-3 of the output's scale (max(1, max |want|)), since an fp32 pre-rounding value that differs in its last
@@ -13,8 +14,8 @@ import numpy as np
 import pytest
 import torch
 
-import fp16_oracle
 from conftest import ALL_CHECKPOINTS, load_golden
+from oracle import gnn as ognn
 
 pytestmark = pytest.mark.gpu
 FLT_MIN = np.finfo(np.float32).min
@@ -55,7 +56,8 @@ def test_fully_connected_vs_oracle():
         r = rng.standard_normal((m, n)).astype(np.float32)
         for relu in (True, False):
             for res in (None, r):
-                want = fp16_oracle.fc(x, w, b, 'ReLU' if relu else 'NONE', res)
+                want = ognn.dense(x, w, b, 'ReLU' if relu else 'NONE', fp16=True)
+                want = want if res is None else want + res
                 got = lib.fully_connected(_cuda(x), _cuda(w), _cuda(b), relu, residual=None if res is None else _cuda(res),
                                           precision=FP16).cpu().numpy()
                 assert got.shape == want.shape and np.abs(got - want).max() <= 1e-4, (m, k, n, relu)
@@ -93,7 +95,7 @@ def test_pooling_edge_layer(name, prepared):
     kp = keypoints[0][:, 0]
     ed = edges[0]
     feats = g.graph['intensity'].astype(np.float32)
-    want = fp16_oracle.pool_edge_max(feats, coords[0], coords[0][kp], ed[:, 0], ed[:, 1], len(kp), ws, bs)
+    want = ognn.pool_edge_layer(feats, coords[0], coords[0][kp], ed[:, 0], ed[:, 1], len(kp), ws, bs, fp16=True)
     seg0 = lib.tc_launch_count(0)
     got = _run_edge(lib, lib.PG_LAYER_EDGE_POOL, lib.PG_EDGE_POOL, ws, bs, feats, coords[0], coords[0], kp,
                     ed[:, 0], ed[:, 1], len(kp), prepared)
@@ -115,7 +117,7 @@ def test_gnn_edge_layer(name, prepared):
     xyz = coords[1].astype(np.float32)
     xyz_dst = xyz + (rng.standard_normal(xyz.shape) * 0.05).astype(np.float32)    # an auto offset
     ed = edges[1]
-    want = fp16_oracle.gnn_edge_max(feats, xyz, xyz_dst, ed[:, 0], ed[:, 1], k, ws, bs)
+    want = ognn.gnn_edge_layer(feats, xyz, xyz_dst, ed[:, 0], ed[:, 1], k, ws, bs, fp16=True)
     seg0 = lib.tc_launch_count(0)
     got = _run_edge(lib, lib.PG_LAYER_EDGE_GNN, lib.PG_EDGE_GNN, ws, bs, feats, xyz, xyz_dst, None, ed[:, 0], ed[:, 1],
                     k, prepared)
@@ -142,7 +144,7 @@ def test_gnn_edge_layer_activations(name):
         bs = [(rng.standard_normal(n) * 0.1).astype(np.float32), (rng.standard_normal(n) * 0.1).astype(np.float32)]
         if neg:
             bs[1] = bs[1] - 20.0
-        want = fp16_oracle.gnn_edge_max(feat, xyz, xyz, src, dst, nv, ws, bs, act=name)
+        want = ognn.gnn_edge_layer(feat, xyz, xyz, src, dst, nv, ws, bs, act=name, fp16=True)
         act = gnn.activation_fn_dict[name]
         for prepared in (False, True):
             got = _run_edge(lib, lib.PG_LAYER_EDGE_GNN, lib.PG_EDGE_GNN, ws, bs, feat, xyz, xyz, None, src, dst, nv,
@@ -172,8 +174,8 @@ def test_predict_every_checkpoint(name):
     lib = _lib()
     g = load_golden(name)
     coords, keypoints, edges = g.graph_tuple()
-    want_l, want_b = fp16_oracle.predict(g.weights, g.layer_configs, g.config['num_classes'], 7, g.graph['intensity'],
-                                         coords, keypoints, edges)
+    want_l, want_b = ognn.predict(g.weights, g.layer_configs, g.config['num_classes'], 7, g.graph['intensity'], coords,
+                                  keypoints, edges, fp16=True)
     tc0 = (lib.tc_launch_count(0), lib.tc_launch_count(1))
     logits, boxes, _ = _predict(g, 'fp16')
     assert lib.tc_launch_count(0) > tc0[0] and lib.tc_launch_count(1) > tc0[1]
@@ -211,7 +213,7 @@ def test_saturation():
     w[5, :] = 7e4
     w[9, ::3] = -1e9
     b = rng.standard_normal(n).astype(np.float32)
-    want = fp16_oracle.fc(x, w, b, 'NONE')
+    want = ognn.dense(x, w, b, 'NONE', fp16=True)
     got = lib.fully_connected(_cuda(x), _cuda(w), _cuda(b), False, precision=FP16).cpu().numpy()
     assert np.isfinite(got).all() and np.isfinite(want).all()
     assert np.abs(want).max() > 1e9                  # the clamped values really are in play
@@ -226,7 +228,7 @@ def test_saturation():
     ws = [(rng.standard_normal((63, 64)) * 0.05).astype(np.float32), (rng.standard_normal((64, 64)) * 0.05).astype(np.float32)]
     ws[0][7, :] = 3.0
     bs = [np.zeros(64, np.float32), np.zeros(64, np.float32)]
-    want = fp16_oracle.gnn_edge_max(feat, xyz, xyz, src, dst, 50, ws, bs)
+    want = ognn.gnn_edge_layer(feat, xyz, xyz, src, dst, 50, ws, bs, fp16=True)
     got = _run_edge(lib, lib.PG_LAYER_EDGE_GNN, lib.PG_EDGE_GNN, ws, bs, feat, xyz, xyz, None, src, dst, 50, False)
     _close(got, want, 'edge saturation')
 

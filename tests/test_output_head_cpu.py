@@ -5,9 +5,8 @@ NumPy restatements, which the GPU tests (test_output_head_gpu.py) compare agains
   * ``canonical_decode``: classaware_all_class_box_canonical_decoding, float32 in the reference's operation order.  It
     reproduces tests/golden/box_canonical.npz (made from the reference's own function, tools/make_golden.py
     box_canonical) bit for bit.
-  * ``separated_predictor``: ClassAwareSeparatedPredictor.apply_regular with the registry's heads (models.py:70-74) and
-    any activation of the table, on real ``np.split`` slices.  No saved graph of this predictor exists, so this
-    restatement of gnn.py:177-209 is its oracle.
+  * The separated predictor is oracle/gnn.py's ``class_aware_predictor(..., separated=True)``, on real ``np.split``
+    slices.  No saved graph of this predictor exists, so that restatement of gnn.py:177-209 is its oracle.
   * ``separated_checkpoint``: the car_auto_T3 weights with each loc head's first weight cut to its slice's rows, the
     checkpoint the end-to-end tests run.
 """
@@ -21,7 +20,6 @@ import pytest
 from conftest import GOLDEN
 from oracle import gnn as ognn
 from oracle import postprocess as opp
-from test_activations_cpu import _fc_fn
 
 CANONICAL = 'classaware_all_class_box_canonical_encoding'
 THREE_ARGUMENT_CODECS = ('direct_encoding', 'center_box_encoding', 'voxelnet_box_encoding',
@@ -62,22 +60,6 @@ def canonical_decode_all(box_encodings, points_xyz, label_map):
         labels = np.full((k, 1), cls)
         out[:, cls] = canonical_decode(labels, points_xyz, box_encodings[:, cls:cls + 1], label_map)[:, 0]
     return out
-
-
-def separated_predictor(weights, scope_name, features, num_classes, box_encoding_len, activation_type='ReLU'):
-    """ClassAwareSeparatedPredictor.apply_regular (gnn.py:177-209) with cls_fn / loc_fn of models.py:70-74."""
-    features = np.asarray(features, dtype=np.float32)
-    pred = ognn._Scope(weights, scope_name).sub('predictor')
-    logits = _fc_fn(features, pred.sub('cls'), Ks=(64,), num_layer=2, num_classes=num_classes, is_logits=True,
-                    normalization_type='NONE', activation_type=activation_type)
-    splits = np.split(features, num_classes, axis=-1)
-    boxes = []
-    for class_idx in range(num_classes):
-        b = _fc_fn(splits[class_idx], pred.sub('loc').sub('cls_%d' % class_idx), Ks=(64, 64), num_layer=3,
-                   num_classes=box_encoding_len, is_logits=True, normalization_type='NONE',
-                   activation_type=activation_type)
-        boxes.append(b[:, None, :])
-    return logits, np.concatenate(boxes, axis=1)
 
 
 def loc_first_layer(scope_name, c):
@@ -265,7 +247,7 @@ def test_separated_restatement_equals_shared_predictor_on_expanded_weights():
     config, weights = separated_checkpoint()
     rng = np.random.default_rng(3)
     feats = rng.standard_normal((50, 300)).astype(np.float32)
-    logits, boxes = separated_predictor(weights, 'output', feats, 4, 7)
+    logits, boxes = ognn.class_aware_predictor(weights, 'output', feats, 4, 7, separated=True)
     l2, b2 = ognn.class_aware_predictor(expanded_weights(weights, 'output', 4), 'output', feats, 4, 7)
     assert np.allclose(logits, l2, atol=1e-5) and np.allclose(boxes, b2, atol=1e-5)
     assert weights[loc_first_layer('output', 3)].shape == (75, 64)

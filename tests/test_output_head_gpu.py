@@ -1,8 +1,9 @@
-"""The class-aware separated predictor and the canonical box codec on the GPU, against the NumPy restatements of
-test_output_head_cpu.py (pinned there to the reference's own decoder through tests/golden/box_canonical.npz).
+"""The class-aware separated predictor and the canonical box codec on the GPU, against the oracle's separated
+predictor (oracle/gnn.py) and the canonical decoder of test_output_head_cpu.py (pinned there to the reference's own
+decoder through tests/golden/box_canonical.npz).
 
 Tolerances.  Separated head: fp32 1e-4 and BF16x3 1e-3 of the restatement, FP16 1e-3 of the FP16 oracle
-(tests/fp16_oracle.py) on the zero-padded loc weights, all relative to max(1, |want|).  Whole model: 1e-3 at BF16x3,
+(oracle/gnn.py, fp16=True) on the zero-padded loc weights, all relative to max(1, |want|).  Whole model: 1e-3 at BF16x3,
 the FP16 suite's 8e-3 / 4e-3 at FP16.  Canonical decode: x, y, z and yaw bit for bit (cos / sin are NumPy's float32
 routine, restated); the sizes exp(e) l within 4 ulp, because exp is CUDA's expf (within 2 ulp of exp), as in the
 all-class rule, whose sizes they equal byte for byte.  NMS: as test_post_stage_gpu.py
@@ -16,15 +17,13 @@ import numpy as np
 import pytest
 import torch
 
-import fp16_oracle
 from conftest import GOLDEN, Golden
 from oracle import gnn as ognn
 from oracle import graph as ograph
 from oracle import kitti as ok
 from oracle import postprocess as opp
-from test_activations_cpu import NAMES, activation_oracle
-from test_output_head_cpu import (CANONICAL, canonical_decode_all, expanded_weights, separated_checkpoint,
-                                  separated_predictor)
+from oracle.gnn import NAMES
+from test_output_head_cpu import CANONICAL, canonical_decode_all, expanded_weights, separated_checkpoint
 from test_run_batched_gpu import _tree
 
 pytestmark = pytest.mark.gpu
@@ -74,10 +73,9 @@ def _run_head(weights, features, c, precision, act='ReLU'):
 
 def _want(weights, features, c, precision, act):
     if precision == 'fp16':
-        return fp16_oracle.class_aware_predictor(expanded_weights(weights, 'output', c), 'output', features, c, BOX,
-                                                 activation_type=act)
-    with activation_oracle():
-        return separated_predictor(weights, 'output', features, c, BOX, act)
+        return ognn.class_aware_predictor(expanded_weights(weights, 'output', c), 'output', features, c, BOX,
+                                          activation_type=act, fp16=True)
+    return ognn.class_aware_predictor(weights, 'output', features, c, BOX, activation_type=act, separated=True)
 
 
 def _check(got, want, precision, what):
@@ -145,17 +143,6 @@ def test_separated_head_indivisible_width_is_an_error_not_a_launch():
 # ---------------------------------------------------------------------------------------------
 # whole model: car_auto_T3 with the separated predictor
 # ---------------------------------------------------------------------------------------------
-def _separated_oracle(config, weights, intensity, coords, keypoints, edges):
-    """fp32: oracle/gnn.py's layers up to the predictor (their variables are the shipped ones), then the
-    restatement on the last layer's features."""
-    shared = copy.deepcopy(config['model_kwargs']['layer_configs'])
-    shared[-1]['type'] = 'classaware_predictor'
-    c = config['num_classes']
-    feats = ognn.predict(expanded_weights(weights, 'output', c), shared, c, BOX, intensity, coords, keypoints, edges,
-                         return_features=True)[2][-1]
-    return separated_predictor(weights, 'output', feats, c, BOX)
-
-
 @pytest.mark.parametrize('precision', ['bf16x3', 'fp16'])
 def test_separated_car_model_predict(precision):
     import pointgnn_b200
@@ -171,11 +158,12 @@ def test_separated_car_model_predict(precision):
     if precision == 'fp16':
         shared = copy.deepcopy(config['model_kwargs']['layer_configs'])
         shared[-1]['type'] = 'classaware_predictor'
-        want_l, want_b = fp16_oracle.predict(expanded_weights(weights, 'output', c), shared, c, BOX, intensity,
-                                             coords, keypoints, edges)
+        want_l, want_b = ognn.predict(expanded_weights(weights, 'output', c), shared, c, BOX, intensity, coords,
+                                      keypoints, edges, fp16=True)
         tol_l, tol_b = 8e-3, 4e-3
     else:
-        want_l, want_b = _separated_oracle(config, weights, intensity, coords, keypoints, edges)
+        want_l, want_b = ognn.predict(weights, config['model_kwargs']['layer_configs'], c, BOX, intensity, coords,
+                                      keypoints, edges)
         tol_l = tol_b = 1e-3
     pointgnn_b200.set_precision(precision)
     try:
@@ -320,7 +308,8 @@ def _oracle_text(root, name, config, weights):
     calib = ok.parse_calib(os.path.join(root, 'calib/testing/calib', name + '.txt'))
     xyz, attr = ok.cam_points_in_image(velo, calib, 1242, 375, None)
     coords, kp, edges = ograph.gen_multi_level_local_graph_v3(xyz, **config['runtime_graph_gen_kwargs'])
-    logits, boxes = _separated_oracle(config, weights, attr, coords, kp, edges)
+    logits, boxes = ognn.predict(weights, config['model_kwargs']['layer_configs'], config['num_classes'], BOX, attr,
+                                 coords, kp, edges)
     probs = ognn.postprocess(logits)
     last = coords[config['model_kwargs']['layer_configs'][-1]['graph_level'] + 1]
     dec = canonical_decode_all(boxes, last, opp.LABEL_MAPS[config['label_method']])

@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 import torch
 
-import fp16_oracle
+from oracle import gnn as ognn
 
 pytestmark = pytest.mark.gpu
 FMIN = np.finfo(np.float32).min
@@ -35,7 +35,7 @@ def _act(name, x):
 
 def _want(f, x, src, dst, nd, ws, bs, prec, act):
     if prec == FP16:
-        return fp16_oracle.gnn_edge_max(f, x, x, src, dst, nd, ws, bs, act=act)
+        return ognn.gnn_edge_layer(f, x, x, src, dst, nd, ws, bs, act=act, fp16=True)
     out = np.full((nd, ws[1].shape[1]), FMIN, np.float32)
     e0 = np.concatenate([f[src], x[src] - x[dst]], axis=1)
     np.maximum.at(out, dst, _act(act, _act(act, e0 @ ws[0] + bs[0]) @ ws[1] + bs[1]).astype(np.float32))

@@ -30,9 +30,8 @@ def split(a, dt):
     return hi, lo
 
 
-def make_fc(mode):
-    def _fc(x, scope, relu):
-        w, b = scope.next_fc()
+def make_dense(mode):
+    def _dense(x, w, b, act, tc=False):
         if mode == 'fp32' or w.shape[0] < 32:
             y = x @ w.astype(x.dtype) + b.astype(x.dtype)[None, :]
         else:
@@ -57,30 +56,28 @@ def make_fc(mode):
             else:
                 raise KeyError(mode)
             y = (y + b.astype(np.float64)[None, :]).astype(np.float32)
-        if relu:
-            np.maximum(y, 0, out=y)
-        return y
-    return _fc
+        return ognn.activate(act, y)
+    return _dense
 
 
 def main():
-    orig = ognn._fc
+    orig = ognn._dense
     for name in ('car_auto_T3_train', 'ped_cyl_auto_T3_trainval'):
         g = load_golden(name)
         coords, kp, edges = g.graph_tuple()
         inten = g.graph['intensity']
         args = (g.weights, g.layer_configs, g.config['num_classes'], 7, inten, coords, kp, edges)
-        ognn._fc = orig
+        ognn._dense = orig
         l64, b64 = ognn.predict(*args, dtype=np.float64)
         l32, b32 = ognn.predict(*args)
         print('%s: |logit| max %.2f, |box| max %.2f; fp32 vs fp64: %.2e / %.2e' % (
             name, np.abs(l32).max(), np.abs(b32).max(), np.abs(l32 - l64).max(), np.abs(b32 - b64).max()))
         for mode in ('bf16x3', 'fp16x3', 'fp16x2a', 'fp16x1', 'tf32x1', 'bf16x1'):
-            ognn._fc = make_fc(mode)
+            ognn._dense = make_dense(mode)
             l, b = ognn.predict(*args)
             print('   %-8s max|dlogit| %.2e  max|dbox| %.2e   (vs fp32 oracle)' % (
                 mode, np.abs(l - l32).max(), np.abs(b - b32).max()))
-    ognn._fc = orig
+    ognn._dense = orig
 
 
 if __name__ == '__main__':
